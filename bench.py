@@ -1,17 +1,18 @@
 """bench.py -- headline benchmark: sampled trajectories / second for a full ``sample()`` call.
 
-Workload (BASELINE.json configs[1], SURVEY 8d "cfg2"): JannerUNet1d(in 14, model_dim 32, dim_mult [1,2,2,2], k=5),
+Workload (cleandiffuser_b200/workloads.py::cfg2, SURVEY 8d "cfg2"): JannerUNet1d(in 14, model_dim 32, dim_mult [1,2,2,2], k=5),
 H=32, d=14, DiscreteDiffusionSDE(predict_noise=False, 100 diffusion steps, cosine), DDPM solver with 100 sampling
 steps, temperature 0.5, fix_mask on the first observation, batch 4096 candidate trajectories PER GPU (weak scaling),
 synthetic weights (seed 0) / inputs (seed 1) / noise (seed 2 + rank).  The workload definitions live in
 ``cleandiffuser_b200/workloads.py`` and are the ones the full-size parity tests run (tests/test_baseline_configs_gpu.py).
 
-Math mode: ``tf32`` (the library default): tcgen05 kind::tf32 over fp32 activations and weights, fp32 accumulate -- the
+Math mode: ``tf32`` (the library default): wgmma .tf32 over fp32 activations and weights, fp32 accumulate -- the
 arithmetic of the reference's own GPU path (cuDNN TF32 convs); ``--math bf16`` / ``--math fp32`` select the other programs.
 
 One "step" = one complete ``sample()`` call (initial noise, 100 reverse iterations, final all-gather when N > 1).
 
   python bench.py --gpus 1 --steps 5 --warmup 3              # this framework (CUDA engine through the C ABI)
+  python bench.py --steps 5 --warmup 3 --dump-outputs DIR    # ... and write the last timed step's samples to DIR/x0.npy
   python bench.py --impl reference --steps 2 --warmup 1      # CPU arm: the reference's algorithm (oracle port) on host cores
   torchrun ... bench.py --gpus N ...                         # one rank per GPU, NCCL
 
@@ -20,7 +21,7 @@ Prints ONE JSON line (rank 0).  See the task contract for the keys; additionally
   cpu_baseline        the oracle port timed on the host cores on a bounded sample of the same workload
   gpu_eager_baseline  the SAME sample() on the SAME GPU through this package's PyTorch loop (CDS_BACKEND=torch: ATen / cuDNN /
                       cuBLAS kernels launched op by op from Python, TF32 convs as torch defaults) -- what the reference's own
-                      code path costs on this B200 (SURVEY 8d's "beat this" number); N = 1 only
+                      code path costs on this GPU (SURVEY 8d's "beat this" number); N = 1 only
   other_configs       short measurements of BASELINE configs 3 / 4 / 5 at their per-GPU batch on the same ranks (value is the
                       whole-job aggregate like the headline), with their tensor-roofline fraction
 """
@@ -52,7 +53,7 @@ def peaks():
         with open(path) as f:
             p = json.load(f)
         return p["hbm_gbs"], "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (HBM3)"
 
 
 def build_agent(device, seed=0):
@@ -71,18 +72,18 @@ def make_prior(batch, seed=1):
 
 def tensor_peaks():
     """(tf32 dense TFLOP/s, bf16 dense TFLOP/s, source): bf16 measured (MEASURED_PEAKS.json, sustained), tf32 = half of it (the
-    tensor pipe runs kind::tf32 at half the bf16 rate; no measured tf32 figure exists in MEASURED_PEAKS.json)"""
+    tensor cores run TF32 at half the bf16 rate; no measured tf32 figure exists in MEASURED_PEAKS.json)"""
     path = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(path):
         with open(path) as f:
             bf16 = json.load(f)["bf16_tflops_sustained"]
         return bf16 / 2, bf16, "MEASURED_PEAKS.json bf16_tflops_sustained (tf32 = half)"
-    return 1125.0, 2250.0, "fallback (B200_PROFILING.md nominal dense)"
+    return 495.0, 989.0, "H100 SXM data sheet (dense, 700 W)"
 
 
 # ------------------------------------------------------------------------------------------ clocks
 class ClockSampler:
-    """nvidia-smi sampled every 200 ms during the timed region (B200_PROFILING.md clocks line)."""
+    """nvidia-smi sampled every 100 ms during the timed region."""
 
     def __init__(self, index):
         self.index, self.rows, self.proc = index, [], None
@@ -279,12 +280,14 @@ def main():
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--batch", type=int, default=BATCH, help="trajectories per GPU (default: the BASELINE config)")
     ap.add_argument("--math", default=os.environ.get("CDS_MATH", "tf32"), choices=["tf32", "bf16", "fp32"],
-                    help="tf32 (default = the library default): tcgen05 kind::tf32 over fp32 activations; bf16: tcgen05 with bf16 "
+                    help="tf32 (default = the library default): wgmma .tf32 over fp32 activations; bf16: wgmma with bf16 "
                          "operands and activations; fp32: CUDA-core FMA")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-other-configs", action="store_true")
     ap.add_argument("--no-eager-baseline", action="store_true")
     ap.add_argument("--cpu-sample-batch", type=int, default=256, help="trajectories per step of the CPU arm (bounded sample)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step returned (the sampled trajectories, float32) as DIR/x0.npy")
     args = ap.parse_args()
 
     rank = int(os.environ.get("RANK", "0"))
@@ -293,7 +296,7 @@ def main():
     config = {"workload": WORKLOAD, "backbone": "JannerUNet1d(14,32,[1,2,2,2],k5)", "horizon": H, "dim": D,
               "solver": "ddpm", "sample_steps": S_STEPS, "batch_per_gpu": args.batch,
               "global_batch": args.batch * world, "parallelism": f"dp{world}",
-              "l2": "working set (fp32 activations + 99-slot noise tape, ~1.5 GB) exceeds the 126 MB L2; no explicit flush"}
+              "l2": "working set (fp32 activations + 99-slot noise tape, ~1.5 GB) exceeds the 50 MB L2; no explicit flush"}
 
     if args.impl == "reference":
         if rank != 0:
@@ -348,10 +351,13 @@ def main():
     kw = dict(solver="ddpm", n_samples=B, sample_steps=S_STEPS, temperature=0.5)
     torch.manual_seed(2 + rank)
 
+    last = {}
+
     def step_resident():
         x0, _ = agent.sample(prior_dev, **kw)
         if world > 1:
             dist.all_gather_into_tensor(gathered, x0)      # the one collective of the path: finished samples
+        last["x0"] = gathered if world > 1 else x0
         return x0
 
     def step_e2e():
@@ -366,7 +372,7 @@ def main():
 
     with torch.no_grad():
         log("warm-up")
-        for i in range(max(args.warmup, 3)):
+        for i in range(args.warmup):
             step_resident()
             torch.cuda.synchronize()
             log(f"warm-up step {i} done")
@@ -380,6 +386,10 @@ def main():
             runtime.STATS["loop_events"] = []
             ms = timed(step_resident, args.steps)
             row1 = len(clk.rows)
+            if args.dump_outputs and rank == 0:         # before any further call can touch the result of the last timed step
+                import numpy as np
+                os.makedirs(args.dump_outputs, exist_ok=True)
+                np.save(os.path.join(args.dump_outputs, "x0.npy"), last["x0"].float().cpu().numpy())
             extended = 0
             t_ext = time.time()
             while len(clk.rows) - row0 < 5 and time.time() - t_ext < 3.0:    # short timed regions: keep the same load running
@@ -440,26 +450,17 @@ def main():
         log(f"iteration total {iter_ms * 1e3:.1f} us (direct launches, event-bracketed)")
         share = conv_ms / iter_ms
         # the timed region replays CUDA graphs (no per-launch events possible inside): the conv kernels' time per iteration is
-        # the event-timed loop time x their share of the iteration (share from the event-bracketed direct launches above;
-        # the ncu launch list under profiles/ gives the same share)
+        # the event-timed loop time x their share of the iteration (share from the event-bracketed direct launches above)
         loop_iter_ms = loop_ms_mean / S_STEPS
         conv_ms_graph = loop_iter_ms * share
         achieved = conv_bytes / (conv_ms_graph * 1e-3) / 1e9
-        traffic, traffic_src = None, None
-        tpath = os.path.join(ROOT, "profiles", "ncu_traffic.json")
-        if os.path.exists(tpath):
-            with open(tpath) as f:
-                tj = json.load(f)
-            ent = tj.get(args.math) if isinstance(tj.get(args.math), dict) else None
-            if ent:
-                traffic, traffic_src = ent.get("conv_dram_bytes_per_launch"), ent.get("source")
         tf32_peak, bf16_peak, tsrc = tensor_peaks()
         tpeak = {"tf32": tf32_peak, "bf16": bf16_peak}.get(args.math)
         tfl = conv_flops / (conv_ms_graph * 1e-3) / 1e12
-        roofline = {"bound": "hbm", "kernel": "conv_tc_kernel / conv_ps_kernel (fused Conv1d+GroupNorm+Mish+FiLM+residual), all "
+        roofline = {"bound": "hbm", "kernel": "conv_tc_kernel (fused Conv1d+GroupNorm+Mish+FiLM+residual), all "
                                               f"{n_conv} conv launches of one reverse iteration",
                     "achieved": achieved, "peak": hbm_peak, "unit": "GB/s", "frac": achieved / hbm_peak,
-                    "peak_source": peak_src, "traffic": traffic, "traffic_source": traffic_src,
+                    "peak_source": peak_src,
                     "how": "algorithmic bytes (SURVEY 8d: fp32 in+out of every fused conv) of one iteration / (event-timed graph-replay "
                            "loop time per iteration x conv share of the iteration)",
                     "launches_per_iter": n_conv, "avg_launch_us": conv_ms_graph / max(n_conv, 1) * 1e3,
@@ -503,9 +504,9 @@ def main():
         os.close(saved_stdout)
     if rank == 0:
         line = {"metric": "sampled trajectories/sec (H=32, 100 DDPM steps)", "value": value, "unit": "trajectories/s",
-                "n_gpus": world, "steps": args.steps, "warmup": max(args.warmup, 3), "ms_per_step": ms / args.steps,
+                "n_gpus": world, "steps": args.steps, "warmup": args.warmup, "ms_per_step": ms / args.steps,
                 "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
-                "dtype": {"fp32": "f32", "tf32": "tf32 (fp32 activations and weights in HBM, tcgen05 kind::tf32, f32 accumulate)",
+                "dtype": {"fp32": "f32", "tf32": "tf32 (fp32 activations and weights in HBM, wgmma .tf32, f32 accumulate)",
                           "bf16": "bf16 operands and activations / f32 accumulate"}[args.math], "data": "synthetic",
                 "config": config, "clocks": clocks,
                 "e2e": {"value": e2e_value, "unit": "trajectories/s", "h2d_bytes_per_step": prior_host.numel() * 4,

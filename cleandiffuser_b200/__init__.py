@@ -1,7 +1,7 @@
-"""cleandiffuser_b200 -- B200-native diffusion-policy sampling engine.
+"""cleandiffuser_b200 -- H100-native diffusion-policy sampling engine.
 
 Keeps CleanDiffuser's ``diffusion`` / ``nn_diffusion`` / ``nn_condition`` plugin surfaces and
-runs ``sample()``'s reverse loop as hand-written sm_100a CUDA behind a C-ABI (``include/cds.h``).
+runs ``sample()``'s reverse loop as hand-written sm_90a CUDA behind a C-ABI (``include/cds.h``).
 """
 __version__ = "0.1.0"
 

@@ -1,4 +1,4 @@
-// libcds: C ABI (include/cds.h) over the sm_100a kernels.  Plans, validation, CUDA-graph replay.
+// libcds: C ABI (include/cds.h) over the sm_90a kernels.  Plans, validation, CUDA-graph replay.
 #include <cuda_runtime.h>
 
 #include <cstdarg>

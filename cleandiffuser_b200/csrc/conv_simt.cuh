@@ -13,7 +13,7 @@
 // (the 1x1 shortcut conv of a ResidualBlock) is accumulated on top of the finished tile.
 //
 // Algorithmic HBM bytes per launch: 4*(batch*L_in*C_in + batch*L_out*C_out*phases) (+ shortcut input, +weights
-// once per CTA column through L2).  The tcgen05 path (conv_tc.cuh) replaces the main loop; the epilogue is shared.
+// once per CTA column through L2).  The wgmma path (conv_tc.cuh) replaces the main loop; the epilogue is shared.
 #pragma once
 #include <cuda_bf16.h>
 

@@ -1,23 +1,25 @@
-// CDS_OP_CONV, tensor-core path (CDS_MATH_BF16_TC / CDS_MATH_TF32_TC): implicit-GEMM 1-D convolution on tcgen05 with the
-// UNet block post-processing fused into the TMEM epilogue.  Template parameter TF32 selects the operand type: bf16
-// activations / weights (kind::f16) or fp32 activations / weights read as TF32 (kind::tf32).  Everything about the operand
+// CDS_OP_CONV, tensor-core path (CDS_MATH_BF16_TC / CDS_MATH_TF32_TC): implicit-GEMM 1-D convolution on wgmma with the
+// UNet block post-processing fused into the epilogue.  Template parameter TF32 selects the operand type: bf16
+// activations / weights (.bf16) or fp32 activations / weights read as TF32 (.tf32).  Everything about the operand
 // tiles is expressed in BYTES: "KC" is the row width of a chunk in bf16-equivalents (row bytes / 2: 64 -> 128-byte rows,
 // SWIZZLE_128B; 32 -> 64-byte rows, SWIZZLE_64B), i.e. KC channels of bf16 or KC/2 channels of fp32, and one MMA
 // instruction always consumes 32 bytes of K (16 bf16 / 8 tf32).
 //
-//   D[128 rows x N] (fp32, TMEM) = sum over (tap, 64- or 32-channel chunk) of  A_tap[128 x KC] * W_tap[N x KC]^T
+//   D[128 rows x N] (fp32) = sum over (tap, 64- or 32-channel chunk) of  A_tap[128 x KC] * W_tap[N x KC]^T
 //
 // * rows = 128/L whole trajectories x L positions.  The im2col never exists: the A tile of tap j is ONE TMA box
-//   {KC channels, L positions, T trajectories} of the channels-last bf16 activation whose position coordinate starts at
+//   {KC channels, L positions, T trajectories} of the channels-last activation whose position coordinate starts at
 //   j - pad; positions outside [0, L) are zero-filled by the TMA unit (out-of-bound fill), which is exactly the conv's
 //   zero padding, and trajectories never bleed into each other because they are a separate tensor dimension.
-// * W_tap is a TMA box {KC, N} of the bf16 weight packed [tap][C_out][C_in]; both operands land in shared memory in the
-//   K-major SWIZZLE_128B (KC=64) / SWIZZLE_64B (KC=32) layout that tcgen05.mma consumes directly.
-// * warp roles: warp 0 TMA producer, warp 1 MMA issuer (one elected thread), warp 2 TMEM allocator,
-//   warps 4..11 epilogue.  smem ring of kStages, mbarrier full/empty pairs, one tcgen05.commit per stage.
-// * an optional second accumulator (TMEM columns N..2N) receives the 1x1 shortcut conv of a ResidualBlock.
-// * epilogue: thread = one output row (TMEM lane); GroupNorm statistics = in-thread sum over the group's columns +
-//   warp-shuffle reduction over the L lanes of the trajectory; then GN-affine, Mish, FiLM, residual, bf16/fp32 store.
+// * W_tap is a TMA box {KC, N} of the weight packed [tap][C_out][C_in]; both operands land in shared memory in the
+//   K-major SWIZZLE_128B (KC=64) / SWIZZLE_64B (KC=32) layout that wgmma consumes directly.
+// * warp roles: warp 8 TMA producer (smem ring of kStages, mbarrier full/empty pairs); warps 0-7 = two consumer
+//   warpgroups.  Warpgroup g accumulates rows [64 g, 64 g + 64) of the tile in registers (wgmma, N columns), then writes
+//   them into a shared-memory accumulator tile; an optional 1x1 shortcut conv of a ResidualBlock is accumulated next and
+//   lands in columns N..2N of that tile.  The producer runs ahead across tiles while the consumers work on the epilogue.
+// * epilogue (the same 8 warps): thread = one output row of the accumulator tile; GroupNorm statistics = in-thread sum over
+//   the group's columns + warp-shuffle reduction over the L lanes of the trajectory; then GN-affine, Mish, FiLM, residual,
+//   bf16/fp32 store.
 //
 // Algorithmic HBM bytes per launch: 2*(batch*L*C_in + batch*L*C_out) (+ shortcut input), weights once through L2.
 #pragma once
@@ -29,12 +31,12 @@
 #include <type_traits>
 
 #include "common.cuh"
-#include "ptx_sm100.cuh"
+#include "ptx_sm90.cuh"
 
 namespace cds {
 
-constexpr int kTcThreads = 320;   // warps 0-7 epilogue (TMEM lane quarter = warp % 4, column slice = warp / 4),
-                                  // warp 8 TMA producer, warp 9 TMEM allocator + MMA issuer
+constexpr int kTcThreads = 288;   // warps 0-7: two consumer warpgroups (MMA, then epilogue: accumulator row quarter = warp % 4,
+                                  // column slice = warp / 4), warp 8 TMA producer
 constexpr int kTcEpiThreads = 256;
 constexpr int kTcMaxStages = 10;
 
@@ -44,12 +46,6 @@ struct ConvTcParams {
   // x 16 columns, staged in shared memory (SWIZZLE_64B for 4-byte / SWIZZLE_32B for 2-byte elements).  Valid when out_tma != 0.
   CUtensorMap tm_out;
   int out_tma;
-  // SPLIT > 1 kernels: the SPLIT column-tile CTAs of a row tile form a thread-block cluster (cluster = SPLIT, else 1) and share
-  // the activation tiles: CTA r fetches trajectories [r*T/SPLIT, (r+1)*T/SPLIT) of the tile (tm_a_mc / tm_a2_mc: the same
-  // tensors with that smaller box) and MULTICASTS them into every CTA's stage -- the A bytes cross the L2 -> SM fabric once per
-  // row tile instead of once per column tile.
-  CUtensorMap tm_a_mc, tm_a2_mc;
-  int cluster;
   // identity residual as a TMA-load source with the box of tm_out: the fast lane prefetches the next 32 rows x 16 columns of the
   // residual into per-warp staging rows while it works on the current ones (valid when res_tma != 0; tiles of N <= 64 only)
   CUtensorMap tm_res;
@@ -75,7 +71,6 @@ constexpr int kTraceSlots = 64;
 // [10+4t] epilogue saw the accumulator, [11+4t] epilogue done
 __device__ __forceinline__ long long gtimer() { long long t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)); return t; }
 #define CDS_TRACE(slot, val) do { if (p.trace) p.trace[(int64_t)blockIdx.x * kTraceSlots + (slot)] = (val); } while (0)
-
 // MUFU approximations with flush-to-zero: ONE instruction each (the non-ftz forms expand into range fix-ups)
 __device__ __forceinline__ float ex2_ftz(float x) { float y; asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
 __device__ __forceinline__ float rcp_ftz(float x) { float y; asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
@@ -180,28 +175,30 @@ struct ConvTcCfg {
   static constexpr int kABytes = 128 * kRowBytes;
   static constexpr int kBBytes = N * kRowBytes;
   static constexpr int kStageBytes = kABytes + kBBytes;
-  // Operand ring: as deep as the shared memory of the designed residency allows (2 CTAs/SM: ~100 KB each; 1 CTA/SM: ~200 KB),
-  // at least 3, at most kTcMaxStages.  A tile is taps x C_in/KC k-blocks (5..20): only a ring that holds more than one tile
-  // lets the TMA producer run ahead of the tile whose accumulator the epilogue is still draining -- with 4 stages and
-  // 5 k-blocks per tile every tile paid one exposed L2 round trip (~1 us) on the narrow layers.
-  // (2 CTAs/SM: 227 KB - 2 x (22 KB static: per-column constants, 16 KB of epilogue store staging, barriers; + 16 KB of residual
-  // staging for the narrow tiles) - 2 x 1 KB reserved)
   static constexpr bool kResStage = N <= 64;             // per-warp staging of TMA-prefetched identity residuals
-  static constexpr int kRingBudget = (N <= 64 ? 72 : (N <= 128 ? 88 : 184)) * 1024;
-  static constexpr int kStagesFit = kRingBudget / kStageBytes;
-  static constexpr int kStages = kStagesFit < 3 ? 3 : (kStagesFit > kTcMaxStages ? kTcMaxStages : kStagesFit);
-  static constexpr int kSmemBytes = kStages * kStageBytes + 1024;
   static constexpr int kCols = N * SPLIT;                                 // columns of the whole layer
   static constexpr int kColsPerTile = N * (HAS_RES ? 2 : 1);             // main (+ shortcut) accumulator
-  static constexpr int kAccBufs = 2 * kColsPerTile <= 512 ? 2 : 1;       // double-buffered when TMEM allows
-  static constexpr uint32_t kTmemNeed = (uint32_t)(kAccBufs * kColsPerTile);
-  static constexpr uint32_t kTmemCols = kTmemNeed <= 32 ? 32 : (kTmemNeed <= 64 ? 64 : (kTmemNeed <= 128 ? 128 : (kTmemNeed <= 256 ? 256 : 512)));   // power of two
+  // shared-memory accumulator tile: 128 rows, padded by 4 floats so that the row-per-thread float4 reads of a warp are
+  // conflict-free
+  static constexpr int kAccPitch = kColsPerTile + 4;
+  static constexpr int kAccBytes = 128 * kAccPitch * 4;
+  // static shared memory: per-column constants, 16 KB of epilogue store staging (+ 16 KB of residual staging), barriers
+  static constexpr int kStaticBytes = 24 * kCols + 16 * 1024 + (kResStage ? 16 * 1024 : 0) + 512;
+  // Residency: two CTAs per SM (one's MMA overlaps the other's epilogue) when the accumulator tile, the static buffers and a
+  // ring of at least 2 stages fit into half of the SM's 227 KB; else one CTA with the deepest ring that fits.  A ring that
+  // holds more than one tile's k-blocks lets the producer run ahead of the tile whose epilogue is still running.
+  static constexpr int kPerCta2 = 113 * 1024 - kAccBytes - kStaticBytes - 1024;
+  static constexpr int kMinBlocks = kPerCta2 >= 2 * kStageBytes ? 2 : 1;
+  static constexpr int kRingBudget = kMinBlocks == 2 ? kPerCta2 : 227 * 1024 - kAccBytes - kStaticBytes - 2048;
+  static constexpr int kStagesFit = kRingBudget / kStageBytes;
+  static constexpr int kStages = kStagesFit < 1 ? 1 : (kStagesFit > kTcMaxStages ? kTcMaxStages : kStagesFit);
+  // instantiable at all: wgmma is at most 256 columns wide and the accumulator tile must leave room for one stage
+  static constexpr bool kFits = kColsPerTile <= 256 && kStagesFit >= 1;
+  static constexpr int kSmemBytes = kStages * kStageBytes + kAccBytes + 1024;
   // GroupNorm lanes exist for the power-of-two tile widths only (the 160 / 192-wide tiles serve un-normalised Linear layers)
   static constexpr bool kGnOk = (N & (N - 1)) == 0;
-  static constexpr int kEpiSplit = N >= 32 ? 2 : 1;     // epilogue warps per TMEM lane quarter (column split)
-  // designed CTAs per SM: 2 (102 registers per thread: the epilogue keeps 16-32 columns live).  3 CTAs (68 registers) were
-  // measured on the narrow tiles: the spills cost more than the extra residency buys (471 -> 490 us per iteration).
-  static constexpr int kMinBlocks = N <= 128 ? 2 : 1;
+  // epilogue warps per accumulator row quarter (column split); one when a GroupNorm group is wider than half the tile
+  static constexpr int kEpiSplit = (N >= 32 && kCols / 8 <= N / 2) ? 2 : 1;
 };
 
 // W consecutive activations (bf16 or fp32) <-> registers, 8/16-byte vector accesses
@@ -273,37 +270,30 @@ conv_tc_kernel(const __grid_constant__ ConvTcParams p, const int* __restrict__ i
   extern __shared__ uint8_t smem_raw[];
   __shared__ __align__(8) uint64_t full_bar[kTcMaxStages];
   __shared__ __align__(8) uint64_t empty_bar[kTcMaxStages];
-  __shared__ __align__(8) uint64_t tmem_full_bar[2];    // MMA -> epilogue, per accumulator buffer
-  __shared__ __align__(8) uint64_t tmem_empty_bar[2];   // epilogue -> MMA
-  __shared__ uint32_t tmem_base_holder;
   // per-column constants of the epilogue, staged once per CTA while the main loop runs:
   // 0 bias  1 GN gamma  2 GN beta  3 FiLM scale  4 FiLM shift  5 shortcut bias   (iteration-indexed "step" parts)
   __shared__ __align__(16) float s_col[6][Cfg::kCols];
   // epilogue store staging: every epilogue warp owns 32 rows x 16 columns (2 KB of fp32 / 1 KB of bf16), written in the
-  // swizzle of p.tm_out and handed to the TMA unit as one bulk store -- a warp-level st.global of its 32 rows would touch 32
-  // different cache lines per instruction (measured: the LSU serialises them, the store's source registers stay locked and the
-  // epilogue stalls on them), the bulk store writes whole sectors and costs the warp 4 conflict-free st.shared
+  // swizzle of p.tm_out and handed to the TMA unit as one bulk store -- a warp-level st.global of its 32 rows touches 32
+  // different cache lines per instruction, the bulk store writes whole sectors and costs the warp 4 conflict-free st.shared
   __shared__ __align__(1024) uint8_t s_stage[kTcEpiThreads / 32][2048];
   __shared__ __align__(1024) uint8_t s_resb[Cfg::kResStage ? kTcEpiThreads / 32 : 1][Cfg::kResStage ? 2048 : 16];
   __shared__ __align__(8) uint64_t res_bar[kTcEpiThreads / 32];
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  // operand ring, 1024-byte aligned (swizzle atoms)
+  // operand ring, 1024-byte aligned (swizzle atoms), followed by the accumulator tile (128 rows x kAccPitch floats)
   const uint32_t smem_base = (ptx::smem_u32(smem_raw) + 1023u) & ~1023u;
   uint8_t* smem_al = smem_raw + (smem_base - ptx::smem_u32(smem_raw));
+  float* const acc_s = reinterpret_cast<float*>(smem_al + Cfg::kStages * Cfg::kStageBytes);
 
   const int T = 128 >> p.log2L;                       // trajectories per tile
   if (threadIdx.x == 0) { CDS_TRACE(0, gtimer()); CDS_TRACE(1, clock64()); }
   const int n_kb_main = p.taps * p.kchunks;
   const int n_kb = n_kb_main + (HAS_RES ? p.kchunks2 : 0);
 
-  const int cs = SPLIT > 1 ? p.cluster : 1;           // cluster size (1 = no multicast)
-  const uint32_t crank = cs > 1 ? ptx::cluster_ctarank() : 0u;
-  const uint16_t cmask = (uint16_t)((1u << cs) - 1u);
   if (threadIdx.x == 0) {
-    // a stage is free again when the MMAs of EVERY CTA of the cluster have consumed it (peers multicast into it)
-    for (int s = 0; s < kTcStages; ++s) { ptx::mbar_init(&full_bar[s], 1); ptx::mbar_init(&empty_bar[s], (uint32_t)cs); }
-    for (int i = 0; i < 2; ++i) { ptx::mbar_init(&tmem_full_bar[i], 1); ptx::mbar_init(&tmem_empty_bar[i], kTcEpiThreads / 32); }
+    // a stage is free again when every consumer warp's MMAs have read it
+    for (int s = 0; s < kTcStages; ++s) { ptx::mbar_init(&full_bar[s], 1); ptx::mbar_init(&empty_bar[s], kTcEpiThreads / 32); }
     for (int i = 0; i < kTcEpiThreads / 32; ++i) ptx::mbar_init(&res_bar[i], 1);
     ptx::fence_barrier_init();
   }
@@ -312,15 +302,9 @@ conv_tc_kernel(const __grid_constant__ ConvTcParams p, const int* __restrict__ i
     ptx::prefetch_tensormap(&p.tm_b);
     if (HAS_RES) { ptx::prefetch_tensormap(&p.tm_a2); ptx::prefetch_tensormap(&p.tm_b2); }
     if (p.out_tma) ptx::prefetch_tensormap(&p.tm_out);
-    if (cs > 1) { ptx::prefetch_tensormap(&p.tm_a_mc); if (HAS_RES) ptx::prefetch_tensormap(&p.tm_a2_mc); }
     if (p.res_tma) ptx::prefetch_tensormap(&p.tm_res);
   }
-  if (warp == 9) ptx::tmem_alloc<Cfg::kTmemCols>(&tmem_base_holder);
-  ptx::tc_fence_before_sync();
   __syncthreads();
-  if (cs > 1) ptx::cluster_sync();                    // every CTA's barriers exist before a peer can signal them
-  ptx::tc_fence_after_sync();
-  const uint32_t tmem_base = tmem_base_holder;
   if (threadIdx.x == 0) CDS_TRACE(2, clock64());
   // programmatic dependent launch: the next kernel of the stream may start its own prologue and weight prefetch now; it
   // blocks in grid_dep_wait() until this grid has completed before it touches anything a predecessor wrote
@@ -366,64 +350,73 @@ conv_tc_kernel(const __grid_constant__ ConvTcParams p, const int* __restrict__ i
         uint8_t* sb = sa + Cfg::kABytes;
         if (!HAS_RES || kb < n_kb_main) {
           const int tap = kb / p.kchunks, ck = kb - tap * p.kchunks;
-          if (cs == 1) ptx::tma_load_3d(sa, &p.tm_a, &full_bar[s], ck * KE, tap - p.pad, a_b0);
-          else ptx::tma_load_3d_mc(sa + crank * (Cfg::kABytes / SPLIT), &p.tm_a_mc, &full_bar[s], ck * KE, tap - p.pad,
-                                   a_b0 + (int)crank * (T / SPLIT), cmask);
+          ptx::tma_load_3d(sa, &p.tm_a, &full_bar[s], ck * KE, tap - p.pad, a_b0);
           if (!w_done) ptx::tma_load_2d(sb, &p.tm_b, &full_bar[s], ck * KE, tap * p.C_out * p.phases + n_off);
         } else {
           const int ck = kb - n_kb_main;
-          if (cs == 1) ptx::tma_load_3d(sa, &p.tm_a2, &full_bar[s], ck * KE, 0, r_b0);
-          else ptx::tma_load_3d_mc(sa + crank * (Cfg::kABytes / SPLIT), &p.tm_a2_mc, &full_bar[s], ck * KE, 0,
-                                   r_b0 + (int)crank * (T / SPLIT), cmask);
+          ptx::tma_load_3d(sa, &p.tm_a2, &full_bar[s], ck * KE, 0, r_b0);
           if (!w_done) ptx::tma_load_2d(sb, &p.tm_b2, &full_bar[s], ck * KE, n_off);
         }
       }
       { const int t_i = (tile - blockIdx.x) / gridDim.x; if (t_i < 14) CDS_TRACE(8 + 4 * t_i, clock64()); }
       }
     }
-  } else if (warp == 9) {
-    // ===================================== MMA issuer =====================================
-    if (ptx::elect_one()) {
-      constexpr uint32_t idesc = ptx::make_idesc<TF32>(128, N);
-      int ring = 0, it = 0;
-      for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x, ++it) {
-      const int buf = it % Cfg::kAccBufs;
-      const uint32_t use = (uint32_t)(it / Cfg::kAccBufs);            // how often this buffer has been used before
-      ptx::mbar_wait(&tmem_empty_bar[buf], (use & 1) ^ 1);              // epilogue has drained the previous use
-      ptx::tc_fence_after_sync();
-      const uint32_t acc_base = tmem_base + (uint32_t)(buf * Cfg::kColsPerTile);
-      for (int kb = 0; kb < n_kb; ++kb, ++ring) {
-        const int s = ring % kTcStages;
-        const uint32_t ph = (ring / kTcStages) & 1;
-        ptx::mbar_wait(&full_bar[s], ph);
-        ptx::tc_fence_after_sync();
-        if (kb == 0 && it < 14) CDS_TRACE(9 + 4 * it, clock64());
-        const uint32_t sa = smem_base + s * Cfg::kStageBytes;
-        const uint64_t da = ptx::make_kmajor_desc<Cfg::kRowBytes>(sa);
-        const uint64_t db = ptx::make_kmajor_desc<Cfg::kRowBytes>(sa + Cfg::kABytes);
-        const bool second = HAS_RES && kb >= n_kb_main;
-        const uint32_t d_addr = acc_base + (second ? (uint32_t)N : 0u);
-        const bool first_of_acc = second ? (kb == n_kb_main) : (kb == 0);
-#pragma unroll
-        for (int k = 0; k < KC / 16; ++k) {
-          // advancing 16 bf16 / 8 tf32 (32 B) along K inside the swizzle span = +2 in the (addr >> 4) field
-          ptx::umma<TF32>(d_addr, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), idesc, (first_of_acc && k == 0) ? 0u : 1u);
-        }
-        // frees the smem slot once these MMAs have read it (in every CTA of the cluster when the slot is filled by multicast)
-        if (cs > 1) ptx::umma_commit_mc(&empty_bar[s], cmask); else ptx::umma_commit(&empty_bar[s]);
-      }
-      ptx::umma_commit(&tmem_full_bar[buf]);      // this tile's accumulators complete
-      }
-    }
   } else {
-    // ===================================== epilogue (warps 0..7) =====================================
-    // thread = one output row (TMEM lane m) x NH columns.  Everything per ELEMENT is branch-free: the operator's options
+    // ===================================== consumers (warps 0..7) =====================================
+    // MMA: warpgroup wg accumulates rows [64 wg, 64 wg + 64) of the tile in registers and writes them into acc_s; epilogue:
+    // thread = one output row of acc_s (row 32 (warp % 4) + lane) x NH columns.
+    const int wg = warp >> 2;
+    int ring = 0;                                   // k-blocks consumed so far (smem ring position, across tiles)
+    // k-blocks [kb0, kb1) of the current tile into d; each stage goes back to the producer once its MMAs have completed
+    auto mma_range = [&](float (&d)[N / 2], int kb0, int kb1, int it_) {
+#pragma unroll
+      for (int i = 0; i < N / 2; ++i) d[i] = 0.f;
+      for (int kb = kb0; kb < kb1; ++kb, ++ring) {
+        const int s = ring % kTcStages;
+        ptx::mbar_wait(&full_bar[s], (ring / kTcStages) & 1);
+        if (kb == 0 && it_ < 14 && threadIdx.x == 0) CDS_TRACE(9 + 4 * it_, clock64());
+        const uint32_t sa = smem_base + s * Cfg::kStageBytes;
+        const uint64_t da = ptx::make_kmajor_desc<Cfg::kRowBytes>(sa + wg * 64 * Cfg::kRowBytes);
+        const uint64_t db = ptx::make_kmajor_desc<Cfg::kRowBytes>(sa + Cfg::kABytes);
+        ptx::wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < KC / 16; ++k)
+          ptx::Wgmma<N, TF32>::mma(d, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), (kb > kb0 || k > 0) ? 1u : 0u);
+        ptx::wgmma_commit();
+        if constexpr (kTcStages > 1) {
+          ptx::wgmma_wait<1>();                     // the previous k-block's MMAs are complete: its stage is free
+          if (kb > kb0) { __syncwarp(); if (lane == 0) ptx::mbar_arrive(&empty_bar[(ring - 1) % kTcStages]); }
+        } else {
+          ptx::wgmma_wait<0>();                     // a one-stage ring: the producer needs this very stage for the next k-block
+          __syncwarp();
+          if (lane == 0) ptx::mbar_arrive(&empty_bar[s]);
+        }
+      }
+      if constexpr (kTcStages > 1) {
+        ptx::wgmma_wait<0>();
+        __syncwarp();
+        if (lane == 0) ptx::mbar_arrive(&empty_bar[(ring - 1) % kTcStages]);
+      }
+    };
+    // the whole tile -> acc_s (main accumulator in columns [0, N), shortcut in [N, 2N)); entered by all 8 warps
+    auto mma_tile = [&](int it_) {
+      float d[N / 2];
+      mma_range(d, 0, n_kb_main, it_);
+      ptx::named_bar_sync(2, kTcEpiThreads);        // every warp's epilogue has left the previous tile's accumulator
+      ptx::acc_store<N>(acc_s + 64 * wg * Cfg::kAccPitch, Cfg::kAccPitch, d, threadIdx.x & 127);
+      if constexpr (HAS_RES) {
+        mma_range(d, n_kb_main, n_kb, it_);
+        ptx::acc_store<N>(acc_s + 64 * wg * Cfg::kAccPitch + N, Cfg::kAccPitch, d, threadIdx.x & 127);
+      }
+      ptx::named_bar_sync(2, kTcEpiThreads);        // the tile's accumulator is complete
+    };
+    // thread = one output row (accumulator row m) x NH columns.  Everything per ELEMENT is branch-free: the operator's options
     // pick one of a few compile-time specialised chunk loops (CTA-uniform dispatch, once per tile).
     ptx::grid_dep_wait();                           // iteration counter, tables, residual inputs: all written by predecessors
     const int iter = iter_ptr ? *iter_ptr : 0;
     constexpr int EW = Cfg::kEpiSplit;
     constexpr int NH = N / EW;                      // columns per thread
-    const int q = warp & 3;                         // TMEM lane quarter this warp may touch
+    const int q = warp & 3;                         // accumulator row quarter of this warp
     const int half = warp >> 2;                     // which slice of the N columns this warp handles
     const bool active = half < EW;                  // warp-uniform (N = 16: only warps 0..3 work)
     const int n_real = p.C_out * p.phases;          // < N only for narrow heads (C_out <= 16)
@@ -496,25 +489,21 @@ conv_tc_kernel(const __grid_constant__ ConvTcParams p, const int* __restrict__ i
         ptx::tma_load_3d(rstg, &p.tm_res, &res_bar[warp], (tile_ % SPLIT) * N + col0 + 16 * gi_, 0, (tile_ / SPLIT) * T_ + traj_q);
       };
       if (res_pf && lane == 0 && (int)blockIdx.x < p.num_tiles) issue_res((int)blockIdx.x, 0);
-      const uint32_t t_lane = tmem_base + ((uint32_t)(32 * q) << 16);
       for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x, ++it) {
-        const int buf = it % Cfg::kAccBufs;
-        const uint32_t use = (uint32_t)(it / Cfg::kAccBufs);
         const int n_off = (tile % SPLIT) * N;
         const int b = (tile / SPLIT) * T_ + tb;
         const bool valid = b < batch_;
-        const uint32_t t_row = t_lane + (uint32_t)(buf * Cfg::kColsPerTile);
+        const float* const a_row = acc_s + (32 * q + lane) * Cfg::kAccPitch;
         const int traj0 = (tile / SPLIT) * T_ + traj_q;
         const ET* const res_row_p = RES ? res_l + (int64_t)b * res_bs + n_off : nullptr;
-        ptx::mbar_wait(&tmem_full_bar[buf], use & 1);
-        ptx::tc_fence_after_sync();
+        mma_tile(it);
         if (threadIdx.x == 0 && it < 14) CDS_TRACE(10 + 4 * it, clock64());
 #pragma unroll 1
         for (int ch = 0; ch < NH / WC; ++ch) {
           const int n0 = col0 + ch * WC;                            // CTA-tile column
           const float* const cb = &s_col[0][n_off + n0];            // staged constants of these columns (row stride kCols)
           float v[WC];
-          ptx::tmem_ld<WC>(t_row + (uint32_t)n0, v);
+          ptx::acc_ld<WC>(a_row + (int)n0, v);
           float s1[GPC], s2[GPC], ga[GPC], gc[GPC];
 #pragma unroll
           for (int g = 0; g < GPC; ++g) { s1[g] = 0.f; s2[g] = 0.f; }
@@ -588,7 +577,7 @@ conv_tc_kernel(const __grid_constant__ ConvTcParams p, const int* __restrict__ i
             }
             if constexpr (HAS_RES) {
               float r2[16];
-              ptx::tmem_ld<16>(t_row + (uint32_t)(N + n0 + 16 * h), r2);
+              ptx::acc_ld<16>(a_row + (int)(N + n0 + 16 * h), r2);
 #pragma unroll
               for (int k = 0; k < 4; ++k) {
                 const float4 rb = reinterpret_cast<const float4*>(cb + 5 * Cfg::kCols + 16 * h)[k];
@@ -632,14 +621,12 @@ conv_tc_kernel(const __grid_constant__ ConvTcParams p, const int* __restrict__ i
             }
           }
         }
-        // hand the accumulator buffer back to the MMA warp (one arrival per epilogue warp)
-        ptx::tc_fence_before_sync();
-        __syncwarp();
-        if (lane == 0) ptx::mbar_arrive(&tmem_empty_bar[buf]);
         if (threadIdx.x == 0 && it < 14) CDS_TRACE(11 + 4 * it, clock64());
       }
     };
-    if constexpr (N >= 32 && Cfg::kCols <= 256 && Cfg::kGnOk) {
+    // the fast and plain lanes give every one of the 8 warps a column half (they do not check `active`): only kernels with two
+    // epilogue warps per row quarter may enter them
+    if constexpr (N >= 32 && Cfg::kCols <= 256 && Cfg::kGnOk && Cfg::kEpiSplit == 2) {
       if (fast_ok) {
         using T1 = std::integral_constant<int, 1>;
         using T0 = std::integral_constant<int, 0>;
@@ -671,14 +658,11 @@ conv_tc_kernel(const __grid_constant__ ConvTcParams p, const int* __restrict__ i
       const int nct = SPLIT > 1 ? SPLIT : p.n_col_tiles;
       const int batch_ = p.batch, phases_ = p.phases, C_out_ = p.C_out;
       const int64_t out_bs = p.out_bstride, out_ls = p.out_lstride;
-      const uint32_t t_lane = tmem_base + ((uint32_t)(32 * q) << 16);
       // out_tma: 1 = {C, L, batch} view (one phase), 2 = {C, phase, L, batch} view of a two-phase transposed conv's output
       const int use_tma = p.out_tma;
       uint8_t* const stg = &s_stage[warp][0];
       const int traj_q = (32 * q) >> p.log2L;
       for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x, ++it) {
-        const int buf = it % Cfg::kAccBufs;
-        const uint32_t use = (uint32_t)(it / Cfg::kAccBufs);
         const int n_off = (tile % nct) * N;
         const int sc_off = SPLIT > 1 ? n_off : 0;
         if (SPLIT == 1 && nct > 1) {                   // runtime column tiles: this tile's constants
@@ -688,9 +672,8 @@ conv_tc_kernel(const __grid_constant__ ConvTcParams p, const int* __restrict__ i
         }
         const int b = (tile / nct) * T_ + tb;
         const bool valid = b < batch_;
-        const uint32_t t_row = t_lane + (uint32_t)(buf * Cfg::kColsPerTile);
-        ptx::mbar_wait(&tmem_full_bar[buf], use & 1);
-        ptx::tc_fence_after_sync();
+        const float* const a_row = acc_s + (32 * q + lane) * Cfg::kAccPitch;
+        mma_tile(it);
         if (threadIdx.x == 0 && it < 14) CDS_TRACE(10 + 4 * it, clock64());
 #pragma unroll 1
         for (int ch = 0; ch < NH / 16; ++ch) {
@@ -699,7 +682,7 @@ conv_tc_kernel(const __grid_constant__ ConvTcParams p, const int* __restrict__ i
           const int phase = (phases_ == 1 || ng0 < C_out_) ? 0 : 1;
           const int c0 = ng0 - phase * C_out_;
           float v[16];
-          ptx::tmem_ld<16>(t_row + (uint32_t)n0, v);
+          ptx::acc_ld<16>(a_row + (int)n0, v);
           const float4* b4 = reinterpret_cast<const float4*>(&s_col[0][sc_off + n0]);
 #pragma unroll
           for (int k = 0; k < 4; ++k) {
@@ -800,13 +783,10 @@ conv_tc_kernel(const __grid_constant__ ConvTcParams p, const int* __restrict__ i
             }
           }
         }
-        ptx::tc_fence_before_sync();
-        __syncwarp();
-        if (lane == 0) ptx::mbar_arrive(&tmem_empty_bar[buf]);
         if (threadIdx.x == 0 && it < 14) CDS_TRACE(11 + 4 * it, clock64());
       }
     };
-    if constexpr (N >= 32 && !HAS_RES) {
+    if constexpr (N >= 32 && !HAS_RES && Cfg::kEpiSplit == 2) {
       using G = std::integral_constant<int, CDS_ACT_GELU_TANH>;
       using Z = std::integral_constant<int, CDS_ACT_NONE>;
       using DF = std::integral_constant<int, CDS_F32>;
@@ -830,8 +810,6 @@ conv_tc_kernel(const __grid_constant__ ConvTcParams p, const int* __restrict__ i
     }
     // generic lane (everything else; a no-op after the fast lane: `it` then already counts all of this CTA's tiles)
     for (int tile = blockIdx.x + it * (int)gridDim.x; tile < p.num_tiles; tile += gridDim.x, ++it) {
-    const int buf = it % Cfg::kAccBufs;
-    const uint32_t use = (uint32_t)(it / Cfg::kAccBufs);
     const int nct = SPLIT > 1 ? SPLIT : p.n_col_tiles;
     const int64_t row = (int64_t)(tile / nct) * 128 + m;
     const int n_off = (tile % nct) * N;
@@ -845,7 +823,7 @@ conv_tc_kernel(const __grid_constant__ ConvTcParams p, const int* __restrict__ i
     }
     const bool valid = active && row < (int64_t)p.batch * p.L;
     const int b = (int)(row >> p.log2L), l = (int)(row & (p.L - 1));
-    const uint32_t t_row = tmem_base + ((uint32_t)(32 * q) << 16) + (uint32_t)(buf * Cfg::kColsPerTile);
+    const float* const a_row = acc_s + (32 * q + lane) * Cfg::kAccPitch;
     const int bs = p.sample_div > 1 ? b / p.sample_div : b;        // owner of the per-trajectory vectors (flattened token rows)
     const float* bias_smp = p.bias.sample ? p.bias.sample + (int64_t)bs * p.bias.sample_stride : nullptr;
     const float* scale_smp = p.scale.sample ? p.scale.sample + (int64_t)bs * p.scale.sample_stride : nullptr;
@@ -853,8 +831,7 @@ conv_tc_kernel(const __grid_constant__ ConvTcParams p, const int* __restrict__ i
     const int rb = p.res_batch_mod > 0 ? b % p.res_batch_mod : b;
     const int64_t res_row = (int64_t)rb * p.res_bstride + (int64_t)l * p.res_lstride;
 
-    ptx::mbar_wait(&tmem_full_bar[buf], use & 1);
-    ptx::tc_fence_after_sync();
+    mma_tile(it);
     if (threadIdx.x == 0 && it < 14) CDS_TRACE(10 + 4 * it, clock64());
 
     // ---- 16 finished pre-activation columns (y) -> activation, FiLM, residual(s), store.  n0 = CTA-tile column.
@@ -886,7 +863,7 @@ conv_tc_kernel(const __grid_constant__ ConvTcParams p, const int* __restrict__ i
       }
       if constexpr (HAS_RES) {
         float r2[16];
-        ptx::tmem_ld<16>(t_row + (uint32_t)(N + n0), r2);
+        ptx::acc_ld<16>(a_row + (int)(N + n0), r2);
         const float4* rb4 = reinterpret_cast<const float4*>(&s_col[5][sg0]);
 #pragma unroll
         for (int k = 0; k < 4; ++k) {
@@ -940,7 +917,7 @@ conv_tc_kernel(const __grid_constant__ ConvTcParams p, const int* __restrict__ i
       }
       if (p.out_tma == 1 && io_vec) {
         // like the fast / plain lanes: the warp's 32 rows x 16 columns through its swizzled staging rows and ONE bulk tensor store
-        // (a thread storing its own row reaches a third of that: profiles/r02_micro_store_patterns.txt).  This is the lane of
+        // (a thread storing its own row touches 32 cache lines per warp-wide store).  This is the lane of
         // ChiUNet1d's FiLM convs (per-trajectory scale and shift); rows beyond the batch are clipped by the TMA unit.
         uint8_t* const stg = &s_stage[warp][0];
         if (lane == 0) ptx::bulk_wait_group_read<0>();
@@ -1006,7 +983,7 @@ conv_tc_kernel(const __grid_constant__ ConvTcParams p, const int* __restrict__ i
       constexpr bool GN = decltype(gn_tag)::value;
       if constexpr (GN && N >= 32 && (Cfg::kCols / 8) > 32) {
         // wide layers (C_out = 512 / 1024: ChiUNet1d): a GroupNorm group is 64 / 128 columns -- too many to hold in registers,
-        // so the group is read from TMEM twice: statistics first, then normalise + activation + store, 32 columns at a time
+        // so the group is read from the accumulator tile twice: statistics first, then normalise + activation + store, 32 columns at a time
         constexpr int CPG = Cfg::kCols / 8;
         constexpr int GPT = NH / CPG;                 // whole groups per thread
         static_assert(NH % CPG == 0 && GPT >= 1, "a thread's column slice must hold whole GroupNorm groups");
@@ -1018,7 +995,7 @@ conv_tc_kernel(const __grid_constant__ ConvTcParams p, const int* __restrict__ i
           for (int ch = 0; ch < CPG / 32; ++ch) {
             const int n0 = col0 + g * CPG + ch * 32;
             float v[32];
-            ptx::tmem_ld<32>(t_row + (uint32_t)n0, v);
+            ptx::acc_ld<32>(a_row + (int)n0, v);
             add_bias(std::integral_constant<int, 32>{}, v, n0);
 #pragma unroll
             for (int j = 0; j < 32; ++j) { s1[0] += v[j]; s2[0] = fmaf(v[j], v[j], s2[0]); }
@@ -1028,7 +1005,7 @@ conv_tc_kernel(const __grid_constant__ ConvTcParams p, const int* __restrict__ i
           for (int ch = 0; ch < CPG / 32; ++ch) {
             const int n0 = col0 + g * CPG + ch * 32;
             float v[32];
-            ptx::tmem_ld<32>(t_row + (uint32_t)n0, v);
+            ptx::acc_ld<32>(a_row + (int)n0, v);
             add_bias(std::integral_constant<int, 32>{}, v, n0);
             const float4* ga4 = reinterpret_cast<const float4*>(&s_col[1][n_off + n0]);
             const float4* be4 = reinterpret_cast<const float4*>(&s_col[2][n_off + n0]);
@@ -1045,7 +1022,7 @@ conv_tc_kernel(const __grid_constant__ ConvTcParams p, const int* __restrict__ i
           }
         }
       } else if constexpr (GN && N >= 32) {
-        // GroupNorm (8 groups over the layer's kCols columns).  A chunk of WC = max(16, CPG) columns is read from TMEM
+        // GroupNorm (8 groups over the layer's kCols columns).  A chunk of WC = max(16, CPG) columns is read from the accumulator
         // once and holds GPC = WC / CPG whole groups: per-thread sums over the group's columns, all-reduce over the L
         // lanes (= positions) of the trajectory, then y = ((v - mean) * rstd) * gamma + beta as two FMAs per element.
         constexpr int CPG = Cfg::kCols / 8;
@@ -1056,7 +1033,7 @@ conv_tc_kernel(const __grid_constant__ ConvTcParams p, const int* __restrict__ i
         for (int ch = 0; ch < NH / WC; ++ch) {
           const int n0 = col0 + ch * WC;
           float v[WC];
-          ptx::tmem_ld<WC>(t_row + (uint32_t)n0, v);
+          ptx::acc_ld<WC>(a_row + (int)n0, v);
           add_bias(std::integral_constant<int, WC>{}, v, n0);
           float s1[GPC], s2[GPC], ga[GPC], gc[GPC];
 #pragma unroll
@@ -1084,7 +1061,7 @@ conv_tc_kernel(const __grid_constant__ ConvTcParams p, const int* __restrict__ i
 #pragma unroll 1
         for (int ch = 0; ch < NH / 16; ++ch) {
           float v[16];
-          ptx::tmem_ld<16>(t_row + (uint32_t)(col0 + ch * 16), v);
+          ptx::acc_ld<16>(a_row + (int)(col0 + ch * 16), v);
           add_bias(std::integral_constant<int, 16>{}, v, col0 + ch * 16);
           post16(act_tag, film_tag, v, std::integral_constant<int, 0>{}, col0 + ch * 16);
         }
@@ -1115,10 +1092,6 @@ conv_tc_kernel(const __grid_constant__ ConvTcParams p, const int* __restrict__ i
         else run(F{}, AX{}, F2{});
       }
     }
-    // hand the accumulator buffer back to the MMA warp (one arrival per epilogue warp)
-    ptx::tc_fence_before_sync();
-    __syncwarp();
-    if (lane == 0) ptx::mbar_arrive(&tmem_empty_bar[buf]);
     if (threadIdx.x == 0 && it < 14) CDS_TRACE(11 + 4 * it, clock64());
     }   // tile loop
     if (threadIdx.x == 0) CDS_TRACE(5, (long long)it);
@@ -1128,11 +1101,6 @@ conv_tc_kernel(const __grid_constant__ ConvTcParams p, const int* __restrict__ i
   // the CTA retires
   if (warp < kTcEpiThreads / 32 && lane == 0) ptx::bulk_wait_group<0>();
   __syncthreads();
-  if (cs > 1) ptx::cluster_sync();                    // no CTA retires while a peer may still multicast into it / signal its barriers
-  if (warp == 9) {
-    ptx::tc_fence_after_sync();
-    ptx::tmem_dealloc<Cfg::kTmemCols>(tmem_base);
-  }
   if (threadIdx.x == 0) { CDS_TRACE(3, clock64()); CDS_TRACE(4, gtimer()); }
 }
 
@@ -1223,6 +1191,13 @@ inline bool conv_tc_eligible(const cds_conv_op& c) {
   if (c.stride == 1 ? (c.L_in != L) : (c.L_in != 2 * L || c.phases != 1 || c.res_w || c.res)) return false;
   if (conv_tc_width(c) == 0) return false;
   if (conv_tc_width(c) > 256 && c.groups != 0 && conv_tc_pick_kc(c) != 64) return false;   // wide GN variants: KC = 64 only
+  if (c.res_w) {
+    // the main and the shortcut accumulator share one wgmma-width (256-column) tile: CTA tiles of at most 128 columns
+    const int n = conv_tc_width(c);
+    const bool fixed = n == 16 || n == 32 || n == 64 || n == 128 || n == 256 || ((n == 512 || n == 1024) && c.groups != 0);
+    const int tile = fixed ? (n > 256 ? 128 : (n >= 128 ? n / 2 : n)) : conv_tc_runtime_tile(n, conv_tc_pick_kc(c));
+    if (tile > 128) return false;
+  }
   if (c.sample_row_div > 1 && c.L_out != 1) return false;
   if (c.C_in % kmin != 0) return false;
   if (c.groups != 0 && (c.groups != 8 || c.phases != 1 || c.C_out < 32)) return false;
@@ -1252,19 +1227,14 @@ struct ConvTcLaunch {
 };
 
 // Share a layer's columns between two CTAs?  Yes for the wide layers (C_out >= 128: halves the per-CTA epilogue and main
-// loop and lets two CTAs share an SM) and for C_out = 64 when there are too few row tiles to fill the machine.
+// loop) and for C_out = 64 when there are too few row tiles to fill the machine.
 inline int conv_tc_pick_split(const cds_conv_op& c, int n_total, int m_tiles) {
-  if (n_total > 256) return n_total / 256;
+  if (n_total > 256) return n_total / (c.res_w ? 128 : 256);     // (with a shortcut conv: 2 x 128 accumulator columns per CTA)
   if (c.phases != 1 || n_total < 64) return 1;
-  if (const char* ns = getenv("CDS_TC_NOSPLIT")) { if (ns[0] == '1') return 1; if (ns[0] == '2' && n_total == 128) return 1; }   // experiment
   if (n_total >= 128) return 2;
-  // TF32 programs: two 32-wide CTAs fetch the (fp32) activation tile twice, and the kernels are bound by the L2 -> SM feed of
-  // their operand tiles (DESIGN.md section 5), so the 64-wide layers stay whole even when that leaves fewer tiles than CTA slots
-  // (cfg2, TF32: 597 vs 608 us per iteration)
+  // TF32 programs: two 32-wide CTAs fetch the (fp32) activation tile twice, so the 64-wide layers stay whole
   if (conv_is_tf32(c)) return 1;
-  const char* e = getenv("CDS_TC_SPLIT64");
-  if (e && e[0] == '1') return 2;                    // experiment: C_out = 64 always as two N = 32 CTAs (3 CTAs/SM residency)
-  return m_tiles < 296 ? 2 : 1;
+  return m_tiles < 2 * 132 ? 2 : 1;                  // fewer row tiles than two per SM of an H100 (132 SMs): split
 }
 
 inline bool conv_tc_prepare(const cds_conv_op& c, ConvTcLaunch* out) {
@@ -1307,27 +1277,12 @@ inline bool conv_tc_prepare(const cds_conv_op& c, ConvTcLaunch* out) {
     uint32_t box[2] = {(uint32_t)ke, (uint32_t)L.n};
     if (!encode_act_map(&p.tm_b, c.w, 2, dims, str, box, kc, tf32)) return false;
   }
-  // Opt-in (CDS_MULTICAST=1).  Measured on B200 (cfg2, batch 4096): 636 vs 615 us per iteration in TF32, 474 vs 452 in bf16 --
-  // what binds the main loop is the bytes INGESTED into each SM's shared memory (TMA fill + MMA operand reads, ~128 B/clk/SM),
-  // which multicast does not reduce, while the lock-step of the cluster costs a little.
-  { const char* mc = getenv("CDS_MULTICAST"); p.cluster = (L.split > 1 && T % L.split == 0 && mc && mc[0] == '1') ? L.split : 1; }
-  if (p.cluster > 1) {      // the activation tensor again, with the box of ONE cluster CTA's share of the tile's trajectories
-    uint64_t dims[3] = {(uint64_t)c.C_in, (uint64_t)c.L_in, in_b};
-    uint64_t str[2] = {(uint64_t)c.in_lstride, (uint64_t)c.in_bstride};
-    uint32_t box[3] = {(uint32_t)ke, (uint32_t)(Lp * c.stride), (uint32_t)(T / L.split)};
-    uint32_t es[3] = {1u, (uint32_t)c.stride, 1u};
-    if (!encode_act_map(&p.tm_a_mc, c.in, 3, dims, str, box, kc, tf32, es)) return false;
-  }
   if (L.has_res) {
     const uint64_t r_b = c.res_batch_mod > 0 ? (uint64_t)c.res_batch_mod : (uint64_t)c.batch;
     uint64_t dims[3] = {(uint64_t)c.res_C, (uint64_t)Lp, r_b};
     uint64_t str[2] = {(uint64_t)c.res_in_lstride, (uint64_t)c.res_in_bstride};
     uint32_t box[3] = {(uint32_t)ke, (uint32_t)Lp, (uint32_t)T};
     if (!encode_act_map(&p.tm_a2, c.res_in, 3, dims, str, box, kc, tf32)) return false;
-    if (p.cluster > 1) {
-      uint32_t boxp[3] = {(uint32_t)ke, (uint32_t)Lp, (uint32_t)(T / L.split)};
-      if (!encode_act_map(&p.tm_a2_mc, c.res_in, 3, dims, str, boxp, kc, tf32)) return false;
-    }
     uint64_t d2[2] = {(uint64_t)c.res_C, (uint64_t)c.C_out};
     uint64_t s2[1] = {(uint64_t)c.res_C};
     uint32_t b2[2] = {(uint32_t)ke, (uint32_t)L.n};
@@ -1405,6 +1360,9 @@ long long* conv_tc_trace_hook(int grid);
 template <int KC, int N, bool HAS_RES, int SPLIT, bool TF32>
 cudaError_t conv_tc_launch_t(const ConvTcLaunch& L, const int* iter_ptr, cudaStream_t st) {
   using Cfg = ConvTcCfg<KC, N, HAS_RES, SPLIT>;
+  if constexpr (!Cfg::kFits) {
+    return cudaErrorInvalidConfiguration;      // (never picked: conv_tc_eligible keeps shortcut tiles at <= 128 columns)
+  } else {
   static bool attr = false;
   static int resident = 0;                   // CTAs of this instantiation that fit on the device at once
   static int sm_count = 0;
@@ -1413,26 +1371,21 @@ cudaError_t conv_tc_launch_t(const ConvTcLaunch& L, const int* iter_ptr, cudaStr
     cudaError_t e = cudaFuncSetAttribute(conv_tc_kernel<KC, N, HAS_RES, SPLIT, TF32>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                          Cfg::kSmemBytes);
     if (e != cudaSuccess) return e;
-    // several CTAs per SM for the narrow tiles: ask for the maximum shared-memory carve-out
     e = cudaFuncSetAttribute(conv_tc_kernel<KC, N, HAS_RES, SPLIT, TF32>, cudaFuncAttributePreferredSharedMemoryCarveout,
                              cudaSharedmemCarveoutMaxShared);
     if (e != cudaSuccess) return e;
     int dev = 0, sms = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    // residency we design for: launch-bounds blocks, TMEM (kTmemCols of 512 columns per SM), 227 KB shared memory
-    int want = Cfg::kMinBlocks;
-    int by_tmem = 512 / (int)Cfg::kTmemCols;
-    // static shared memory: 16 KB store staging + 24 B/column of constants + barriers (+ 16 KB residual staging), 1 KB reserved
-    const int static_smem = 16 * 1024 + 24 * Cfg::kCols + 1024 + (Cfg::kResStage ? 16 * 1024 : 0) + 1024;
-    int by_smem = (227 * 1024) / (Cfg::kSmemBytes + static_smem);
-    if (want > by_tmem) want = by_tmem;
-    if (want > by_smem) want = by_smem;
+    int want = 0;
+    e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&want, conv_tc_kernel<KC, N, HAS_RES, SPLIT, TF32>, kTcThreads, Cfg::kSmemBytes);
+    if (e != cudaSuccess) return e;
+    if (want > Cfg::kMinBlocks) want = Cfg::kMinBlocks;
     if (const char* cap = getenv("CDS_TC_MAXCTAS")) { int c = atoi(cap); if (c >= 1 && c < want) want = c; }
     if (want < 1) want = 1;
     if (getenv("CDS_DEBUG"))
-      fprintf(stderr, "[cds] conv_tc<%d,%d,%d,%d,%s>: designed %d CTA/SM (tmem %d, smem %d), smem %d B, %d stages\n", KC, N,
-              (int)HAS_RES, SPLIT, TF32 ? "tf32" : "bf16", want, by_tmem, by_smem, Cfg::kSmemBytes, Cfg::kStages);
+      fprintf(stderr, "[cds] conv_tc<%d,%d,%d,%d,%s>: %d CTA/SM, smem %d B, %d stages\n", KC, N, (int)HAS_RES, SPLIT,
+              TF32 ? "tf32" : "bf16", want, Cfg::kSmemBytes, Cfg::kStages);
     resident = want * sms;
     sm_count = sms;
     const char* pdl_env = getenv("CDS_PDL");
@@ -1442,34 +1395,32 @@ cudaError_t conv_tc_launch_t(const ConvTcLaunch& L, const int* iter_ptr, cudaStr
   unsigned cap = (unsigned)resident;
   if (L.max_ctas_per_sm > 0 && (unsigned)(L.max_ctas_per_sm * sm_count) < cap) cap = (unsigned)(L.max_ctas_per_sm * sm_count);
   dim3 grid(L.grid.x < cap ? L.grid.x : cap);
-  const unsigned cl = L.prm.cluster > 1 ? (unsigned)L.prm.cluster : 1u;
-  if (cl > 1) grid.x -= grid.x % cl;                 // whole clusters: the CTAs of a cluster walk the same row tiles in lockstep
   ConvTcParams prm = L.prm;
   prm.trace = conv_tc_trace_hook((int)grid.x);
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = grid; cfg.blockDim = dim3(kTcThreads); cfg.dynamicSmemBytes = Cfg::kSmemBytes; cfg.stream = st;
-  cudaLaunchAttribute at[2];
+  cudaLaunchAttribute at[1];
   int na = 0;
   if (pdl) { at[na].id = cudaLaunchAttributeProgrammaticStreamSerialization; at[na].val.programmaticStreamSerializationAllowed = 1; ++na; }
-  if (cl > 1) {
-    at[na].id = cudaLaunchAttributeClusterDimension;
-    at[na].val.clusterDim.x = cl; at[na].val.clusterDim.y = 1; at[na].val.clusterDim.z = 1;
-    ++na;
-  }
   cfg.attrs = at; cfg.numAttrs = na;
   return cudaLaunchKernelEx(&cfg, conv_tc_kernel<KC, N, HAS_RES, SPLIT, TF32>, prm, iter_ptr);
+  }
 }
 // touch the kernel once (module load) so that nothing lazy happens inside a stream capture
 template <int KC, int N, bool HAS_RES, int SPLIT, bool TF32>
 cudaError_t conv_tc_preload_t() {
-  cudaFuncAttributes a;
-  return cudaFuncGetAttributes(&a, conv_tc_kernel<KC, N, HAS_RES, SPLIT, TF32>);
+  if constexpr (!ConvTcCfg<KC, N, HAS_RES, SPLIT>::kFits) {
+    return cudaSuccess;
+  } else {
+    cudaFuncAttributes a;
+    return cudaFuncGetAttributes(&a, conv_tc_kernel<KC, N, HAS_RES, SPLIT, TF32>);
+  }
 }
 
 // every (KC, N, SPLIT) the dispatcher can pick (each with and without the shortcut accumulator); X(kc, n, split)
 #define CDS_TC_VARIANTS(X)                                                                              \
   X(64, 16, 1) X(64, 32, 1) X(64, 64, 1) X(64, 128, 1) X(64, 256, 1) X(64, 32, 2) X(64, 64, 2) X(64, 128, 2) \
-  X(64, 256, 2) X(64, 256, 4) X(64, 160, 1) X(64, 192, 1)                                                \
+  X(64, 256, 2) X(64, 256, 4) X(64, 128, 4) X(64, 128, 8) X(64, 160, 1) X(64, 192, 1)                    \
   X(32, 16, 1) X(32, 32, 1) X(32, 64, 1) X(32, 128, 1) X(32, 256, 1) X(32, 32, 2) X(32, 64, 2) X(32, 128, 2)
 
 #ifndef CDS_TC_INSTANTIATE

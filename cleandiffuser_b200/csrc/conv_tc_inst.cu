@@ -19,9 +19,9 @@ namespace cds {
   template cudaError_t conv_tc_preload_t<KC_, N_, true, S_, (CDS_TC_TF32 != 0)>();
 
 #if CDS_TC_PART == 0
-CDS_TC_INST(64, 16, 1) CDS_TC_INST(32, 16, 1) CDS_TC_INST(64, 256, 2)
+CDS_TC_INST(64, 16, 1) CDS_TC_INST(32, 16, 1) CDS_TC_INST(64, 256, 2) CDS_TC_INST(64, 128, 8)
 #elif CDS_TC_PART == 1
-CDS_TC_INST(64, 32, 1) CDS_TC_INST(32, 32, 1) CDS_TC_INST(64, 256, 4)
+CDS_TC_INST(64, 32, 1) CDS_TC_INST(32, 32, 1) CDS_TC_INST(64, 256, 4) CDS_TC_INST(64, 128, 4)
 #elif CDS_TC_PART == 2
 CDS_TC_INST(64, 64, 1) CDS_TC_INST(32, 64, 1) CDS_TC_INST(64, 160, 1)
 #elif CDS_TC_PART == 3

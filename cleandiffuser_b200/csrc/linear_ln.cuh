@@ -6,28 +6,29 @@
 //
 // It replaces, at plan-finalize time, a CDS_OP_CONV in its "gated" form directly followed by the CDS_OP_LNMOD that reads its
 // output (cds_api.cu: fuse_linear_ln) -- the ABI and the lowering do not know about it.  Why a kernel of its own:
-//   * LayerNorm needs the whole row, so one CTA owns all C = 2 * NH output columns of its 128 rows: two tcgen05.mma (N = NH) per
-//     32-byte K step into TMEM columns [0, NH) and [NH, 2 NH); the activation chunk is staged ONCE for both halves (the generic
-//     kernel's 160-wide column tiles re-fetch it per tile), which is what the L2-feed-bound TF32 main loop cares about;
+//   * LayerNorm needs the whole row, so one CTA owns all C = 2 * NH output columns of its 128 rows: two consumer warpgroups
+//     (rows [0, 64) / [64, 128)) issue two wgmma (N = NH) per 32-byte K step into register accumulators for the column halves
+//     [0, NH) and [NH, 2 NH); the activation chunk is staged ONCE for both halves (the generic kernel's 160-wide column tiles
+//     re-fetch it per tile), which is what the L2-feed-bound TF32 main loop cares about;
 //   * the separate LayerNorm launch (read X, write Y: 8 bytes per element of HBM traffic, ~230 us per call at cfg4's size)
 //     disappears: X never leaves the SM between the two.
-// Epilogue, 8 warps (TMEM lane quarter q = warp & 3, column half hh = warp >> 2), two passes over the thread's NH columns; the
-// accumulator is released after the FIRST one, so the next tile's main loop overlaps the second:
+// Once a tile's MMAs have read their operands, the accumulators are written as a 128 x C fp32 tile over the operand ring (the
+// ring is idle then: the producer is held back by the tile's last ring stages, which are handed back only after pass 1).
+// Epilogue, the same 8 warps (accumulator row quarter q = warp & 3, column half hh = warp >> 2), two passes over the thread's
+// NH columns; the ring is released after the FIRST one, so the producer fetches the next tile's operands during the second:
 //   1. x = (acc + bias) * gate + residual.  The residual arrives by TMA, 16 columns x 32 rows per warp and request, one request
 //      ahead (a thread walking its own 1280-byte-pitch row with ld.global costs 13 us per tile: scripts/micro/store_patterns.cu
 //      v5 is the store-side twin of that pattern); x is computed IN PLACE in that buffer and bulk-stored from it to X; row moments
 //      about a pivot (the row's first x: no cancellation), the two halves' (mean, M2) combine exactly in shared memory
 //   2. the x chunks come back by TMA from the X just written (L2 hits; each request waits for the completion of that chunk's
 //      store): y = (x - mean) * rstd * (1 + scale) + shift, in place, bulk-stored to Y (rounded to TF32 when Y feeds a Linear)
-// The accumulator is single-buffered (2 NH <= 512 TMEM columns leave no room for a second one): the MMA of the next tile waits
-// for pass 1 only, the producer keeps prefetching operand stages meanwhile.
 // Algorithmic HBM bytes per row: 4 K (A) + 4 C (R) + 4 C (X) + 4 C (Y);  flops per row: 2 K C.
 #pragma once
 #include "conv_tc.cuh"
 
 namespace cds {
 
-constexpr int kLlThreads = 320;                      // warps 0-7 epilogue, 8 producer, 9 MMA + TMEM owner
+constexpr int kLlThreads = 288;                      // warps 0-7 MMA (two warpgroups) + epilogue, warp 8 TMA producer
 constexpr int kLlEpiThreads = 256;
 constexpr int kLlAhead = 4;                          // steps between the request of a per-trajectory vector chunk and its use
 
@@ -59,6 +60,8 @@ struct LinLnCfg {
   static constexpr int kStage = kStageA + kStageB;
   static constexpr int kStaging = 8 * 3 * 2048;                       // per epilogue warp: three buffers of 32 rows x 16 fp32
   static constexpr int kSmemBytes = kStages * kStage + kStaging + 1024;
+  static constexpr int kAccPitch = 2 * NH + 4;                        // accumulator tile row (floats), padded against bank conflicts
+  static_assert(kStages * kStage >= 128 * kAccPitch * 4, "the accumulator tile must fit over the operand ring");
   static_assert(NH % 16 == 0 && NH >= 16 && NH <= 256, "column half");
   static_assert((NH * 128) % 1024 == 0, "the second weight half must start on a swizzle atom");
 };
@@ -67,10 +70,8 @@ template <int NH>
 __global__ void __launch_bounds__(kLlThreads, 1) linear_ln_kernel(const __grid_constant__ LinLnParams p, const int* __restrict__ iter_ptr) {
   using Cfg = LinLnCfg<NH>;
   constexpr int C = 2 * NH;
-  constexpr uint32_t kTmemCols = 512;
   extern __shared__ uint8_t ll_smem_raw[];
-  __shared__ __align__(8) uint64_t full_bar[Cfg::kStages], empty_bar[Cfg::kStages], tmem_full_bar, tmem_empty_bar;
-  __shared__ uint32_t tmem_base_holder;
+  __shared__ __align__(8) uint64_t full_bar[Cfg::kStages], empty_bar[Cfg::kStages];
   __shared__ __align__(16) float s_bias[C];
   __shared__ float s_red[2][2][2][128];            // [tile parity][mean | M2][column half][row]
   __shared__ __align__(8) uint64_t res_bar[8][3];
@@ -81,19 +82,15 @@ __global__ void __launch_bounds__(kLlThreads, 1) linear_ln_kernel(const __grid_c
   const int n_k = p.K >> 5;                            // 32-channel chunks
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < Cfg::kStages; ++s) { ptx::mbar_init(&full_bar[s], 1); ptx::mbar_init(&empty_bar[s], 1); }
-    ptx::mbar_init(&tmem_full_bar, 1);
-    ptx::mbar_init(&tmem_empty_bar, 8);
+    // a stage is free again when every consumer warp is done with it (one arrival per warp)
+    for (int s = 0; s < Cfg::kStages; ++s) { ptx::mbar_init(&full_bar[s], 1); ptx::mbar_init(&empty_bar[s], kLlEpiThreads / 32); }
     for (int w = 0; w < 8; ++w) for (int j = 0; j < 3; ++j) ptx::mbar_init(&res_bar[w][j], 1);
     ptx::fence_barrier_init();
     ptx::prefetch_tensormap(&p.tm_a); ptx::prefetch_tensormap(&p.tm_b);
     ptx::prefetch_tensormap(&p.tm_x); ptx::prefetch_tensormap(&p.tm_y); ptx::prefetch_tensormap(&p.tm_r); ptx::prefetch_tensormap(&p.tm_xl);
   }
-  if (warp == 9) ptx::tmem_alloc<kTmemCols>(&tmem_base_holder);
-  ptx::tc_fence_before_sync();
   __syncthreads();
-  ptx::tc_fence_after_sync();
-  const uint32_t tmem_base = tmem_base_holder;
+  float* const acc = reinterpret_cast<float*>(sm);     // accumulator tile over the operand ring: 128 rows x kAccPitch floats
   ptx::grid_dep_wait();                                // (no-op unless launched with a programmatic dependency)
 
   if (warp == 8) {                                     // ------------------------------------------------ producer
@@ -111,35 +108,49 @@ __global__ void __launch_bounds__(kLlThreads, 1) linear_ln_kernel(const __grid_c
         }
       }
     }
-  } else if (warp == 9) {                              // ------------------------------------------------ MMA issuer
-    if (lane == 0) {
-      constexpr uint32_t idesc = ptx::make_idesc_tf32(128, NH);
-      uint32_t n = 0, t = 0;
-      for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x, ++t) {
-        ptx::mbar_wait(&tmem_empty_bar, (t & 1u) ^ 1u);                // the epilogue has drained the previous tile
-        ptx::tc_fence_after_sync();
-        for (int kc = 0; kc < n_k; ++kc, ++n) {
-          const int s = n % Cfg::kStages;
-          ptx::mbar_wait(&full_bar[s], (n / Cfg::kStages) & 1u);
-          ptx::tc_fence_after_sync();
-          const uint32_t a = base_u + (uint32_t)(s * Cfg::kStage);
-          const uint64_t da = ptx::make_kmajor_desc<128>(a);
-          const uint64_t db0 = ptx::make_kmajor_desc<128>(a + Cfg::kStageA);
-          const uint64_t db1 = ptx::make_kmajor_desc<128>(a + Cfg::kStageA + NH * 128);
-#pragma unroll
-          for (int k = 0; k < 4; ++k) {
-            const uint32_t acc = (kc | k) ? 1u : 0u;
-            ptx::umma_tf32(tmem_base, da + (uint64_t)(2 * k), db0 + (uint64_t)(2 * k), idesc, acc);
-            ptx::umma_tf32(tmem_base + (uint32_t)NH, da + (uint64_t)(2 * k), db1 + (uint64_t)(2 * k), idesc, acc);
-          }
-          ptx::umma_commit(&empty_bar[s]);             // stage free when these MMAs have read it
-        }
-        ptx::umma_commit(&tmem_full_bar);
-      }
-    }
   } else {                                             // ------------------------------------------------ epilogue (warps 0..7)
     const int q = warp & 3, hh = warp >> 2;
     const int m = 32 * q + lane;
+    // ---- MMA of one tile: warpgroup hh accumulates rows [64 hh, 64 hh + 64) x all C columns in registers, then acc <- them
+    uint32_t n = 0;                                    // k-blocks consumed so far (ring position)
+    uint32_t n_tile0 = 0;                              // ... at the start of the current tile
+    auto mma_tile = [&]() {
+      float d0[NH / 2], d1[NH / 2];
+#pragma unroll
+      for (int i = 0; i < NH / 2; ++i) { d0[i] = 0.f; d1[i] = 0.f; }
+      n_tile0 = n;
+      for (int kc = 0; kc < n_k; ++kc, ++n) {
+        const int s = n % Cfg::kStages;
+        ptx::mbar_wait(&full_bar[s], (n / Cfg::kStages) & 1u);
+        const uint32_t a = base_u + (uint32_t)(s * Cfg::kStage);
+        const uint64_t da = ptx::make_kmajor_desc<128>(a + (uint32_t)(hh * 64 * 128));
+        const uint64_t db0 = ptx::make_kmajor_desc<128>(a + Cfg::kStageA);
+        const uint64_t db1 = ptx::make_kmajor_desc<128>(a + Cfg::kStageA + NH * 128);
+        ptx::wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+          ptx::Wgmma<NH, true>::mma(d0, da + (uint64_t)(2 * k), db0 + (uint64_t)(2 * k), 1u);
+          ptx::Wgmma<NH, true>::mma(d1, da + (uint64_t)(2 * k), db1 + (uint64_t)(2 * k), 1u);
+        }
+        ptx::wgmma_commit();
+        ptx::wgmma_wait<1>();
+        // the previous k-block's stage goes back to the producer, unless it is one of the tile's last kStages k-blocks: those
+        // stages are where the accumulator tile goes (handed back after pass 1)
+        if (kc >= 1 && kc - 1 < n_k - Cfg::kStages) { __syncwarp(); if (lane == 0) ptx::mbar_arrive(&empty_bar[(n - 1) % Cfg::kStages]); }
+      }
+      ptx::wgmma_wait<0>();
+      ptx::named_bar_sync(2, kLlEpiThreads);           // both warpgroups' MMAs have read the ring
+      ptx::acc_store<NH>(acc + 64 * hh * Cfg::kAccPitch, Cfg::kAccPitch, d0, threadIdx.x & 127);
+      ptx::acc_store<NH>(acc + 64 * hh * Cfg::kAccPitch + NH, Cfg::kAccPitch, d1, threadIdx.x & 127);
+      ptx::named_bar_sync(2, kLlEpiThreads);           // the accumulator tile is complete
+    };
+    // after pass 1 of every warp: the withheld stages (the accumulator tile) go back to the producer
+    auto release_ring = [&]() {
+      ptx::fence_proxy_async();                        // generic writes of the tile before the TMA unit refills the ring
+      __syncwarp();
+      if (lane == 0)
+        for (int j = n_k - Cfg::kStages; j < n_k; ++j) ptx::mbar_arrive(&empty_bar[(n_tile0 + (uint32_t)j) % Cfg::kStages]);
+    };
     for (int i = threadIdx.x; i < C; i += kLlEpiThreads) s_bias[i] = p.bias[(int64_t)(*iter_ptr) * p.bias_step_stride + i];
     ptx::named_bar_sync(1, kLlEpiThreads);
     // three rotating 2 KB buffers per warp (32 rows x 16 fp32, SWIZZLE_64B).  Use number u works in buffer u % 3: a 16-column
@@ -149,11 +160,12 @@ __global__ void __launch_bounds__(kLlThreads, 1) linear_ln_kernel(const __grid_c
     uint8_t* const stg = s_stage + warp * 6144;
     const int sw = (lane >> 1) & 3;
     const uint32_t lane_off = (uint32_t)lane * 64u;
-    const uint32_t t_row = tmem_base + ((uint32_t)(32 * q) << 16) + (uint32_t)(hh * NH);
+    const float* const a_row = acc + m * Cfg::kAccPitch + hh * NH;
     const float inv_c = 1.f / (float)C;
     uint64_t* const rbar = &res_bar[warp][0];
     uint32_t t = 0, u = 0, par = 0;                    // tiles done, buffer uses, phase bit of each buffer's load barrier
     for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x, ++t) {
+      mma_tile();
       const int64_t grow = (int64_t)tile * 128 + m;
       const int row0 = tile * 128 + 32 * q;
       // Per-trajectory vectors (gate in pass 1; scale, shift in pass 2).  A warp's 32 rows touch at most two trajectories (L >= 32):
@@ -197,8 +209,6 @@ __global__ void __launch_bounds__(kLlThreads, 1) linear_ln_kernel(const __grid_c
         const int nt = tile + (int)gridDim.x;
         if (nt < p.num_tiles) ptx::tma_prefetch_2d(&p.tm_rp, hh * NH, nt * 128 + 32 * q);   // (residual form only: see the guard above)
       }
-      ptx::mbar_wait(&tmem_full_bar, t & 1u);
-      ptx::tc_fence_after_sync();
       // ---- pass 1: x = (acc + bias) * gate + residual -> X; shifted row moments
       float sh0 = 0.f, sd = 0.f, sdd = 0.f;            // pivot (the row's first x of this half), sum (x - pivot), sum (x - pivot)^2
 #pragma unroll 1
@@ -216,7 +226,7 @@ __global__ void __launch_bounds__(kLlThreads, 1) linear_ln_kernel(const __grid_c
           aq[kLlAhead - 1] = __ldg(scp_ld + 16 * j2); dq[kLlAhead - 1] = __ldg(shp_ld + 16 * j2);
         }
         float v[16];
-        ptx::tmem_ld<16>(t_row + (uint32_t)(16 * ch), v);
+        ptx::acc_ld<16>(a_row + 16 * ch, v);
         float4 rt[4];
         if (table) {
 #pragma unroll
@@ -266,10 +276,6 @@ __global__ void __launch_bounds__(kLlThreads, 1) linear_ln_kernel(const __grid_c
           ptx::bulk_commit_group();
         }
       }
-      // the accumulator has been read: the MMA of the next tile may overwrite it while pass 2 runs
-      ptx::tc_fence_before_sync();
-      __syncwarp();
-      if (lane == 0) ptx::mbar_arrive(&tmem_empty_bar);
       // this half's (mean, M2) from the shifted moments; the two halves combine exactly (Chan et al.): M2 = M2a + M2b + d^2 n / 2
       {
         const float mh = sd * (1.f / (float)NH);
@@ -289,6 +295,7 @@ __global__ void __launch_bounds__(kLlThreads, 1) linear_ln_kernel(const __grid_c
         }
       }
       ptx::named_bar_sync(1, kLlEpiThreads);
+      release_ring();                                  // every warp has read its accumulator rows
       const float ma = s_red[t & 1][0][0][m], mb = s_red[t & 1][0][1][m];
       const float mean = 0.5f * (ma + mb);
       const float m2 = s_red[t & 1][1][0][m] + s_red[t & 1][1][1][m] + (mb - ma) * (mb - ma) * (0.5f * (float)NH);
@@ -336,25 +343,22 @@ __global__ void __launch_bounds__(kLlThreads, 1) linear_ln_kernel(const __grid_c
     if (lane == 0) ptx::bulk_wait_group<0>();
   }
   ptx::grid_dep_launch_dependents();
-  ptx::tc_fence_before_sync();
   __syncthreads();
-  if (warp == 9) {
-    ptx::tc_fence_after_sync();
-    ptx::tmem_dealloc<kTmemCols>(tmem_base);
-  }
 }
 
 // ------------------------------------------------------------------------------------------------ host side
 // Can the pair (conv, lnmod) run as one linear_ln launch?  conv: TF32 tensor-core Linear over flattened tokens in its gated form
 // out = (acc + bias) * gate(trajectory) + res; lnmod: reads exactly that output, one row per token.
 inline int linear_ln_pick_nh(int c_out) {
-  switch (c_out) { case 256: return 128; case 320: return 160; case 384: return 192; case 512: return 256; default: return 0; }
+  // C = 256 only: each warpgroup holds 64 rows x C fp32 accumulators in registers, and a 9-warp CTA gets at most 168
+  // registers per thread -- wider rows spill and run slower than the two-launch form, which serves them
+  switch (c_out) { case 256: return 128; default: return 0; }
 }
 inline bool linear_ln_eligible(const cds_conv_op& c, const cds_lnmod_op& l) {
   { const char* e = getenv("CDS_FUSE_LN"); if (e && e[0] == '0') return false; }      // (read at every finalize: tests toggle it)
   if (c.math != CDS_MATH_TF32_TC || linear_ln_pick_nh(c.C_out) == 0) return false;
   if (c.taps != 1 || c.stride != 1 || c.pad != 0 || c.phases != 1 || c.L_in != 1 || c.L_out != 1) return false;
-  if (c.C_in % 32 != 0 || c.C_in < 32 || c.groups != 0 || c.act != CDS_ACT_NONE) return false;
+  if (c.C_in % 32 != 0 || c.C_in < 32 * 3 || c.groups != 0 || c.act != CDS_ACT_NONE) return false;   // (>= kStages k-blocks)
   if (c.in_batch_mod < 0 || c.in_batch_mod % 128 != 0) return false;        // (CFG branches sharing x_t: whole 128-row tiles repeat)
   if (c.in_dtype == CDS_BF16 || c.out_dtype == CDS_BF16 || c.res_dtype == CDS_BF16) return false;
   if (c.in_bstride != c.C_in || c.out_bstride != c.C_out) return false;                       // dense rows
@@ -419,13 +423,13 @@ typedef void (*LinLnKernel)(const LinLnParams, const int*);
 inline LinLnKernel linear_ln_kernel_for(int nh, int* smem) {
   switch (nh) {
 #define CDS_LL(N) case N: *smem = LinLnCfg<N>::kSmemBytes; return linear_ln_kernel<N>;
-    CDS_LL(128) CDS_LL(160) CDS_LL(192) CDS_LL(256)
+    CDS_LL(128)
 #undef CDS_LL
     default: return nullptr;
   }
 }
 inline cudaError_t linear_ln_preload_all() {
-  for (int nh : {128, 160, 192, 256}) {
+  for (int nh : {128}) {
     int smem = 0;
     LinLnKernel k = linear_ln_kernel_for(nh, &smem);
     cudaError_t e = cudaFuncSetAttribute(reinterpret_cast<const void*>(k), cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
@@ -437,7 +441,7 @@ inline cudaError_t linear_ln_launch(const LinLnLaunch& L, const int* iter_ptr, i
   int smem = 0;
   LinLnKernel k = linear_ln_kernel_for(L.nh, &smem);
   if (!k) return cudaErrorInvalidValue;
-  int grid = sm_count > 0 ? sm_count : 148;
+  int grid = sm_count > 0 ? sm_count : 132;
   if (grid > L.prm.num_tiles) grid = L.prm.num_tiles;
   k<<<grid, kLlThreads, smem, st>>>(L.prm, iter_ptr);
   return cudaGetLastError();

@@ -55,7 +55,7 @@ class DiffusionModel:
         self.fix_mask = to_tensor(fix_mask, self.device)[None, ] if fix_mask is not None else 0.
         self.loss_weight = to_tensor(loss_weight, self.device)[None, ] if loss_weight is not None else 1.
 
-        # sm_100a sampling plans, keyed by (which weights, shapes, option set); see engine/runtime.py.  The plans hold packed
+        # sm_90a sampling plans, keyed by (which weights, shapes, option set); see engine/runtime.py.  The plans hold packed
         # copies of the weights: ``_weights_epoch`` is bumped by everything in this class that mutates parameters (optimiser
         # step, EMA update, checkpoint load) and is part of the version the plans compare before every run.
         self._engine_plans = {}

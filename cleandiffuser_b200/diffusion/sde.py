@@ -6,7 +6,7 @@ cleandiffuser/diffusion/diffusionsde.py (:35-245 base, :247-606 discrete, :609-9
 ``sample()`` is a dispatcher.  When the model lives on a CUDA device, the backbone is one the
 engine can lower (JannerUNet1d / ChiUNet1d / DiT1d / DQLMlp), gradients are not requested and no
 per-step Python hook is needed (classifier guidance, history capture), the whole reverse loop
-runs as one replayed CUDA-graph of hand-written sm_100a kernels with x_t resident on the device
+runs as one replayed CUDA-graph of hand-written sm_90a kernels with x_t resident on the device
 (``engine/runtime.py``).  Everything else -- CPU tensors, user-defined backbones,
 ``requires_grad=True`` (Diffusion-QL back-propagates through the loop), classifier guidance,
 ``preserve_history`` -- takes the PyTorch loop below, which is step-for-step the reference

@@ -2,7 +2,7 @@
 
 No torch types cross this boundary: operators carry raw device pointers (``tensor.data_ptr()``),
 sizes and strides; the stream is the integer ``cudaStream_t`` of ``torch.cuda.current_stream()``.
-The library is built in-tree by ``__graft_entry__.build()`` (nvcc, sm_100a).  There is NO fallback:
+The library is built in-tree by ``__graft_entry__.build()`` (nvcc, sm_90a).  There is NO fallback:
 if the shared object is missing, ``load()`` raises and the CUDA sampling path fails loudly.
 """
 import ctypes as C
@@ -114,7 +114,7 @@ def load():
         return _lib
     if not os.path.exists(_LIB_PATH):
         raise RuntimeError(
-            f"{_LIB_PATH} is missing: the sm_100a extension has not been built "
+            f"{_LIB_PATH} is missing: the sm_90a extension has not been built "
             "(run `python -c 'import __graft_entry__ as g; g.build()'`). There is no CPU/PyTorch fallback "
             "for the CUDA sampling path.")
     lib = C.CDLL(_LIB_PATH)

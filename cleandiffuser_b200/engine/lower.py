@@ -130,8 +130,8 @@ def w_convT(conv: nn.ConvTranspose1d) -> WSpec:
 
 
 def round_tf32(w: torch.Tensor) -> torch.Tensor:
-    """fp32 -> nearest TF32-representable fp32 (10-bit mantissa, ties away from zero like cvt.rna.tf32.f32).  tcgen05
-    kind::tf32 ignores the low 13 mantissa bits of its operands, i.e. truncates; weights are rounded once here so that
+    """fp32 -> nearest TF32-representable fp32 (10-bit mantissa, ties away from zero like cvt.rna.tf32.f32).  wgmma
+    .tf32 ignores the low 13 mantissa bits of its operands, i.e. truncates; weights are rounded once here so that
     their part of the error is unbiased."""
     bits = w.detach().to(torch.float32).contiguous().view(torch.int32)
     return ((bits + 0x1000) & ~0x1FFF).view(torch.float32)
@@ -471,6 +471,18 @@ def _unet_body_with_mod(p, net, x, horizon, k, film_of, stage_len, final_k, in_b
     return pred
 
 
+def _fixed_shape_rows(fn, x: torch.Tensor, chunk: int = 1024) -> torch.Tensor:
+    """``fn`` over the rows of ``x`` in chunks of ``chunk`` rows (the last one zero-padded): every row goes through GEMMs of
+    the same shape whatever the batch, so a trajectory's conditioning rows do not depend on how many trajectories share the
+    call (BLAS libraries pick their algorithm, and with it the summation order, by problem size).  Pinned by the sub-batch
+    check of tests/test_baseline_configs_gpu.py::test_cfg5_consistency_one_step_per_gpu_batch (8192 vs 256 trajectories)."""
+    n = x.shape[0]
+    pad = (-n) % chunk
+    if pad:
+        x = torch.cat([x, x.new_zeros((pad,) + tuple(x.shape[1:]))])
+    return torch.cat([fn(c) for c in x.split(chunk)])[:n]
+
+
 def lower_chi(p: Program, net: nn.Module, x: View, horizon: int, has_cond: bool, in_batch_mod: int) -> View:
     if not net.obs_as_global_cond:
         raise Unsupported("ChiUNet1d(obs_as_global_cond=False)")
@@ -489,10 +501,13 @@ def lower_chi(p: Program, net: nn.Module, x: View, horizon: int, has_cond: bool,
     def fill(ctx):
         # cond_encoder(cat[time, obs]) = W_t Mish(time) + b  (per iteration)  +  W_o Mish(obs)  (per trajectory)
         te = F.mish(net.map_emb(net.map_noise(ctx.t_all)))
-        oe = F.mish(net.global_cond_encoder(torch.flatten(ctx.cond_rows, 1)))
         step_tab.copy_(torch.cat([F.linear(te, b.cond_encoder[1].weight[:, :e_dim], b.cond_encoder[1].bias)
                                   for b in blocks], 1))
-        samp_tab.copy_(torch.cat([F.linear(oe, b.cond_encoder[1].weight[:, e_dim:]) for b in blocks], 1))
+
+        def per_traj(c):
+            oe = F.mish(net.global_cond_encoder(c))
+            return torch.cat([F.linear(oe, b.cond_encoder[1].weight[:, e_dim:]) for b in blocks], 1)
+        samp_tab.copy_(_fixed_shape_rows(per_traj, torch.flatten(ctx.cond_rows, 1)))
     p.per_call.append(fill)
 
     def film_of(b):
@@ -751,7 +766,7 @@ def lower_dit(p: Program, net: nn.Module, x: View, horizon: int, has_cond: bool,
     # ---- tokens
     # residual stream X and the attention operands QKV stay fp32; what feeds a Linear layer (the modulated tokens Y, the
     # attention output, the MLP hidden) has the program's activation dtype: bf16 on tensor-core programs, where those Linear
-    # layers (97 % of DiT1d's FLOPs outside attention) run on tcgen05 over the flattened token stream
+    # layers (97 % of DiT1d's FLOPs outside attention) run on wgmma over the flattened token stream
     f32 = torch.float32
     X = p.act(L, d, f32)
     # head_dim 32 (every pipeline) and L <= 128: attention runs on tensor cores (mma.sync, bf16 q/k/v); otherwise fp32 CUDA cores
@@ -792,7 +807,7 @@ def lower_denoiser(p: Program, net: nn.Module, x: View, x_shape, has_cond: bool,
     """Dispatch on the backbone type (reference instances are recognised structurally by class name)."""
     name = type(net).__name__
     if name in ("JannerUNet1d", "ChiUNet1d") and len(x_shape) == 2 and p.tc:
-        # TMA/UMMA want K in whole 64-byte rows: 32 bf16 / 16 fp32 channels
+        # TMA/wgmma want K in whole 64-byte rows: 32 bf16 / 16 fp32 channels
         x = p.cast_pad(x, p.k_align * ((x.C + p.k_align - 1) // p.k_align), rows=in_batch_mod or p.rows)
     if name == "JannerUNet1d" and len(x_shape) == 2:
         return lower_janner(p, net, x, x_shape[0], has_cond, in_batch_mod)

@@ -14,8 +14,8 @@ odd shapes ...) and the caller continues on the PyTorch path; a missing/unsound 
 
 Environment switches (no flag system, pipelines stay unchanged):
   CDS_BACKEND = auto | torch | cuda    (torch: never use the engine; cuda: raise instead of falling back)
-  CDS_MATH    = tf32 | bf16 | fp32     (conv/linear GEMMs: tcgen05 with fp32 activations read as TF32 -- the default, the
-                                        arithmetic of the reference's own GPU path --, tcgen05 with bf16 operands and
+  CDS_MATH    = tf32 | bf16 | fp32     (conv/linear GEMMs: wgmma with fp32 activations read as TF32 -- the default, the
+                                        arithmetic of the reference's own GPU path --, wgmma with bf16 operands and
                                         activations, or fp32 FMA on CUDA cores)
   CDS_GRAPH   = 1 | 0                  (0: launch kernels directly, for profilers)
   CDS_NOISE_TAPE_MB                    (cap of the pre-drawn noise tape, default 4096: longer loops are run in chunks)
@@ -59,19 +59,19 @@ def _weights_version(module: torch.nn.Module, epoch: int = 0):
 
 
 def _device_ok(device: torch.device) -> bool:
-    """Can the engine serve tensors on ``device``?  CDS_BACKEND=auto: only a CUDA device of compute capability >= 10.0 with
-    the sm_100a library built; anything else (CPU, A100/H100, extension not built) quietly takes the PyTorch loop like the
-    reference would.  CDS_BACKEND=cuda: any CUDA device qualifies here and a missing library / wrong architecture fails
+    """Can the engine serve tensors on ``device``?  CDS_BACKEND=auto: only a CUDA device of compute capability 9.0 (H100) with
+    the sm_90a library built; anything else (CPU, other architectures, extension not built) quietly takes the PyTorch loop like
+    the reference would.  CDS_BACKEND=cuda: any CUDA device qualifies here and a missing library / wrong architecture fails
     loudly further down (tests and bench run that way)."""
     if device.type != "cuda":
         return False
     if _backend() == "cuda":
         return True
     try:
-        major = torch.cuda.get_device_capability(device)[0]
+        cap = torch.cuda.get_device_capability(device)
     except Exception:
         return False
-    return major >= 10 and os.path.exists(cabi.lib_path())
+    return cap == (9, 0) and os.path.exists(cabi.lib_path())
 
 
 def _tape_budget_bytes():
@@ -112,9 +112,7 @@ class _Ctx:
 def _n_branches(batch, row, consistency):
     """Independent sub-batches ("branches") whose kernel chains run on parallel streams: while one chain sits at a kernel
     boundary (drain, dependency latency, ramp-up: ~3 us of every ~12 us layer) the other chain's kernel keeps the SMs busy.
-    CDS_BRANCHES sets the count, CDS_BRANCH_MIN_BATCH the smallest sub-batch worth a branch (default 1024).  Default 1:
-    measured on B200 (cfg2, batch 4096) two branches neither gain nor lose (473.9 vs 471.1 us per iteration) -- every CTA is
-    bound by its own per-tile epilogue latency, not by the boundaries -- and four lose 9 %."""
+    CDS_BRANCHES sets the count, CDS_BRANCH_MIN_BATCH the smallest sub-batch worth a branch (default 1024).  Default 1."""
     want = int(os.environ.get("CDS_BRANCHES", "1"))
     min_sub = int(os.environ.get("CDS_BRANCH_MIN_BATCH", "1024"))
     if consistency:

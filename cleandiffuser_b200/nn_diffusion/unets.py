@@ -7,7 +7,7 @@ the reference so ``.pt`` checkpoints interchange:
 These modules are the weight containers and the autograd (training /
 ``requires_grad=True``) path.  For sampling, ``engine/lower.py`` walks the same
 module tree and emits the fused conv+GN+Mish(+FiLM/+residual) op list that the
-sm_100a kernels execute.
+sm_90a kernels execute.
 """
 from typing import List, Optional
 

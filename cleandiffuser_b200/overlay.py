@@ -7,7 +7,7 @@
 
 to this package's classes, so that a pipeline's ``from cleandiffuser.diffusion import DiscreteDiffusionSDE`` -- and
 everything else it imports from the reference: datasets, envs, classifiers, ``nn_classifier``, ``utils.report_parameters``
-... -- keeps working, while ``agent.sample(...)`` runs the reverse loop on the sm_100a engine.  The reference's own
+... -- keeps working, while ``agent.sample(...)`` runs the reverse loop on the sm_90a engine.  The reference's own
 ``nn_diffusion`` / ``nn_condition`` modules are accepted as they are: the lowering recognises backbones structurally
 (class name + attributes, ``engine/lower.py``), and the PyTorch path calls them like the reference does.
 
@@ -45,7 +45,7 @@ def reference_available() -> bool:
 
 
 def install(strict: bool = True) -> List[str]:
-    """Rebind the reference's sampler classes to the B200 engine's.  Returns the patched ``module.attr`` names.
+    """Rebind the reference's sampler classes to the H100 engine's.  Returns the patched ``module.attr`` names.
     ``strict=False`` returns [] instead of raising when the reference is not importable.  Idempotent."""
     from . import diffusion as ours
     if _PATCHED:

@@ -1,4 +1,4 @@
-"""The BASELINE.json configurations as synthetic workloads (SURVEY 8d recipe: weights seed 0, inputs seed 1).
+"""The BASELINE configurations (cfg2 .. cfg5: the headline of bench.py and its other_configs) as synthetic workloads (SURVEY 8d recipe: weights seed 0, inputs seed 1).
 
 One place that says what "cfg2 .. cfg5" are, shared by ``bench.py`` (headline + ``other_configs``), the parity
 tests at the configs' full sizes (``tests/test_baseline_configs_gpu.py``) and the profiling scripts, so that the

@@ -1,7 +1,7 @@
 """Alias package: ``import cleandiffuser`` resolves to ``cleandiffuser_b200`` (use when the reference is NOT installed).
 
 Put ``<repo>/compat`` (and the repo root) on PYTHONPATH; the reference's pipeline scripts then import
-``cleandiffuser.diffusion`` / ``nn_diffusion`` / ``nn_condition`` / ``utils`` unchanged and get the B200 engine.
+``cleandiffuser.diffusion`` / ``nn_diffusion`` / ``nn_condition`` / ``utils`` unchanged and get the H100 engine.
 Sub-packages outside the hot path (dataset, env, classifier, invdynamic ...) are deliberately absent."""
 import importlib
 import sys
@@ -22,6 +22,6 @@ _NOT_PORTED = ("classifier", "nn_classifier", "dataset", "env", "invdynamic")
 
 def __getattr__(name):
     if name in _NOT_PORTED:
-        raise ImportError(f"cleandiffuser.{name} is outside the B200 engine's scope (SURVEY section 8) and not part of the alias "
+        raise ImportError(f"cleandiffuser.{name} is outside the H100 engine's scope (SURVEY section 8) and not part of the alias "
                           "package: install the reference and call cleandiffuser_b200.install() instead (drop-in route A)")
     raise AttributeError(name)

@@ -1,4 +1,4 @@
-/* cds.h -- C ABI of the B200 diffusion-sampling engine (libcds.so).
+/* cds.h -- C ABI of the H100 diffusion-sampling engine (libcds.so).
  *
  * The reference (CleanDiffuser) has no FFI of its own: its hot path is the Python loop
  * DiscreteDiffusionSDE.sample / ContinuousDiffusionSDE.sample (cleandiffuser/diffusion/diffusionsde.py:401-606,
@@ -63,13 +63,13 @@ typedef enum cds_act { CDS_ACT_NONE = 0, CDS_ACT_MISH = 1, CDS_ACT_SILU = 2, CDS
                        CDS_ACT_GELU_ERF = 6 /* exact GELU 0.5 x (1 + erf(x / sqrt 2)) (nn.GELU default; pearcemlp.py:30) */ } cds_act;
 /* math mode of CDS_OP_CONV:
  *   CDS_MATH_FP32     fp32 CUDA-core FMA (bit-faithful to the fp32 oracle up to summation order)
- *   CDS_MATH_BF16_TC  tcgen05 tensor cores, bf16 operands and bf16 inter-layer activations, fp32 TMEM accumulation
- *   CDS_MATH_TF32_TC  tcgen05 tensor cores kind::tf32: fp32 activations and weights in memory, read by the MMA as TF32
+ *   CDS_MATH_BF16_TC  wgmma tensor cores, bf16 operands and bf16 inter-layer activations, fp32 accumulation
+ *   CDS_MATH_TF32_TC  wgmma tensor cores (.tf32): fp32 activations and weights in memory, read by the MMA as TF32
  *                     (10-bit mantissa), fp32 accumulation -- the arithmetic of the reference's own GPU path
  *                     (torch.backends.cudnn.allow_tf32 = True is PyTorch's default for convolutions)            */
 typedef enum cds_math { CDS_MATH_FP32 = 0, CDS_MATH_BF16_TC = 1, CDS_MATH_TF32_TC = 2 } cds_math;
 /* element type of an activation tensor.  CDS_TF32 is fp32 STORAGE whose values are rounded to the nearest TF32 (10-bit
- * mantissa, ties away from zero, like cvt.rna.tf32.f32) when an operator writes them: tcgen05 kind::tf32 ignores the low 13
+ * mantissa, ties away from zero, like cvt.rna.tf32.f32) when an operator writes them: wgmma .tf32 ignores the low 13
  * mantissa bits of its fp32 operands (truncation), so an operand that is already rounded is read exactly and its rounding
  * error is unbiased and half as large.  Producers honour it on store; consumers read CDS_TF32 exactly like CDS_F32. */
 typedef enum cds_dtype { CDS_F32 = 0, CDS_BF16 = 1, CDS_TF32 = 2 } cds_dtype;
@@ -110,7 +110,7 @@ typedef struct cds_conv_op {
   int32_t in_batch_mod;            /* >0: read in() at batch index b % in_batch_mod (CFG branches share x_t) */
   const void* in;   int64_t in_bstride;  int32_t in_lstride;   /* strides in ELEMENTS of the tensor's dtype */
   const void*  w;                  /* CDS_MATH_FP32: fp32 [taps*C_in][C_out*phases] (K rows, N contiguous)
-                                      CDS_MATH_BF16_TC: bf16 [taps][C_out][C_in]     (K contiguous, TMA/UMMA K-major)
+                                      CDS_MATH_BF16_TC: bf16 [taps][C_out][C_in]     (K contiguous, TMA/wgmma K-major)
                                       CDS_MATH_TF32_TC: fp32 [taps][C_out][C_in]     (same packing, fp32 elements) */
   cds_vec bias;
   int32_t groups; const float* gn_gamma; const float* gn_beta; float gn_eps;

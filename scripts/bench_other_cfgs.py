@@ -1,5 +1,5 @@
 """Per-operator device times and throughput of BASELINE configs 3 / 4 / 5 on one GPU (workloads of cleandiffuser_b200/workloads.py,
-per-GPU batch).  Not the bench contract (bench.py = cfg2 + an other_configs block): detail for DESIGN.md / profiles/.
+per-GPU batch).  Not the headline benchmark (bench.py = cfg2 + an other_configs block): per-operator detail.
   python scripts/bench_other_cfgs.py [cfg3 cfg4 cfg5] [--math tf32|bf16|fp32] [--reps 3] [--once]"""
 import argparse
 import json

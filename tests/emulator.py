@@ -3,7 +3,7 @@
 It lets the CPU test-suite execute the *lowered* program (``engine/lower.py`` output, with CPU tensors behind
 the raw pointers) and compare it with the reference goldens, so that lowering bugs (wrong strides, offsets,
 table columns, phase packing ...) are caught here without a GPU; the kernels themselves are then checked
-against the same goldens on the B200.  Never imported by the product.
+against the same goldens on the H100.  Never imported by the product.
 """
 import ctypes
 
@@ -91,7 +91,7 @@ def _act(kind, x):
 
 
 def _tf32_trunc(x):
-    """what tcgen05 kind::tf32 sees of an fp32 operand: the low 13 mantissa bits are ignored"""
+    """what wgmma .tf32 sees of an fp32 operand: the low 13 mantissa bits are ignored"""
     return (np.ascontiguousarray(x, dtype=np.float32).view(np.uint32) & np.uint32(0xFFFFE000)).view(np.float32)
 
 

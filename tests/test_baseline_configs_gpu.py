@@ -1,4 +1,4 @@
-"""Parity at BASELINE.json's FULL sizes, in the math mode bench.py measures (CDS_MATH=tf32, the library default): every config
+"""Parity at the BASELINE configurations' FULL sizes (cleandiffuser_b200/workloads.py), in the math mode bench.py measures (CDS_MATH=tf32, the library default): every config
 runs its complete ``sample()`` at its per-GPU batch through the CUDA engine (C ABI), and a slice of the batch is compared with
 the CPU oracle (fp32) run on the same prior / condition / noise draws.
 

@@ -1,5 +1,5 @@
 """Parity of the CUDA engine (through the C ABI) against the golden vectors of the reference and the
-CPU oracle.  Everything here needs a B200: run with ``-m gpu``."""
+CPU oracle.  Everything here needs an H100: run with ``-m gpu``."""
 import os
 
 import numpy as np
@@ -149,7 +149,7 @@ def test_smoke_entry():
 
 
 # ------------------------------------------------------------------------------------------------------------------
-# tensor-core programs (CDS_MATH=bf16): bf16 operands / activations, fp32 TMEM accumulation and fp32 GN/Mish epilogue.
+# tensor-core programs (CDS_MATH=bf16): bf16 operands / activations, fp32 accumulation and fp32 GN/Mish epilogue.
 # Stated tolerance vs the fp32 reference (SURVEY 8c, measured by emulation: ~8e-3 relative per forward, no
 # compounding over the reverse steps): max-abs 2e-1, mean-abs 2e-2 on O(1) outputs.
 BF16_NETS = ["janner_cfg2", "janner_kitchen_cond", "chi_small", "chi_cm_fourier", "dit_small", "dit_pos_uncond"]
@@ -248,7 +248,7 @@ def test_parallel_branches_give_the_same_bits(math, monkeypatch):
 
 # ------------------------------------------------------------------------------------------------------------------
 # TF32 tensor-core programs (CDS_MATH=tf32, the library default and what bench.py measures): fp32 activations and weights in
-# memory, tcgen05 kind::tf32 (operands read with a 10-bit mantissa), fp32 TMEM accumulation and fp32 GN/Mish epilogue -- the
+# memory, wgmma .tf32 (operands read with a 10-bit mantissa), fp32 accumulation and fp32 GN/Mish epilogue -- the
 # arithmetic of the reference's own GPU path (cuDNN TF32 convs).  Stated tolerance vs the fp32 reference: max-abs 2e-2,
 # mean-abs 2e-3 (per forward and after a full sampler; emulated figures: ~4e-3 / ~9e-4 per forward).
 TF32_MAX, TF32_MEAN = 2e-2, 2e-3
@@ -309,7 +309,7 @@ def test_tf32_is_the_default_math_mode(monkeypatch):
 
 def test_chiunet_full_size_on_tensor_cores(monkeypatch):
     """cfg3's backbone exactly as the DP pipelines build it (model_dim 256 -> 256/512/1024 channels, 68.9 M parameters): every conv,
-    the C_out = 512 / 1024 ones included (2 / 4 CTAs of 256 columns, two-pass GroupNorm), runs on tcgen05; checked against the
+    the C_out = 512 / 1024 ones included (2 / 4 CTAs of 256 columns, two-pass GroupNorm), runs on wgmma; checked against the
     module's own fp32 forward on the GPU (TF32 off), bf16 tolerance."""
     monkeypatch.setenv("CDS_MATH", "bf16")
     from cleandiffuser_b200.engine.lower import Program, View, lower_denoiser
@@ -335,7 +335,7 @@ def test_chiunet_full_size_on_tensor_cores(monkeypatch):
 
 def test_dit_full_size_on_tensor_cores(monkeypatch):
     """cfg4's backbone as the DD pipeline builds it (d_model 320, 10 heads of 32, depth 2, L = 100 tokens -- not a multiple of
-    the 16-row MMA tile: padded keys are masked, padded queries dropped): Linear layers on tcgen05 over the flattened token
+    the 16-row MMA tile: padded keys are masked, padded queries dropped): Linear layers on wgmma over the flattened token
     stream, attention on mma.sync, checked against the module's own fp32 forward on the GPU."""
     monkeypatch.setenv("CDS_MATH", "bf16")
     from cleandiffuser_b200.engine.lower import Program, View, lower_denoiser

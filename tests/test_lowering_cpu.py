@@ -86,7 +86,7 @@ def test_lowered_denoiser_bf16(golden, name, monkeypatch):
 @pytest.mark.parametrize("name", list(cases.NETS))
 def test_lowered_denoiser_tf32(golden, name, monkeypatch):
     """TF32 programs (the default math mode): fp32 activations, fp32 [tap][Cout][Cin] weights rounded to TF32, operands
-    truncated to a 10-bit mantissa by the interpreter as tcgen05 kind::tf32 does."""
+    truncated to a 10-bit mantissa by the interpreter as wgmma .tf32 does."""
     monkeypatch.setenv("CDS_MATH", "tf32")
     case = cases.NETS[name]
     net, _ = product_net(case)
@@ -148,7 +148,7 @@ def test_bf16_program_uses_tensor_core_ops(monkeypatch):
     lower_denoiser(p, net, View(xin, 32, 14), (32, 14), False, 0)
     kinds = [op.u.conv.math for op in p.ops if op.kind == cabi.OP_CONV]
     # x_t is handed over as a 32-channel bf16 copy (CDS_OP_CAST), so EVERY conv of the UNet -- stride-2 down-sampling,
-    # two-phase transposed up-sampling and the 14-channel 1x1 head included -- runs on tcgen05
+    # two-phase transposed up-sampling and the 14-channel 1x1 head included -- runs on wgmma
     assert p.ops[0].kind == cabi.OP_CAST
     assert kinds.count(cabi.MATH_BF16_TC) == len(kinds) == 40, kinds
 
@@ -301,7 +301,7 @@ def test_dit_tf32_program_keeps_attention_on_tensor_cores(monkeypatch):
     tokens = [c for c in tc if c.batch == B * L]                  # Linear layers over the flattened token stream
     assert sorted((c.C_in, c.C_out) for c in tokens) == sorted([(320, 960), (320, 320), (320, 1280), (1280, 320)] * 2 + [(32, 320), (320, 29)])
     # fp32 operands qualify for the TF32 kernels as they are: the per-trajectory conditioning GEMMs (map_emb 320 -> 320 and the
-    # adaLN 320 -> 4480 Linear) run on tcgen05 too
+    # adaLN 320 -> 4480 Linear) run on wgmma too
     assert sorted((c.C_in, c.C_out) for c in tc if c.batch == B) == [(320, 320), (320, 4480)]
     attn = [op.u.attn for op in p.ops if op.kind == cabi.OP_ATTN]
     assert len(attn) == 2 and all(a.qkv_dtype == cabi.TF32 and a.out_dtype == cabi.TF32 for a in attn)
