@@ -76,40 +76,53 @@ int elementwise_grid(int64_t total, int sm_count) {
   return (int)(blocks < cap ? (blocks > 0 ? blocks : 1) : cap);
 }
 
+// The kernel family of a conv op (CDS_CONV_SIMT / _TC / _PS) and, for conv_simt, its tile width: every check of validate()
+// except the null-pointer ones, so that cds_conv_choice answers for descriptors whose buffers do not exist yet.
+int conv_pick(const cds_conv_op& c, int* family, int* bn) {
+  if (c.batch <= 0 || c.L_in <= 0 || c.L_out <= 0 || c.C_in <= 0 || c.C_out <= 0 || c.taps <= 0 ||
+      c.stride <= 0 || c.phases <= 0)
+    return fail(CDS_ERR_INVALID, "conv: non-positive geometry");
+  if (c.groups > 8) return fail(CDS_ERR_UNSUPPORTED, "conv: more than 8 GroupNorm groups");
+  if (c.res_w && c.res_C <= 0) return fail(CDS_ERR_INVALID, "conv: shortcut conv without input");
+  if (c.res_w && (c.stride != 1 || c.phases != 1)) return fail(CDS_ERR_INVALID, "conv: shortcut conv needs stride 1");
+  *bn = 0;
+  if (c.math == CDS_MATH_BF16_TC || c.math == CDS_MATH_TF32_TC) {
+    if (!cds::conv_tc_eligible(c))
+      return fail(CDS_ERR_INVALID, "conv: op is not eligible for the tensor-core kernel (ask cds_conv_tc_supported)");
+    *family = cds::conv_ps_eligible(c) ? CDS_CONV_PS : CDS_CONV_TC;
+    return CDS_OK;
+  }
+  if (c.math != CDS_MATH_FP32) return fail(CDS_ERR_UNSUPPORTED, "conv: math mode %d unknown", c.math);
+  if (c.sample_row_div > 1) return fail(CDS_ERR_UNSUPPORTED, "conv: sample_row_div needs the tensor-core kernel");
+  *bn = cds::conv_simt_pick_bn(c);
+  if (*bn == 0)
+    return fail(CDS_ERR_UNSUPPORTED, "conv: GroupNorm tile does not fit (L_out=%d C_out=%d groups=%d)", c.L_out,
+                c.C_out, c.groups);
+  *family = CDS_CONV_SIMT;
+  return CDS_OK;
+}
+
 int validate(const cds_op& op, Step* out) {
   out->op = op;
   out->branch = (op.flags & CDS_OPF_BRANCH_MASK) >> CDS_OPF_BRANCH_SHIFT;
   switch (op.kind) {
     case CDS_OP_CONV: {
       const cds_conv_op& c = op.u.conv;
-      if (c.batch <= 0 || c.L_in <= 0 || c.L_out <= 0 || c.C_in <= 0 || c.C_out <= 0 || c.taps <= 0 ||
-          c.stride <= 0 || c.phases <= 0)
-        return fail(CDS_ERR_INVALID, "conv: non-positive geometry");
       if (!c.in || !c.w || !c.out) return fail(CDS_ERR_INVALID, "conv: null in/w/out");
-      if (c.groups > 8) return fail(CDS_ERR_UNSUPPORTED, "conv: more than 8 GroupNorm groups");
       if (c.groups > 0 && (!c.gn_gamma || !c.gn_beta)) return fail(CDS_ERR_INVALID, "conv: GroupNorm without affine");
-      if (c.res_w && (!c.res_in || c.res_C <= 0)) return fail(CDS_ERR_INVALID, "conv: shortcut conv without input");
-      if (c.res_w && (c.stride != 1 || c.phases != 1)) return fail(CDS_ERR_INVALID, "conv: shortcut conv needs stride 1");
-      if (c.math == CDS_MATH_BF16_TC || c.math == CDS_MATH_TF32_TC) {
-        if (!cds::conv_tc_eligible(c))
-          return fail(CDS_ERR_INVALID, "conv: op is not eligible for the tensor-core kernel (ask cds_conv_tc_supported)");
-        if (cds::conv_ps_eligible(c)) {
-          if (!cds::conv_ps_prepare(c, &out->psl))
-            return fail(CDS_ERR_CUDA, "conv: cuTensorMapEncodeTiled failed (position-sliced, C_in=%d C_out=%d)", c.C_in, c.C_out);
-          out->tc = out->ps = true;
-          return CDS_OK;
-        }
+      if (c.res_w && !c.res_in) return fail(CDS_ERR_INVALID, "conv: shortcut conv without input");
+      int family = 0;
+      int rc = conv_pick(c, &family, &out->conv_bn);
+      if (rc != CDS_OK) return rc;
+      if (family == CDS_CONV_PS) {
+        if (!cds::conv_ps_prepare(c, &out->psl))
+          return fail(CDS_ERR_CUDA, "conv: cuTensorMapEncodeTiled failed (position-sliced, C_in=%d C_out=%d)", c.C_in, c.C_out);
+        out->tc = out->ps = true;
+      } else if (family == CDS_CONV_TC) {
         if (!cds::conv_tc_prepare(c, &out->tcl))
           return fail(CDS_ERR_CUDA, "conv: cuTensorMapEncodeTiled failed (C_in=%d L=%d C_out=%d)", c.C_in, c.L_in, c.C_out);
         out->tc = true;
-        return CDS_OK;
       }
-      if (c.math != CDS_MATH_FP32) return fail(CDS_ERR_UNSUPPORTED, "conv: math mode %d unknown", c.math);
-      if (c.sample_row_div > 1) return fail(CDS_ERR_UNSUPPORTED, "conv: sample_row_div needs the tensor-core kernel");
-      out->conv_bn = cds::conv_simt_pick_bn(c);
-      if (out->conv_bn == 0)
-        return fail(CDS_ERR_UNSUPPORTED, "conv: GroupNorm tile does not fit (L_out=%d C_out=%d groups=%d)", c.L_out,
-                    c.C_out, c.groups);
       return CDS_OK;
     }
     case CDS_OP_UPDATE: {
@@ -273,6 +286,28 @@ int cds_conv_tc_supported(const cds_conv_op* op) {
   cds_conv_op c = *op;
   if (c.math != CDS_MATH_TF32_TC) c.math = CDS_MATH_BF16_TC;
   return cds::conv_tc_eligible(c) ? 1 : 0;
+}
+
+int cds_conv_choice(const cds_conv_op* op, int32_t info[8]) {
+  if (!op || !info) return fail(CDS_ERR_INVALID, "conv_choice: null argument");
+  const cds_conv_op& c = *op;
+  int family = 0, bn = 0;
+  int rc = conv_pick(c, &family, &bn);
+  if (rc != CDS_OK) return rc;
+  for (int i = 0; i < 8; ++i) info[i] = 0;
+  info[0] = family;
+  if (family == CDS_CONV_TC) {
+    const cds::ConvTcShape s = cds::conv_tc_shape(c);
+    info[1] = s.kc; info[2] = s.n; info[3] = s.split; info[4] = s.col_tiles;
+  } else if (family == CDS_CONV_PS) {
+    info[1] = cds::kPsKC; info[2] = cds::conv_ps_width(c); info[3] = 1; info[4] = 1;
+  } else {
+    info[2] = bn;
+    return CDS_OK;
+  }
+  info[5] = c.res_w ? 1 : 0;
+  info[6] = cds::conv_is_tf32(c) ? 1 : 0;
+  return CDS_OK;
 }
 
 int cds_device_sm_count(int device) {

@@ -1237,30 +1237,43 @@ inline int conv_tc_pick_split(const cds_conv_op& c, int n_total, int m_tiles) {
   return m_tiles < 2 * 132 ? 2 : 1;                  // fewer row tiles than two per SM of an H100 (132 SMs): split
 }
 
+// The instantiation an eligible op runs on: KC, CTA tile width N, SPLIT, and the runtime column tiles of the SPLIT == 1
+// kernels.  conv_tc_prepare and the host query cds_conv_choice both take it from here.
+struct ConvTcShape { int kc, n, split, col_tiles; };
+inline ConvTcShape conv_tc_shape(const cds_conv_op& c) {
+  ConvTcShape s;
+  s.kc = conv_tc_pick_kc(c);
+  const int m_tiles = (int)(((int64_t)c.batch * c.L_out + 127) / 128);
+  const int n_total = conv_tc_width(c);
+  const bool fixed = n_total == 16 || n_total == 32 || n_total == 64 || n_total == 128 || n_total == 256 ||
+                     ((n_total == 512 || n_total == 1024) && c.groups != 0);
+  if (fixed) {
+    s.split = conv_tc_pick_split(c, n_total, m_tiles);
+    s.n = n_total / s.split;
+    s.col_tiles = 1;
+  } else {
+    s.split = 1;
+    s.n = conv_tc_runtime_tile(n_total, s.kc);
+    s.col_tiles = n_total / s.n;
+  }
+  return s;
+}
+
 inline bool conv_tc_prepare(const cds_conv_op& c, ConvTcLaunch* out) {
   ConvTcLaunch& L = *out;
   memset(&L.prm, 0, sizeof(L.prm));
-  const int kc = conv_tc_pick_kc(c);
+  const ConvTcShape shape = conv_tc_shape(c);
+  const int kc = shape.kc;
   const bool tf32 = conv_is_tf32(c);
   const int ke = tf32 ? kc / 2 : kc;                   // channels per chunk
   L.tf32 = tf32;
   ConvTcParams& p = L.prm;
   const int Lp = c.L_out, T = 128 / Lp;
-  const int64_t rows = (int64_t)c.batch * Lp;
-  const int m_tiles = (int)((rows + 127) / 128);
-  const int n_total = conv_tc_width(c);
+  const int m_tiles = (int)(((int64_t)c.batch * Lp + 127) / 128);
   L.kc = kc; L.has_res = c.res_w != nullptr;
-  int col_tiles = 1;                                  // runtime column tiles (SPLIT == 1 kernels)
-  const bool fixed = n_total == 16 || n_total == 32 || n_total == 64 || n_total == 128 || n_total == 256 ||
-                     ((n_total == 512 || n_total == 1024) && c.groups != 0);
-  if (fixed) {
-    L.split = conv_tc_pick_split(c, n_total, m_tiles);
-    L.n = n_total / L.split;
-  } else {
-    L.split = 1;
-    L.n = conv_tc_runtime_tile(n_total, kc);
-    col_tiles = n_total / L.n;
-  }
+  L.split = shape.split;
+  L.n = shape.n;
+  const int col_tiles = shape.col_tiles;              // runtime column tiles (SPLIT == 1 kernels)
   const uint64_t in_b = c.in_batch_mod > 0 ? (uint64_t)c.in_batch_mod : (uint64_t)c.batch;
   {
     uint64_t dims[3] = {(uint64_t)c.C_in, (uint64_t)c.L_in, in_b};

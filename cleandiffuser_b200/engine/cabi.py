@@ -98,7 +98,7 @@ class CdsError(RuntimeError):
 _lib = None
 
 # every symbol include/cds.h declares (tests check that the built library exports all of them)
-EXPORTS = ["cds_version", "cds_op_size", "cds_conv_tc_supported", "cds_last_error", "cds_device_sm_count", "cds_plan_create", "cds_plan_destroy",
+EXPORTS = ["cds_version", "cds_op_size", "cds_conv_tc_supported", "cds_conv_choice", "cds_last_error", "cds_device_sm_count", "cds_plan_create", "cds_plan_destroy",
            "cds_plan_append", "cds_plan_finalize", "cds_plan_run", "cds_plan_run_range", "cds_plan_profile", "cds_plan_launches_per_iter",
            "cds_run_op", "cds_debug_trace"]
 
@@ -122,6 +122,7 @@ def load():
     lib.cds_last_error.restype = C.c_char_p
     lib.cds_device_sm_count.argtypes = [C.c_int]
     lib.cds_conv_tc_supported.argtypes = [C.POINTER(ConvOp)]
+    lib.cds_conv_choice.argtypes = [C.POINTER(ConvOp), C.POINTER(C.c_int32)]
     lib.cds_plan_create.argtypes = [C.c_int, C.POINTER(C.c_void_p)]
     lib.cds_plan_destroy.argtypes = [C.c_void_p]
     lib.cds_plan_append.argtypes = [C.c_void_p, C.POINTER(Op), C.c_int32]
@@ -185,6 +186,21 @@ class Plan:
             self.close()
         except Exception:
             pass
+
+
+CONV_SIMT, CONV_TC, CONV_PS = 0, 1, 2      # cds_conv_choice info[0]
+
+
+def conv_choice(conv: ConvOp):
+    """The kernel the library would run ``conv`` on (cds_conv_choice): a dict with the family ("simt" / "tc" / "ps") and
+    its template parameters.  Raises CdsError if the op would be refused."""
+    info = (C.c_int32 * 8)()
+    check(load().cds_conv_choice(C.byref(conv), info))
+    fam = {CONV_SIMT: "simt", CONV_TC: "tc", CONV_PS: "ps"}[info[0]]
+    if fam == "simt":
+        return {"family": fam, "bn": info[2]}
+    return {"family": fam, "kc": info[1], "n": info[2], "split": info[3], "col_tiles": info[4], "has_res": bool(info[5]),
+            "tf32": bool(info[6])}
 
 
 def run_op(device_index: int, op: Op, it: int, stream: int):

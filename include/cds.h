@@ -210,6 +210,17 @@ int         cds_device_sm_count(int device);
  * bf16 activations).  Pure host logic. */
 int cds_conv_tc_supported(const cds_conv_op* op);
 
+/* kernel families of CDS_OP_CONV (cds_conv_choice info[0]) */
+enum { CDS_CONV_SIMT = 0 /* fp32 CUDA cores, conv_simt.cuh */, CDS_CONV_TC = 1 /* wgmma, conv_tc.cuh */,
+       CDS_CONV_PS = 2 /* wgmma, position-sliced L = 4, conv_ps.cuh */ };
+/* The kernel instantiation cds_plan_append / cds_run_op would choose for `op`.  Pure host logic.  The data pointers in, out and
+ * w (and res_in, gn_gamma, gn_beta, res_bias) may be NULL: only their alignment is read.  res, res_w and the step / sample
+ * parts of bias, scale and shift are presence flags as well: NULL means the operand is absent, which changes the choice.
+ * info[0] = family; CDS_CONV_TC: info[1..6] = KC, N (CTA tile columns), SPLIT, runtime column
+ * tiles, HAS_RES (1x1 shortcut conv), TF32; CDS_CONV_PS: info[1..6] = KC, N, 1, 1, HAS_RES, TF32; CDS_CONV_SIMT: info[2] = BN.
+ * Unused entries are 0.  Returns 0, or the negative cds_status with which the op would be refused. */
+int cds_conv_choice(const cds_conv_op* op, int32_t info[8]);
+
 /* A plan = the per-iteration operator program for one (model, shape, option set) on one device. */
 int cds_plan_create(int device, cds_plan** out);
 int cds_plan_destroy(cds_plan* plan);

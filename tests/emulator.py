@@ -8,7 +8,9 @@ against the same goldens on the H100.  Never imported by the product.
 import ctypes
 
 import numpy as np
+import torch
 
+import opref
 from cleandiffuser_b200.engine import cabi
 
 
@@ -67,99 +69,50 @@ def _vec(v, it, rows, n, row_div=1):
     return out if present else None
 
 
-def _mish(x):
-    sp = np.where(x > 20, x, np.log1p(np.exp(np.minimum(x, 20))))
-    return x * np.tanh(sp)
-
-
-def _act(kind, x):
-    if kind == cabi.ACT_MISH:
-        return _mish(x)
-    if kind == cabi.ACT_SILU:
-        return x / (1 + np.exp(-x))
-    if kind == cabi.ACT_GELU_TANH:
-        return 0.5 * x * (1 + np.tanh(0.7978845608028654 * (x + 0.044715 * x ** 3)))
-    if kind == cabi.ACT_MISH_SILU:
-        m = _mish(x)
-        return m / (1 + np.exp(-m))
-    if kind == cabi.ACT_LEAKY_RELU:
-        return np.where(x > 0, x, 0.01 * x)
-    if kind == cabi.ACT_GELU_ERF:
-        from scipy.special import erf
-        return 0.5 * x * (1 + erf(x * 0.7071067811865476))
-    return x
-
-
-def _tf32_trunc(x):
-    """what wgmma .tf32 sees of an fp32 operand: the low 13 mantissa bits are ignored"""
-    return (np.ascontiguousarray(x, dtype=np.float32).view(np.uint32) & np.uint32(0xFFFFE000)).view(np.float32)
+def _t(a):
+    return None if a is None else torch.from_numpy(np.ascontiguousarray(a))
 
 
 def run_conv(c, it):
+    """CDS_OP_CONV: load the operands of the descriptor and evaluate tests/opref.py's fp64 reference"""
     B, N = c.batch, c.C_out * c.phases
     bmod = c.in_batch_mod if c.in_batch_mod > 0 else B
     xin = _load(c.in_, (bmod, c.L_in, c.C_in), (c.in_bstride, c.in_lstride, 1), c.in_dtype)
-    xin = xin[np.arange(B) % bmod]
     tc = c.math in cabi.TC_MODES
     wdt = cabi.F32 if c.math == cabi.MATH_TF32_TC else cabi.BF16
     if tc:      # bf16 / fp32 [taps][C_out*phases][C_in]
         assert c.in_dtype == wdt or (wdt == cabi.F32 and c.in_dtype == cabi.TF32)
         w = _load(c.w, (c.taps, N, c.C_in), (N * c.C_in, c.C_in, 1), wdt).transpose(0, 2, 1)
-        if c.math == cabi.MATH_TF32_TC:
-            xin, w = _tf32_trunc(xin), _tf32_trunc(w)
     else:
         w = _arr(c.w, (c.taps, c.C_in, N), (c.C_in * N, N, 1))
-    acc = np.zeros((B, c.L_out, N), dtype=np.float64)
-    for tap in range(c.taps):
-        for l in range(c.L_out):
-            pos = l * c.stride + tap - c.pad
-            if 0 <= pos < c.L_in:
-                acc[:, l, :] += xin[:, pos, :].astype(np.float64) @ w[tap].astype(np.float64)
-    y = acc.astype(np.float32)
-    chan = np.arange(N) % c.C_out
     div = c.sample_row_div if c.sample_row_div > 1 else 1
-    bias = _vec(c.bias, it, B, c.C_out, div)
-    if bias is not None:
-        y = y + bias[:, None, chan]
+    kw = dict(bias=_vec(c.bias, it, B, c.C_out, div), scale=_vec(c.scale, it, B, c.C_out, div),
+              shift=_vec(c.shift, it, B, c.C_out, div))
+    kw = {k: _t(v) for k, v in kw.items()}
     if c.groups > 0:
-        assert c.phases == 1
-        g = y.reshape(B, c.L_out, c.groups, c.C_out // c.groups).astype(np.float64)
-        mean = g.mean(axis=(1, 3), keepdims=True)
-        var = g.var(axis=(1, 3), keepdims=True)
-        g = (g - mean) / np.sqrt(var + c.gn_eps)
-        y = g.reshape(B, c.L_out, c.C_out).astype(np.float32)
-        y = y * _arr(c.gn_gamma, (c.C_out,), (1,)) + _arr(c.gn_beta, (c.C_out,), (1,))
-    y = _act(c.act, y.astype(np.float32)).astype(np.float32)
-    scale, shift = _vec(c.scale, it, B, c.C_out, div), _vec(c.shift, it, B, c.C_out, div)
-    if scale is not None:
-        y = y * scale[:, None, chan]
-    if shift is not None:
-        y = y + shift[:, None, chan]
+        kw.update(groups=c.groups, gamma=_t(_arr(c.gn_gamma, (c.C_out,), (1,))), beta=_t(_arr(c.gn_beta, (c.C_out,), (1,))),
+                  eps=c.gn_eps)
     rmod = c.res_batch_mod if c.res_batch_mod > 0 else B
     if c.res:
-        assert c.phases == 1
-        r = _load(c.res, (rmod if c.res_bstride else 1, c.L_out, c.C_out), (c.res_bstride, c.res_lstride, 1), c.res_dtype)
-        y = y + r[(np.arange(B) % rmod) if c.res_bstride else np.zeros(B, dtype=int)]
+        kw["res"] = _t(_load(c.res, (rmod if c.res_bstride else 1, c.L_out, c.C_out), (c.res_bstride, c.res_lstride, 1),
+                             c.res_dtype))
     if c.res_w:
-        rin = _load(c.res_in, (rmod, c.L_out, c.res_C), (c.res_in_bstride, c.res_in_lstride, 1),
-                    c.res_in_dtype)[np.arange(B) % rmod]
-        rw = _load(c.res_w, (c.C_out, c.res_C), (c.res_C, 1), wdt).T if tc else _arr(c.res_w, (c.res_C, N), (N, 1))
-        if c.math == cabi.MATH_TF32_TC:
-            rin, rw = _tf32_trunc(rin), _tf32_trunc(rw)
-        y = y + (rin.astype(np.float64) @ rw.astype(np.float64)).astype(np.float32)
+        kw["res_in"] = _t(_load(c.res_in, (rmod, c.L_out, c.res_C), (c.res_in_bstride, c.res_in_lstride, 1), c.res_in_dtype))
+        kw["res_w"] = _t(_load(c.res_w, (c.C_out, c.res_C), (c.res_C, 1), wdt).T if tc else _arr(c.res_w, (c.res_C, N), (N, 1)))
         if c.res_bias:
-            y = y + _arr(c.res_bias, (c.C_out,), (1,))[chan]
+            kw["res_bias"] = _t(_arr(c.res_bias, (c.C_out,), (1,)))
+    y = opref.conv(_t(xin), _t(w), batch=B, L_out=c.L_out, taps=c.taps, stride=c.stride, pad=c.pad, phases=c.phases,
+                   math_mode=c.math, act_kind=c.act, **kw)
     _store(c.out, (B, c.L_out * c.phases, c.C_out), (c.out_bstride, c.out_lstride, 1), c.out_dtype,
-           y.reshape(B, c.L_out, c.phases, c.C_out).reshape(B, c.L_out * c.phases, c.C_out))
+           y.to(torch.float32).numpy())
 
 
 def run_lnmod(m):
-    x = _arr(m.in_, (m.batch, m.L, m.C), (m.L * m.C, m.C, 1)).astype(np.float64)
-    mu, var = x.mean(-1, keepdims=True), x.var(-1, keepdims=True)
-    n = (x - mu) / np.sqrt(var + m.eps)
-    sh = _arr(m.shift, (m.batch, m.C), (m.mod_bstride, 1))[:, None]
-    sc = _arr(m.scale, (m.batch, m.C), (m.mod_bstride, 1))[:, None]
-    _store(m.out, (m.batch, m.L, m.C), (m.L * m.C, m.C, 1), m.out_dtype, (n * (1 + sc) + sh).astype(np.float32))
+    x = _arr(m.in_, (m.batch, m.L, m.C), (m.L * m.C, m.C, 1))
+    sh = _arr(m.shift, (m.batch, m.C), (m.mod_bstride, 1))
+    sc = _arr(m.scale, (m.batch, m.C), (m.mod_bstride, 1))
+    y = opref.lnmod(_t(x), _t(sh), _t(sc), m.eps)
+    _store(m.out, (m.batch, m.L, m.C), (m.L * m.C, m.C, 1), m.out_dtype, y.to(torch.float32).numpy())
 
 
 def run_attn(a):

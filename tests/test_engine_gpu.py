@@ -219,7 +219,7 @@ def test_sampler_bf16_tensor_cores_goldens(golden, name, monkeypatch):
     assert torch.equal(outs[0], outs[1])         # graph replay == direct launches
 
 
-@pytest.mark.parametrize("math", ["fp32", "bf16"])
+@pytest.mark.parametrize("math", ["fp32", "bf16", "tf32"])
 def test_parallel_branches_give_the_same_bits(math, monkeypatch):
     """CDS_BRANCHES splits the batch into independent kernel chains on parallel streams / graph branches: trajectories are
     independent, so the result must equal the single-chain run bit for bit (graph replay and direct launches)."""
