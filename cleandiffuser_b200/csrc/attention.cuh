@@ -314,18 +314,17 @@ __global__ void __launch_bounds__(128) attention_mma_tf32_hd32_kernel(const cds_
   }
 }
 
-inline cudaError_t attention_launch(const cds_attn_op& p, cudaStream_t st) {
-  int hd = p.C / p.heads;
-  if (p.qkv_dtype == CDS_BF16) {                     // validated: head_dim 32, L <= kAttnMaxL, 16-byte aligned rows
+// family (CDS_ATTN_F32 / _BF16_MMA / _TF32_MMA) and, for the fp32 kernel, HD: as attn_pick (cds_api.cu) chose them
+inline cudaError_t attention_launch(const cds_attn_op& p, int family, int hd, cudaStream_t st) {
+  if (family == CDS_ATTN_BF16_MMA) {
     attention_mma_hd32_kernel<<<dim3(p.batch * p.heads), 128, 0, st>>>(p);
     return cudaGetLastError();
   }
-  // fp32 storage rounded to TF32 (TF32 tensor-core programs): mma.sync tf32 when the shape allows, else the fp32 kernel below
-  if (p.qkv_dtype == CDS_TF32 && hd == 32 && p.L <= kAttnMaxL && p.C % 4 == 0 && ((uintptr_t)p.qkv % 16) == 0 &&
-      p.out_dtype != CDS_BF16 && ((uintptr_t)p.out % 8) == 0) {
+  if (family == CDS_ATTN_TF32_MMA) {
     attention_mma_tf32_hd32_kernel<<<dim3(p.batch * p.heads), 128, 0, st>>>(p);
     return cudaGetLastError();
   }
+  if (family != CDS_ATTN_F32) return cudaErrorInvalidValue;
   size_t smem = sizeof(float) * 2 * (size_t)p.L * hd;
   dim3 grid(p.batch * p.heads);
 #define CDS_ATTN_CASE(HD)                                                                                   \

@@ -11,8 +11,9 @@
 //     swizzle makes all of them bank-conflict free, V needs no transposed copy;
 //   * the normalised 16 x 32 output tile goes through a per-warp 2 KB staging tile and ONE cp.async.bulk.tensor store (full
 //     128-byte lines; rows >= L are clipped by the TMA unit).
-// Same arithmetic as attention_mma_tf32_hd32_kernel (same MMA shapes, same summation order inside a row), so the two agree to
-// rounding of the exp2 arguments only; the k-slot renaming of the P V product is described there.
+// Same arithmetic as attention_mma_tf32_hd32_kernel (same MMA shapes, same summation order inside a row, the same fmaf for
+// every exp2 argument), so the two agree bit for bit unless an exp2 result is subnormal (ex2.approx.ftz here flushes it, exp2f
+// there does not); the k-slot renaming of the P V product is described there.
 // Reference: nn.MultiheadAttention inside DiTBlock, cleandiffuser/nn_diffusion/dit.py:10-36.
 // Algorithmic HBM bytes per (trajectory, head): 4*L*32*3 (q, k, v) + 4*L*32 (out).
 #pragma once
@@ -209,12 +210,15 @@ attention_tma_tf32_hd32_kernel(const cds_attn_op p, const __grid_constant__ CUte
   if (lane == 0) ptx::bulk_wait_group<0>();
 }
 
-inline bool attention_tma_eligible(const cds_attn_op& a) {
+// CDS_ATTN_TMA=0 in the environment (read once per process) sends the ops this kernel would serve to the one-CTA-per-head one
+inline bool attention_tma_enabled() {
   static const bool off = [] { const char* e = getenv("CDS_ATTN_TMA"); return e && e[0] == '0'; }();
-  if (off) return false;
-  const int hd = a.heads > 0 ? a.C / a.heads : 0;
-  return a.qkv_dtype == CDS_TF32 && hd == 32 && a.L <= kAttnMaxL && a.out_dtype != CDS_BF16 && a.C % 4 == 0 &&
-         ((uintptr_t)a.qkv % 16) == 0 && ((uintptr_t)a.out % 16) == 0;
+  return !off;
+}
+
+inline int attention_tma_smem_bytes(int L) {
+  const int LP = (L + 15) & ~15;
+  return kAttnTmaStages * 3 * LP * 128 + kAttnTmaConsumers * 2048 + 1024;
 }
 
 inline bool attention_tma_prepare(const cds_attn_op& a, AttnTmaLaunch* out) {
@@ -232,9 +236,8 @@ inline bool attention_tma_prepare(const cds_attn_op& a, AttnTmaLaunch* out) {
     uint32_t box[3] = {32, 16, 1};
     if (!encode_act_map(&l.tm_out, a.out, 3, dims, str, box, 64, true)) return false;
   }
-  const int LP = (a.L + 15) & ~15;
   l.n_work = a.batch * a.heads;
-  l.smem_bytes = kAttnTmaStages * 3 * LP * 128 + kAttnTmaConsumers * 2048 + 1024;
+  l.smem_bytes = attention_tma_smem_bytes(a.L);
   l.ok = true;
   return true;
 }
@@ -259,14 +262,14 @@ inline cudaError_t attention_tma_preload_all() {
   return cudaSuccess;
 }
 
-inline cudaError_t attention_tma_launch(const cds_attn_op& a, const AttnTmaLaunch& l, int sm_count, cudaStream_t st) {
+inline cudaError_t attention_tma_launch(const cds_attn_op& a, const AttnTmaLaunch& l, int nt, int sm_count, cudaStream_t st) {
   static bool set = false;
   if (!set) {
     cudaError_t e = attention_tma_preload_all();
     if (e != cudaSuccess) return e;
     set = true;
   }
-  AttnTmaKernel k = attention_tma_kernel((a.L + 7) / 8);
+  AttnTmaKernel k = attention_tma_kernel(nt);
   if (!k) return cudaErrorInvalidValue;
   int grid = 2 * (sm_count > 0 ? sm_count : 148);
   if (grid > l.n_work) grid = l.n_work;

@@ -62,6 +62,7 @@ struct Step {            // one validated operator + its kernel choice
   bool skip = false;     // operator folded into another launch by a finalize-time peephole (none at present)
   bool ps = false;       // ... served by the position-sliced kernel (short sequences, conv_ps.cuh)
   cds::ConvPsLaunch psl;
+  int attn_family = 0, attn_param = 0;   // attention: attn_pick's kernel family and template parameter
   cds::AttnTmaLaunch attl;   // TF32 attention: tensor maps of the persistent TMA-fed kernel (attention_tma.cuh)
   // gated Linear directly followed by the LayerNorm+modulate that reads its output: ONE launch of linear_ln_kernel when both
   // operators are in the executed range (the LNMOD step then carries fused_into_prev and is not launched)
@@ -99,6 +100,38 @@ int conv_pick(const cds_conv_op& c, int* family, int* bn) {
     return fail(CDS_ERR_UNSUPPORTED, "conv: GroupNorm tile does not fit (L_out=%d C_out=%d groups=%d)", c.L_out,
                 c.C_out, c.groups);
   *family = CDS_CONV_SIMT;
+  return CDS_OK;
+}
+
+// The kernel family of an attention op (CDS_ATTN_*) and its template parameter (HD of the fp32 kernel, NT = ceil(L / 8) of the
+// TMA kernel, else 0): every check of validate() except the null-pointer ones.  Reads the alignment of qkv and out, never the
+// memory, so that cds_attn_choice answers for descriptors whose buffers do not exist yet.
+int attn_pick(const cds_attn_op& a, int* family, int* param) {
+  if (a.batch <= 0 || a.L <= 0 || a.heads <= 0 || a.C % a.heads != 0) return fail(CDS_ERR_INVALID, "attn: bad arguments");
+  const int hd = a.C / a.heads;
+  if (hd != 16 && hd != 32 && hd != 64) return fail(CDS_ERR_UNSUPPORTED, "attn: head_dim %d", hd);
+  if ((size_t)a.L * hd * 8 > 200 * 1024) return fail(CDS_ERR_UNSUPPORTED, "attn: L=%d too long", a.L);
+  const uintptr_t qkv = (uintptr_t)a.qkv, out = (uintptr_t)a.out;
+  *param = 0;
+  if (a.qkv_dtype == CDS_BF16) {
+    if (hd != 32 || a.L > cds::kAttnMaxL || a.C % 8 != 0 || qkv % 16 != 0)
+      return fail(CDS_ERR_UNSUPPORTED, "attn: bf16 q/k/v needs head_dim 32, L <= %d, 16-byte aligned rows", cds::kAttnMaxL);
+    *family = CDS_ATTN_BF16_MMA;
+    return CDS_OK;
+  }
+  // fp32 storage rounded to TF32 (TF32 tensor-core programs): mma.sync tf32 when the shape allows -- fed by TMA when out is
+  // 16-byte aligned as well --, else the fp32 kernel
+  const bool tf32_mma = a.qkv_dtype == CDS_TF32 && hd == 32 && a.L <= cds::kAttnMaxL && a.C % 4 == 0 && qkv % 16 == 0 &&
+                        a.out_dtype != CDS_BF16 && out % 8 == 0;
+  if (tf32_mma && out % 16 == 0 && cds::attention_tma_enabled()) {
+    *family = CDS_ATTN_TF32_TMA;
+    *param = (a.L + 7) / 8;
+  } else if (tf32_mma) {
+    *family = CDS_ATTN_TF32_MMA;
+  } else {
+    *family = CDS_ATTN_F32;
+    *param = hd;
+  }
   return CDS_OK;
 }
 
@@ -142,14 +175,10 @@ int validate(const cds_op& op, Step* out) {
     }
     case CDS_OP_ATTN: {
       const cds_attn_op& a = op.u.attn;
-      if (a.batch <= 0 || a.L <= 0 || a.heads <= 0 || a.C % a.heads != 0 || !a.qkv || !a.out)
-        return fail(CDS_ERR_INVALID, "attn: bad arguments");
-      int hd = a.C / a.heads;
-      if (hd != 16 && hd != 32 && hd != 64) return fail(CDS_ERR_UNSUPPORTED, "attn: head_dim %d", hd);
-      if ((size_t)a.L * hd * 8 > 200 * 1024) return fail(CDS_ERR_UNSUPPORTED, "attn: L=%d too long", a.L);
-      if (a.qkv_dtype == CDS_BF16 && (hd != 32 || a.L > cds::kAttnMaxL || a.C % 8 != 0 || ((uintptr_t)a.qkv % 16) != 0))
-        return fail(CDS_ERR_UNSUPPORTED, "attn: bf16 q/k/v needs head_dim 32, L <= %d, 16-byte aligned rows", cds::kAttnMaxL);
-      if (cds::attention_tma_eligible(a) && !cds::attention_tma_prepare(a, &out->attl))
+      if (!a.qkv || !a.out) return fail(CDS_ERR_INVALID, "attn: bad arguments");
+      int rc = attn_pick(a, &out->attn_family, &out->attn_param);
+      if (rc != CDS_OK) return rc;
+      if (out->attn_family == CDS_ATTN_TF32_TMA && !cds::attention_tma_prepare(a, &out->attl))
         return fail(CDS_ERR_CUDA, "attn: cuTensorMapEncodeTiled failed (L=%d C=%d)", a.L, a.C);
       return CDS_OK;
     }
@@ -200,8 +229,8 @@ int launch(const Step& s, const int* iter_ptr, int sm_count, cudaStream_t st, in
       return CDS_OK;
     }
     case CDS_OP_ATTN:
-      if (s.attl.ok) CDS_CUDA(cds::attention_tma_launch(s.op.u.attn, s.attl, sm_count, st));
-      else CDS_CUDA(cds::attention_launch(s.op.u.attn, st));
+      if (s.attn_family == CDS_ATTN_TF32_TMA) CDS_CUDA(cds::attention_tma_launch(s.op.u.attn, s.attl, s.attn_param, sm_count, st));
+      else CDS_CUDA(cds::attention_launch(s.op.u.attn, s.attn_family, s.attn_param, st));
       return CDS_OK;
     case CDS_OP_CAST: {
       const cds_cast_op& k = s.op.u.cast;
@@ -307,6 +336,20 @@ int cds_conv_choice(const cds_conv_op* op, int32_t info[8]) {
   }
   info[5] = c.res_w ? 1 : 0;
   info[6] = cds::conv_is_tf32(c) ? 1 : 0;
+  return CDS_OK;
+}
+
+int cds_attn_choice(const cds_attn_op* op, int32_t info[4]) {
+  if (!op || !info) return fail(CDS_ERR_INVALID, "attn_choice: null argument");
+  int family = 0, param = 0;
+  int rc = attn_pick(*op, &family, &param);
+  if (rc != CDS_OK) return rc;
+  const int hd = op->C / op->heads;
+  info[0] = family;
+  info[1] = param;
+  info[2] = hd;
+  info[3] = family == CDS_ATTN_F32 ? (int)(sizeof(float) * 2 * (size_t)op->L * hd)
+          : family == CDS_ATTN_TF32_TMA ? cds::attention_tma_smem_bytes(op->L) : 0;
   return CDS_OK;
 }
 

@@ -98,7 +98,7 @@ class CdsError(RuntimeError):
 _lib = None
 
 # every symbol include/cds.h declares (tests check that the built library exports all of them)
-EXPORTS = ["cds_version", "cds_op_size", "cds_conv_tc_supported", "cds_conv_choice", "cds_last_error", "cds_device_sm_count", "cds_plan_create", "cds_plan_destroy",
+EXPORTS = ["cds_version", "cds_op_size", "cds_conv_tc_supported", "cds_conv_choice", "cds_attn_choice", "cds_last_error", "cds_device_sm_count", "cds_plan_create", "cds_plan_destroy",
            "cds_plan_append", "cds_plan_finalize", "cds_plan_run", "cds_plan_run_range", "cds_plan_profile", "cds_plan_launches_per_iter",
            "cds_run_op", "cds_debug_trace"]
 
@@ -123,6 +123,7 @@ def load():
     lib.cds_device_sm_count.argtypes = [C.c_int]
     lib.cds_conv_tc_supported.argtypes = [C.POINTER(ConvOp)]
     lib.cds_conv_choice.argtypes = [C.POINTER(ConvOp), C.POINTER(C.c_int32)]
+    lib.cds_attn_choice.argtypes = [C.POINTER(AttnOp), C.POINTER(C.c_int32)]
     lib.cds_plan_create.argtypes = [C.c_int, C.POINTER(C.c_void_p)]
     lib.cds_plan_destroy.argtypes = [C.c_void_p]
     lib.cds_plan_append.argtypes = [C.c_void_p, C.POINTER(Op), C.c_int32]
@@ -201,6 +202,19 @@ def conv_choice(conv: ConvOp):
         return {"family": fam, "bn": info[2]}
     return {"family": fam, "kc": info[1], "n": info[2], "split": info[3], "col_tiles": info[4], "has_res": bool(info[5]),
             "tf32": bool(info[6])}
+
+
+ATTN_F32, ATTN_BF16_MMA, ATTN_TF32_MMA, ATTN_TF32_TMA = 0, 1, 2, 3     # cds_attn_choice info[0]
+
+
+def attn_choice(attn: AttnOp):
+    """The kernel the library would run ``attn`` on (cds_attn_choice): a dict with the family ("f32" / "bf16_mma" /
+    "tf32_mma" / "tma"), its template parameter (HD of "f32", NT of "tma", else 0), the head dim and the dynamic shared
+    memory of the launch.  Raises CdsError if the op would be refused."""
+    info = (C.c_int32 * 4)()
+    check(load().cds_attn_choice(C.byref(attn), info))
+    fam = {ATTN_F32: "f32", ATTN_BF16_MMA: "bf16_mma", ATTN_TF32_MMA: "tf32_mma", ATTN_TF32_TMA: "tma"}[info[0]]
+    return {"family": fam, "param": info[1], "hd": info[2], "smem": info[3]}
 
 
 def run_op(device_index: int, op: Op, it: int, stream: int):

@@ -116,14 +116,10 @@ def run_lnmod(m):
 
 
 def run_attn(a):
-    hd = a.C // a.heads
-    qkv = _load(a.qkv, (a.batch, a.L, 3, a.heads, hd), (a.L * 3 * a.C, 3 * a.C, a.C, hd, 1), a.qkv_dtype).astype(np.float64)
-    q, k, v = (qkv[:, :, i].transpose(0, 2, 1, 3) for i in range(3))        # (b, h, L, hd)
-    s = q @ k.transpose(0, 1, 3, 2) / np.sqrt(hd)
-    s = np.exp(s - s.max(-1, keepdims=True))
-    s /= s.sum(-1, keepdims=True)
-    o = (s @ v).transpose(0, 2, 1, 3).reshape(a.batch, a.L, a.C)
-    _store(a.out, (a.batch, a.L, a.C), (a.L * a.C, a.C, 1), a.out_dtype, o.astype(np.float32))
+    """CDS_OP_ATTN: load q|k|v (bf16 values widened exactly) and evaluate tests/opref.py's fp64 reference"""
+    qkv = _load(a.qkv, (a.batch, a.L, 3 * a.C), (a.L * 3 * a.C, 3 * a.C, 1), a.qkv_dtype)
+    o = opref.attn(_t(qkv), a.heads, a.qkv_dtype)
+    _store(a.out, (a.batch, a.L, a.C), (a.L * a.C, a.C, 1), a.out_dtype, o.to(torch.float32).numpy())
 
 
 def run_cast(k):
@@ -174,9 +170,9 @@ def run_update(u, it):
             if k4 != 0 and u.xhat_prev and u.aux:
                 _arr(u.xhat_prev, (u.batch, u.row), (u.row, 1))[...] = x
                 _arr(u.aux, (u.batch, u.row), (u.row, 1))[...] = slope
-        else:
-            hist = _arr(u.xhat_prev, (u.batch, u.row), (u.row, 1))
-            aux = _arr(u.aux, (u.batch, u.row), (u.row, 1))
+        else:                               # (absent history buffers read as 0, as in the kernel)
+            hist = _arr(u.xhat_prev, (u.batch, u.row), (u.row, 1)) if u.xhat_prev else f(0)
+            aux = _arr(u.aux, (u.batch, u.row), (u.row, 1)) if u.aux else f(0)
             out = hist - (aux + slope) / f(2) * k2
     elif kind == 5:
         out = k0 * x + k1 * pr
@@ -206,7 +202,7 @@ def run_update(u, it):
             out = k0 * ((x - sigma * eps) / alpha) + k1 * eps
         else:
             hist = _arr(u.xhat_prev, (u.batch, u.row), (u.row, 1)) if u.xhat_prev else None
-            target = eps if kind == 2 else (k3 * xhat - k4 * hist if kind == 4 else xhat)
+            target = eps if kind == 2 else (k3 * xhat - k4 * (hist if hist is not None else f(0)) if kind == 4 else xhat)
             out = k0 * x - k1 * target
             if z is not None:
                 out = out + k2 * z

@@ -141,6 +141,19 @@ def conv(x, w, *, batch, L_out, taps=1, stride=1, pad=0, phases=1, math_mode=cab
     return out
 
 
+def attn(qkv, heads, qkv_dtype=cabi.F32):
+    """CDS_OP_ATTN in fp64: softmax(q k^T / sqrt(hd)) v per (trajectory, head), (batch, L, C).  qkv (batch, L, 3C) with
+    [q | k | v] column blocks, read as stored: bf16 values, or fp32 as is (a CDS_TF32 tensor already holds TF32 values)."""
+    B, L, C3 = qkv.shape
+    C = C3 // 3
+    hd = C // heads
+    if qkv_dtype == cabi.BF16:
+        qkv = qkv.to(torch.bfloat16)
+    q, k, v = (t.to(F64).reshape(B, L, heads, hd).transpose(1, 2) for t in qkv.split(C, dim=-1))   # (B, heads, L, hd)
+    p = torch.softmax(q @ k.transpose(-1, -2) / math.sqrt(hd), dim=-1)
+    return (p @ v).transpose(1, 2).reshape(B, L, C)
+
+
 def lnmod(x, shift, scale, eps, *, L=1):
     """CDS_OP_LNMOD in fp64: LayerNorm(x) (two-pass statistics, no affine) * (1 + scale) + shift.  x (rows, C) or (batch, L, C);
     shift / scale (batch, C), one vector per trajectory = per L rows of a (rows, C) x."""
