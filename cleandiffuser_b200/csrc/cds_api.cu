@@ -15,6 +15,7 @@
 #include "attention_tma.cuh"
 #include "linear_ln.cuh"
 #include "elementwise.cuh"
+#include "mha.cuh"
 
 namespace {
 
@@ -63,6 +64,7 @@ struct Step {            // one validated operator + its kernel choice
   bool ps = false;       // ... served by the position-sliced kernel (short sequences, conv_ps.cuh)
   cds::ConvPsLaunch psl;
   int attn_family = 0, attn_param = 0;   // attention: attn_pick's kernel family and template parameter
+  int mha_hpl = 0;       // CDS_OP_MHA: head_dim / 32 (mha_pick)
   cds::AttnTmaLaunch attl;   // TF32 attention: tensor maps of the persistent TMA-fed kernel (attention_tma.cuh)
   // gated Linear directly followed by the LayerNorm+modulate that reads its output: ONE launch of linear_ln_kernel when both
   // operators are in the executed range (the LNMOD step then carries fused_into_prev and is not launched)
@@ -135,6 +137,22 @@ int attn_pick(const cds_attn_op& a, int* family, int* param) {
   return CDS_OK;
 }
 
+bool is_act_dtype(int d) { return d == CDS_F32 || d == CDS_TF32 || d == CDS_BF16; }
+
+// The instantiation of mha_f32_kernel for a CDS_OP_MHA op: every check of validate() except the null-pointer ones, so that
+// cds_mha_choice answers for descriptors whose buffers do not exist yet.
+int mha_pick(const cds_mha_op& m, int* hpl) {
+  if (m.batch <= 0 || m.Lq <= 0 || m.Lk <= 0 || m.heads <= 0 || m.C <= 0 || m.C % m.heads != 0)
+    return fail(CDS_ERR_INVALID, "mha: bad arguments");
+  if (!is_act_dtype(m.in_dtype) || !is_act_dtype(m.out_dtype)) return fail(CDS_ERR_INVALID, "mha: unknown dtype");
+  const int hd = m.C / m.heads;
+  if (hd % 32 != 0 || hd > 32 * cds::kMhaMaxHPL) return fail(CDS_ERR_UNSUPPORTED, "mha: head_dim %d", hd);
+  if (m.Lq > cds::kMhaMaxL || m.Lk > cds::kMhaMaxL)
+    return fail(CDS_ERR_UNSUPPORTED, "mha: Lq=%d Lk=%d (at most %d)", m.Lq, m.Lk, cds::kMhaMaxL);
+  *hpl = hd / 32;
+  return CDS_OK;
+}
+
 int validate(const cds_op& op, Step* out) {
   out->op = op;
   out->branch = (op.flags & CDS_OPF_BRANCH_MASK) >> CDS_OPF_BRANCH_SHIFT;
@@ -181,6 +199,11 @@ int validate(const cds_op& op, Step* out) {
       if (out->attn_family == CDS_ATTN_TF32_TMA && !cds::attention_tma_prepare(a, &out->attl))
         return fail(CDS_ERR_CUDA, "attn: cuTensorMapEncodeTiled failed (L=%d C=%d)", a.L, a.C);
       return CDS_OK;
+    }
+    case CDS_OP_MHA: {
+      const cds_mha_op& m = op.u.mha;
+      if (!m.q || (!m.kv_step && !m.kv_sample) || !m.out) return fail(CDS_ERR_INVALID, "mha: null q, k|v or out");
+      return mha_pick(m, &out->mha_hpl);
     }
     case CDS_OP_PREP: {
       const cds_prep_op& p = op.u.prep;
@@ -232,6 +255,9 @@ int launch(const Step& s, const int* iter_ptr, int sm_count, cudaStream_t st, in
       if (s.attn_family == CDS_ATTN_TF32_TMA) CDS_CUDA(cds::attention_tma_launch(s.op.u.attn, s.attl, s.attn_param, sm_count, st));
       else CDS_CUDA(cds::attention_launch(s.op.u.attn, s.attn_family, s.attn_param, st));
       return CDS_OK;
+    case CDS_OP_MHA:
+      CDS_CUDA(cds::mha_launch(s.op.u.mha, s.mha_hpl, iter_ptr, st));
+      return CDS_OK;
     case CDS_OP_CAST: {
       const cds_cast_op& k = s.op.u.cast;
       cds::cast_pad_kernel<<<elementwise_grid((int64_t)k.batch * k.L * (k.C_out / 2), sm_count), 256, 0, st>>>(k);
@@ -256,6 +282,7 @@ int preload_kernels() {
   CDS_CUDA(cudaFuncGetAttributes(&a, cds::attention_mma_hd32_kernel));
   CDS_CUDA(cudaFuncGetAttributes(&a, cds::attention_mma_tf32_hd32_kernel));
   CDS_CUDA(cds::attention_tma_preload_all());
+  CDS_CUDA(cds::mha_preload_all());
   CDS_CUDA(cds::linear_ln_preload_all());
   CDS_CUDA(cudaFuncGetAttributes(&a, cds::solver_update_kernel));
   CDS_CUDA(cudaFuncGetAttributes(&a, cds::cm_prep_kernel));
@@ -281,6 +308,9 @@ long long* conv_tc_trace_hook(int grid) {
   return g_trace_buf;
 }
 }  // namespace cds
+
+// CDS_OP_MHA was added without a layout change: the union keeps its size
+static_assert(sizeof(cds_mha_op) <= sizeof(cds_conv_op), "cds_mha_op must not grow the cds_op union");
 
 struct cds_plan {
   int device = 0;
@@ -350,6 +380,16 @@ int cds_attn_choice(const cds_attn_op* op, int32_t info[4]) {
   info[2] = hd;
   info[3] = family == CDS_ATTN_F32 ? (int)(sizeof(float) * 2 * (size_t)op->L * hd)
           : family == CDS_ATTN_TF32_TMA ? cds::attention_tma_smem_bytes(op->L) : 0;
+  return CDS_OK;
+}
+
+int cds_mha_choice(const cds_mha_op* op, int32_t info[2]) {
+  if (!op || !info) return fail(CDS_ERR_INVALID, "mha_choice: null argument");
+  int hpl = 0;
+  int rc = mha_pick(*op, &hpl);
+  if (rc != CDS_OK) return rc;
+  info[0] = hpl;
+  info[1] = op->in_dtype == CDS_BF16 ? 1 : 0;
   return CDS_OK;
 }
 

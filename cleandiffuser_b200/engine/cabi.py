@@ -13,7 +13,7 @@ _LIB_PATH = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file_
 ABI_VERSION = 5
 OPF_BRANCH_SHIFT = 8   # cds_op.flags bits 8..15: branch index (independent chains run on parallel streams)
 OPF_ONCE = 1          # cds_op.flags: run once per plan run (before its first iteration), not in every iteration
-OP_CONV, OP_UPDATE, OP_LNMOD, OP_ATTN, OP_PREP, OP_CAST = range(6)
+OP_CONV, OP_UPDATE, OP_LNMOD, OP_ATTN, OP_PREP, OP_CAST, OP_MHA = range(7)
 ACT_NONE, ACT_MISH, ACT_SILU, ACT_GELU_TANH, ACT_MISH_SILU, ACT_LEAKY_RELU, ACT_GELU_ERF = range(7)
 MATH_FP32, MATH_BF16_TC, MATH_TF32_TC = 0, 1, 2
 TC_MODES = (MATH_BF16_TC, MATH_TF32_TC)
@@ -59,6 +59,16 @@ class AttnOp(C.Structure):
                 ("qkv", _f32p), ("out", C.c_void_p), ("out_dtype", C.c_int32), ("qkv_dtype", C.c_int32)]
 
 
+class MhaOp(C.Structure):
+    _fields_ = [("batch", C.c_int32), ("Lq", C.c_int32), ("Lk", C.c_int32), ("C", C.c_int32), ("heads", C.c_int32),
+                ("masked", C.c_int32), ("diag", C.c_int32),
+                ("q", C.c_void_p), ("q_bstride", C.c_int64), ("q_lstride", C.c_int32),
+                ("kv_step", C.c_void_p), ("kv_step_stride", C.c_int64), ("kv_step_lstride", C.c_int32),
+                ("kv_sample", C.c_void_p), ("kv_sample_bstride", C.c_int64), ("kv_sample_lstride", C.c_int32),
+                ("out", C.c_void_p), ("out_bstride", C.c_int64), ("out_lstride", C.c_int32),
+                ("in_dtype", C.c_int32), ("out_dtype", C.c_int32)]
+
+
 class PrepOp(C.Structure):
     _fields_ = [("batch", C.c_int32), ("row", C.c_int32), ("x", _f32p), ("xin", _f32p), ("noise", _f32p),
                 ("coef", _f32p)]
@@ -82,7 +92,7 @@ class UpdateOp(C.Structure):
 
 class _OpUnion(C.Union):
     _fields_ = [("conv", ConvOp), ("update", UpdateOp), ("lnmod", LnModOp), ("attn", AttnOp), ("prep", PrepOp),
-                ("cast", CastOp)]
+                ("cast", CastOp), ("mha", MhaOp)]
 
 
 class Op(C.Structure):
@@ -98,7 +108,7 @@ class CdsError(RuntimeError):
 _lib = None
 
 # every symbol include/cds.h declares (tests check that the built library exports all of them)
-EXPORTS = ["cds_version", "cds_op_size", "cds_conv_tc_supported", "cds_conv_choice", "cds_attn_choice", "cds_last_error", "cds_device_sm_count", "cds_plan_create", "cds_plan_destroy",
+EXPORTS = ["cds_version", "cds_op_size", "cds_conv_tc_supported", "cds_conv_choice", "cds_attn_choice", "cds_mha_choice", "cds_last_error", "cds_device_sm_count", "cds_plan_create", "cds_plan_destroy",
            "cds_plan_append", "cds_plan_finalize", "cds_plan_run", "cds_plan_run_range", "cds_plan_profile", "cds_plan_launches_per_iter",
            "cds_run_op", "cds_debug_trace"]
 
@@ -124,6 +134,7 @@ def load():
     lib.cds_conv_tc_supported.argtypes = [C.POINTER(ConvOp)]
     lib.cds_conv_choice.argtypes = [C.POINTER(ConvOp), C.POINTER(C.c_int32)]
     lib.cds_attn_choice.argtypes = [C.POINTER(AttnOp), C.POINTER(C.c_int32)]
+    lib.cds_mha_choice.argtypes = [C.POINTER(MhaOp), C.POINTER(C.c_int32)]
     lib.cds_plan_create.argtypes = [C.c_int, C.POINTER(C.c_void_p)]
     lib.cds_plan_destroy.argtypes = [C.c_void_p]
     lib.cds_plan_append.argtypes = [C.c_void_p, C.POINTER(Op), C.c_int32]
@@ -215,6 +226,14 @@ def attn_choice(attn: AttnOp):
     check(load().cds_attn_choice(C.byref(attn), info))
     fam = {ATTN_F32: "f32", ATTN_BF16_MMA: "bf16_mma", ATTN_TF32_MMA: "tf32_mma", ATTN_TF32_TMA: "tma"}[info[0]]
     return {"family": fam, "param": info[1], "hd": info[2], "smem": info[3]}
+
+
+def mha_choice(mha: MhaOp):
+    """The instantiation the library would run ``mha`` on (cds_mha_choice): a dict with ``hpl`` (head_dim / 32, the template
+    parameter of mha_f32_kernel) and ``bf16`` (q / k / v read as bf16).  Raises CdsError if the op would be refused."""
+    info = (C.c_int32 * 2)()
+    check(load().cds_mha_choice(C.byref(mha), info))
+    return {"hpl": info[0], "bf16": bool(info[1])}
 
 
 def run_op(device_index: int, op: Op, it: int, stream: int):

@@ -19,6 +19,9 @@ What is hoisted out of the iteration loop (SURVEY 8a quirk 5):
   DQLMlp                     : the first Linear over cat[x, time_mlp(t), obs] splits the same way.
   DiT1d / Janner + condition : map_emb(map_noise(t) + cond) is nonlinear in the sum -> small per-trajectory
                                GEMMs stay inside the iteration (0.5 % of the FLOPs).
+  ChiTransformer             : the cross-attention memory is encoder(token + position) per token: token 0 (the time) depends
+                               on the iteration only, tokens 1..To (the observations) on the trajectory only -> every layer's
+                               cross-attention keys / values are a per-iteration table plus a per-trajectory table.
 """
 import ctypes as C
 from typing import Callable, List, Optional
@@ -299,6 +302,25 @@ class Program:
         m.in_, m.out, m.out_dtype = x.ptr, out.ptr, out.dtype
         m.shift, m.scale = mod.data_ptr() + 4 * int(shift_col), mod.data_ptr() + 4 * int(scale_col)
         m.mod_bstride = mod.stride(0)
+        self.ops.append(op)
+
+    def mha(self, q: View, kv_step: Optional[View], kv_sample: Optional[View], out: View, heads: int,
+            diag: Optional[int] = None):
+        """CDS_OP_MHA.  kv_step: (n_iters, Lk, 2C) view (bstride = the iteration stride), kv_sample: (rows, Lk, 2C) view, either
+        may be None; diag: key j is visible to query i iff j <= i + diag, None = no mask."""
+        kv = kv_sample if kv_sample is not None else kv_step
+        op = cabi.Op()
+        op.kind = cabi.OP_MHA
+        m = op.u.mha
+        m.batch, m.Lq, m.Lk, m.C, m.heads = self.rows, q.L, kv.L, q.C, int(heads)
+        m.masked, m.diag = (0, 0) if diag is None else (1, int(diag))
+        m.q, m.q_bstride, m.q_lstride = q.ptr, q.bstride, q.lstride
+        if kv_step is not None:
+            m.kv_step, m.kv_step_stride, m.kv_step_lstride = kv_step.ptr, kv_step.bstride, kv_step.lstride
+        if kv_sample is not None:
+            m.kv_sample, m.kv_sample_bstride, m.kv_sample_lstride = kv_sample.ptr, kv_sample.bstride, kv_sample.lstride
+        m.out, m.out_bstride, m.out_lstride = out.ptr, out.bstride, out.lstride
+        m.in_dtype, m.out_dtype = q.dtype, out.dtype
         self.ops.append(op)
 
     def attn(self, qkv: View, out: View, heads: int):
@@ -729,6 +751,19 @@ def cabi_vec2(step: torch.Tensor, sample: torch.Tensor, sample_col: int) -> cabi
 
 
 # =============================================================================== DiT1d
+def _embed_tokens(p: Program, x: View, lin: nn.Linear, pos: View, X: View, in_batch_mod: int):
+    """X = lin(x_t) + pos (a (L, d) table broadcast over the batch)."""
+    L = X.L
+    if p.tc and x.t.dtype == torch.float32 and x.lstride == x.C and x.bstride == L * x.C:
+        # x_t enters as a channel-padded copy in the activation dtype (kept fresh by the solver update, like the UNets' hand-over)
+        kin = p.k_align * ((x.C + p.k_align - 1) // p.k_align)
+        xb = p.cast_pad(x, kin, rows=in_batch_mod or p.rows)
+        w_in = w_rows(lambda: F.pad(lin.weight, (0, kin - lin.weight.shape[1])))
+        p.token_linear(xb, w_in, X, bias=_const_vec(p.packed(lambda: lin.bias)), res=pos, in_batch_mod=in_batch_mod)
+    else:
+        p.conv(x, w_linear(lin.weight), X, bias=_const_vec(p.packed(lambda: lin.bias)), res=pos, in_batch_mod=in_batch_mod)
+
+
 def lower_dit(p: Program, net: nn.Module, x: View, horizon: int, has_cond: bool, in_batch_mod: int) -> View:
     d = net.d_model
     depth = len(net.blocks)
@@ -772,16 +807,7 @@ def lower_dit(p: Program, net: nn.Module, x: View, horizon: int, has_cond: bool,
     # head_dim 32 (every pipeline) and L <= 128: attention runs on tensor cores (mma.sync, bf16 q/k/v); otherwise fp32 CUDA cores
     QKV = p.act(L, 3 * d) if (d // heads == 32 and L <= 128) else p.act(L, 3 * d, f32)
     Y, ATT, HID = p.act(L, d), p.act(L, d), p.act(L, 4 * d)
-    if p.tc and x.t.dtype == torch.float32 and x.lstride == x.C and x.bstride == L * x.C:
-        # x_t enters as a channel-padded copy in the activation dtype (kept fresh by the solver update, like the UNets' hand-over)
-        kin = p.k_align * ((x.C + p.k_align - 1) // p.k_align)
-        xb = p.cast_pad(x, kin, rows=in_batch_mod or p.rows)
-        w_in = w_rows(lambda: F.pad(net.x_proj.weight, (0, kin - net.x_proj.weight.shape[1])))
-        p.token_linear(xb, w_in, X, bias=_const_vec(p.packed(lambda: net.x_proj.bias)),
-                       res=View(pos, L, d, bstride=0), in_batch_mod=in_batch_mod)
-    else:
-        p.conv(x, w_linear(net.x_proj.weight), X, bias=_const_vec(p.packed(lambda: net.x_proj.bias)),
-               res=View(pos, L, d, bstride=0), in_batch_mod=in_batch_mod)
+    _embed_tokens(p, x, net.x_proj, View(pos, L, d, bstride=0), X, in_batch_mod)
     for i, blk in enumerate(net.blocks):
         o = 6 * d * i       # chunk order: shift_msa, scale_msa, gate_msa, shift_mlp, scale_mlp, gate_mlp
         p.lnmod(X, Y, mod2d, o, o + d, blk.norm1.eps)
@@ -803,6 +829,83 @@ def lower_dit(p: Program, net: nn.Module, x: View, horizon: int, has_cond: bool,
     return p.token_linear(Y, w_linear(fl.linear.weight), out, bias=_const_vec(p.packed(lambda: fl.linear.bias)))
 
 
+# =============================================================================== ChiTransformer
+def _layernorm(p: Program, ln: nn.LayerNorm, x: View, out: View):
+    """Affine nn.LayerNorm as CDS_OP_LNMOD: LN(x) * (1 + (gamma - 1)) + beta, the same vectors for every trajectory."""
+    mod = p.packed(lambda: torch.cat([ln.weight - 1., ln.bias]))
+    p.lnmod(x, out, mod.expand(p.rows, 2 * x.C), x.C, 0, ln.eps)
+
+
+def lower_chitransformer(p: Program, net: nn.Module, x: View, horizon: int, has_cond: bool, in_batch_mod: int) -> View:
+    """chitransformer.py.  Per decoder layer (norm_first): LN -> QKV Linear -> causal CDS_OP_MHA -> out-projection onto the
+    residual stream; LN -> Q Linear -> CDS_OP_MHA over the memory (mask t >= s - 1) -> out-projection; LN -> Linear + exact
+    GELU -> Linear.  The memory's keys / values never enter the loop: token 0 = encoder(map_noise(t) + cond_pos_emb[0]) is a
+    per-iteration row, tokens 1..To = encoder(obs_emb(cond) + cond_pos_emb[1:]) are per-trajectory rows, each projected by
+    every layer's K / V weights once per sample() call into [n_iters | rows, layers, 1 + To, 2 d] tables (the other part's
+    rows are zero, so the operator's step + sample sum picks each token from its own table)."""
+    from ..nn_diffusion.chitransformer import causal_mask, memory_mask
+    if not isinstance(net.encoder, nn.Sequential):
+        raise Unsupported("ChiTransformer(n_cond_layers > 0)")
+    layers = list(net.decoder.layers)
+    if net.training and (net.drop.p > 0 or any(l.dropout.p > 0 for l in layers)):
+        raise Unsupported("ChiTransformer in train mode (dropout)")
+    if net.decoder.norm is not None or any(not l.norm_first or l.activation is not F.gelu for l in layers):
+        raise Unsupported("ChiTransformer decoder other than norm_first with exact GELU")
+    To, L = net.To, horizon
+    if net.mask.shape != (L, L) or not torch.equal(net.mask.detach().cpu(), causal_mask(L)) or \
+            not torch.equal(net.memory_mask.detach().cpu(), memory_mask(L, To)):
+        raise Unsupported("ChiTransformer with other attention masks or horizon != Ta")
+    d, heads, Lk, n = net.pos_emb.shape[2], layers[0].self_attn.num_heads, 1 + To, len(layers)
+    obs_dim, R = net.obs_dim, p.rows
+    xattn = [l.multihead_attn for l in layers]
+
+    kv_step = p.buf(p.n_iters, n, Lk, 2 * d, dtype=p.act_dtype)
+    kv_samp = p.buf(R, n, Lk, 2 * d, dtype=p.act_dtype)
+
+    def kv_of(m, a):                        # memory tokens -> [k | v] of one layer's cross-attention
+        return F.linear(m, a.in_proj_weight[d:], a.in_proj_bias[d:])
+
+    def fill_step(ctx):
+        m0 = net.encoder(net.map_noise(ctx.t_all) + net.cond_pos_emb[0, 0])
+        kv_step[:, :, 0].copy_(torch.stack([kv_of(m0, a) for a in xattn], 1))
+    fill_step.time_only = True
+    p.per_call.append(fill_step)
+
+    def fill_samp(ctx):
+        c = ctx.cond_rows
+        c = torch.zeros(R, To * obs_dim, device=kv_samp.device) if c is None else c.reshape(R, To * obs_dim)
+
+        def per_traj(rows):
+            m = net.encoder(net.obs_emb(rows.view(-1, To, obs_dim)) + net.cond_pos_emb[0, 1:])
+            return torch.stack([kv_of(m, a) for a in xattn], 1)
+        kv_samp[:, :, 1:].copy_(_fixed_shape_rows(per_traj, c))
+    p.per_call.append(fill_samp)
+
+    f32 = torch.float32
+    X = p.act(L, d, f32)                     # the residual stream stays exact fp32
+    Y, Q, ATT, QKV, HID = p.act(L, d), p.act(L, d), p.act(L, d), p.act(L, 3 * d), p.act(L, 4 * d)
+    pos = p.packed(lambda: net.pos_emb[0, :L])
+    _embed_tokens(p, x, net.act_emb, View(pos, L, d, bstride=0), X, in_batch_mod)
+    bias = lambda get: _const_vec(p.packed(get))     # noqa: E731
+    for i, layer in enumerate(layers):
+        sa, xa = layer.self_attn, layer.multihead_attn
+        _layernorm(p, layer.norm1, X, Y)
+        p.token_linear(Y, w_linear(sa.in_proj_weight), QKV, bias=bias(lambda a=sa: a.in_proj_bias))
+        p.mha(QKV.channels(0, d), None, QKV.channels(d, 2 * d), ATT, heads, diag=0)
+        p.token_linear(ATT, w_linear(sa.out_proj.weight), X, bias=bias(lambda a=sa: a.out_proj.bias), res=X)
+        _layernorm(p, layer.norm2, X, Y)
+        p.token_linear(Y, w_rows(lambda a=xa: a.in_proj_weight[:d]), Q, bias=bias(lambda a=xa: a.in_proj_bias[:d]))
+        at = i * Lk * 2 * d
+        p.mha(Q, View(kv_step, Lk, 2 * d, at, n * Lk * 2 * d), View(kv_samp, Lk, 2 * d, at, n * Lk * 2 * d), ATT, heads, diag=1)
+        p.token_linear(ATT, w_linear(xa.out_proj.weight), X, bias=bias(lambda a=xa: a.out_proj.bias), res=X)
+        _layernorm(p, layer.norm3, X, Y)
+        p.token_linear(Y, w_linear(layer.linear1.weight), HID, bias=bias(lambda m=layer: m.linear1.bias), act=cabi.ACT_GELU_ERF)
+        p.token_linear(HID, w_linear(layer.linear2.weight), X, bias=bias(lambda m=layer: m.linear2.bias), res=X)
+    _layernorm(p, net.ln_f, X, Y)
+    out = p.act(L, net.head.out_features, f32)
+    return p.token_linear(Y, w_linear(net.head.weight), out, bias=bias(lambda: net.head.bias))
+
+
 def lower_denoiser(p: Program, net: nn.Module, x: View, x_shape, has_cond: bool, in_batch_mod: int) -> View:
     """Dispatch on the backbone type (reference instances are recognised structurally by class name)."""
     name = type(net).__name__
@@ -815,6 +918,8 @@ def lower_denoiser(p: Program, net: nn.Module, x: View, x_shape, has_cond: bool,
         return lower_chi(p, net, x, x_shape[0], has_cond, in_batch_mod)
     if name == "DiT1d" and len(x_shape) == 2:
         return lower_dit(p, net, x, x_shape[0], has_cond, in_batch_mod)
+    if name == "ChiTransformer" and len(x_shape) == 2:
+        return lower_chitransformer(p, net, x, x_shape[0], has_cond, in_batch_mod)
     if name == "DQLMlp" and len(x_shape) == 1:
         return lower_dql(p, net, x, has_cond, in_batch_mod)
     if name == "DVInvMlp" and len(x_shape) == 1:

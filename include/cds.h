@@ -19,6 +19,8 @@
  *   CDS_OP_CAST         x.permute(0,2,1) entry of the UNets (jannerunet.py:169, chiunet.py:142): layout/dtype hand-over of x_t
  *   CDS_OP_UPDATE       CFG combine, clip_prediction, eps<->x0 conversion, the 8 solver updates, fix_mask
  *                       (diffusionsde.py:202,208-223,539-592) and the CM skip/out combine (consistency_model.py:257-262)
+ *   CDS_OP_MHA          the attention core of nn.TransformerDecoderLayer's causal self-attention and masked cross-attention
+ *                       (chitransformer.py: decoder with tgt_mask / memory_mask), q and k|v from separate strided sources
  *
  * Conventions
  *  - every function returns 0 on success, a negative cds_status otherwise; cds_last_error() gives the
@@ -56,7 +58,7 @@ typedef enum cds_status {
 } cds_status;
 
 typedef enum cds_op_kind { CDS_OP_CONV = 0, CDS_OP_UPDATE = 1, CDS_OP_LNMOD = 2, CDS_OP_ATTN = 3, CDS_OP_PREP = 4,
-                           CDS_OP_CAST = 5 } cds_op_kind;
+                           CDS_OP_CAST = 5, CDS_OP_MHA = 6 } cds_op_kind;
 typedef enum cds_act { CDS_ACT_NONE = 0, CDS_ACT_MISH = 1, CDS_ACT_SILU = 2, CDS_ACT_GELU_TANH = 3,
                        CDS_ACT_MISH_SILU = 4 /* silu(mish(x)): DiT's map_emb tail feeding every adaLN (dit.py:26,43,71) */,
                        CDS_ACT_LEAKY_RELU = 5 /* negative slope 0.01 (nn.LeakyReLU default; pearcemlp.py:44) */,
@@ -143,6 +145,27 @@ typedef struct cds_attn_op {
   int32_t qkv_dtype;                            /* cds_dtype of qkv: bf16 (head_dim 32, L <= 128) runs on tensor cores (mma.sync) */
 } cds_attn_op;
 
+/* Multi-head attention with separate query and key|value sources and an optional diagonal mask:
+ *   out(b, i, h) = sum_{j in vis(i)} softmax_j(q(b,i,h) . k(b,j,h) / sqrt(hd)) v(b,j,h)     (fp32 softmax and accumulation)
+ *   vis(i) = { j < Lk : j <= i + diag } when masked, else every j < Lk
+ * q(b, i, :)   = q[b*q_bstride + i*q_lstride + (0..C)]                   (any column offset: point q at the first channel)
+ * kv(b, j, :)  = kv_step[iter*kv_step_stride + j*kv_step_lstride + (0..2C)] + kv_sample[b*kv_sample_bstride + j*kv_sample_lstride
+ *                + (0..2C)]    (either part may be NULL = 0; k = channels [0, C), v = channels [C, 2C); the cds_vec convention
+ *                               extended to a sequence: a per-iteration token row and per-trajectory rows feed one attention)
+ * heads split C evenly; head_dim = C / heads must be a multiple of 32 up to 256, and Lq, Lk <= 64 (else CDS_ERR_UNSUPPORTED).
+ * q, kv_step and kv_sample are of in_dtype (CDS_F32, CDS_TF32 -- read as fp32 -- or CDS_BF16); strides in elements.
+ * A query row without a visible key (masked, i + diag < 0) is written as zeros.
+ * diag = 0 is causal self-attention; diag = 1 is ChiTransformer's memory mask t >= s - 1 (chitransformer.py). */
+typedef struct cds_mha_op {
+  int32_t batch, Lq, Lk, C, heads;
+  int32_t masked, diag;
+  const void* q; int64_t q_bstride; int32_t q_lstride;
+  const void* kv_step; int64_t kv_step_stride; int32_t kv_step_lstride;
+  const void* kv_sample; int64_t kv_sample_bstride; int32_t kv_sample_lstride;
+  void* out; int64_t out_bstride; int32_t out_lstride;
+  int32_t in_dtype, out_dtype;                  /* cds_dtype */
+} cds_mha_op;
+
 /* dense fp32 (batch, L, C_in) -> dense (batch, L, C_out) of out_dtype, channels [C_in, C_out) zero: gives x_t the
  * channel-padded form the tensor-core conv reads through TMA (the UNets' first conv has C_in = obs+act dims, e.g. 14:
  * 32 bf16 channels for CDS_MATH_BF16_TC, 16 fp32 channels for CDS_MATH_TF32_TC -- rows must be multiples of 16 bytes) */
@@ -192,7 +215,8 @@ enum { CDS_OPF_ONCE = 1 /* run once per cds_plan_run, before its first iteration
 typedef struct cds_op {
   int32_t kind;                  /* cds_op_kind */
   int32_t flags;
-  union { cds_conv_op conv; cds_update_op update; cds_lnmod_op lnmod; cds_attn_op attn; cds_prep_op prep; cds_cast_op cast; } u;
+  union { cds_conv_op conv; cds_update_op update; cds_lnmod_op lnmod; cds_attn_op attn; cds_prep_op prep; cds_cast_op cast;
+          cds_mha_op mha; } u;
 } cds_op;
 
 typedef struct cds_plan cds_plan;
@@ -230,6 +254,11 @@ enum { CDS_ATTN_F32 = 0 /* fp32 CUDA cores, attention_f32_kernel<HD> */, CDS_ATT
  * (CDS_ATTN_TF32_TMA), else 0; info[2] = head_dim; info[3] = dynamic shared memory of the launch in bytes (0 for the
  * one-CTA-per-head mma.sync kernels).  Returns 0, or the negative cds_status with which the op would be refused. */
 int cds_attn_choice(const cds_attn_op* op, int32_t info[4]);
+
+/* The CDS_OP_MHA kernel cds_plan_append / cds_run_op would run `op` on.  Pure host logic: no pointer is dereferenced (they may
+ * be NULL).  info[0] = head_dim / 32 (the template parameter HPL of mha_f32_kernel: head channels per lane), info[1] = 1 when
+ * q / k / v are bf16 (else 0).  Returns 0, or the negative cds_status with which the op would be refused. */
+int cds_mha_choice(const cds_mha_op* op, int32_t info[2]);
 
 /* A plan = the per-iteration operator program for one (model, shape, option set) on one device. */
 int cds_plan_create(int device, cds_plan** out);
