@@ -271,7 +271,8 @@ int cds_plan_finalize(cds_plan* plan, int32_t n_iters);
  * replays of the iteration program.  The first call captures the program into a CUDA graph; later calls replay it.
  * use_graph = 0 launches kernels directly (debug/ncu).  Consecutive tensor-core conv kernels are chained with
  * programmatic dependent launch (the next kernel's prologue and weight prefetch overlap the previous kernel's tail);
- * CDS_PDL=0 in the environment switches that off. */
+ * CDS_PDL=0 in the environment switches that off.  It is latched at each kernel instantiation's first launch: an instantiation
+ * already launched ignores later changes, one first launched after a change reads the new value. */
 int cds_plan_run(cds_plan* plan, int32_t first, int32_t count, void* stream, int32_t use_graph);
 /* Single-step entry ("cds_step"): enqueue operators [op_first, op_first + op_count) of the program (indices into the appended
  * operator list; CDS_OPF_ONCE operators inside the range are skipped) for iteration `iter` with direct launches -- the device

@@ -389,16 +389,21 @@ RTOL = {cabi.F32: 0.0, cabi.TF32: 2.0 ** -10, cabi.BF16: 2.0 ** -8}
 U = 2.0 ** -24
 
 
-def gn_offset_atol(c, d):
-    """Extra absolute error allowed by the fp32 statistics var = E[x^2] - mean^2 of the tensor-core kernels, per output
-    element: with d = summation depth (a thread's columns of the group + the shuffle rounds over L + 4), E[x^2] carries a
-    relative error <= (d + 2) u, i.e. var an absolute one <= (d + 2) u (mu^2 + sigma^2): rstd is off by half that over
-    sigma^2, the normalised value z by |z| times it; the mean is off by <= d u |mu|, z by d u |mu| / sigma.  gamma and the
-    Mish slope (<= 1.1) scale both."""
+def pre_norm(c, d):
+    """the fp64 conv + bias of case ``c``: the GroupNorm input"""
     import opref
-    pre = opref.conv(d["view/in"], d["w"], batch=c["B"], L_out=c["L"], taps=c["taps"], stride=c["stride"],
-                     pad=c["taps"] // 2, math_mode=MATH[c["math"]], bias=d["bias"])
-    B, L, C, G = c["B"], c["L"], c["C_out"], c["groups"]
+    return opref.conv(d["view/in"], d["w"], batch=c["B"], L_out=c["L"], taps=c["taps"], stride=c["stride"],
+                      pad=c["taps"] // 2, math_mode=MATH[c["math"]], bias=d["bias"])
+
+
+def gn_offset_atol(pre, groups, gamma):
+    """Extra absolute error allowed by the fp32 statistics var = E[x^2] - mean^2 of the tensor-core kernels, per output
+    element, for the GroupNorm input ``pre`` (batch, L, C) in fp64: with d = summation depth (a thread's columns of the
+    group + the shuffle rounds over L + 4), E[x^2] carries a relative error <= (d + 2) u, i.e. var an absolute one
+    <= (d + 2) u (mu^2 + sigma^2): rstd is off by half that over sigma^2, the normalised value z by |z| times it; the mean
+    is off by <= d u |mu|, z by d u |mu| / sigma.  gamma and the Mish slope (<= 1.1) scale both."""
+    B, L, C = pre.shape
+    G = groups
     g = pre.reshape(B, L, G, C // G)
     mu = g.mean(dim=(1, 3), keepdim=True)
     sig = ((g - mu) ** 2).mean(dim=(1, 3), keepdim=True).sqrt()
@@ -406,17 +411,17 @@ def gn_offset_atol(c, d):
     depth = C // G + max(1, L).bit_length() + 4
     ratio = mu.abs() / sig
     dz = 0.5 * (depth + 2) * U * (1 + ratio ** 2) * z + depth * U * ratio
-    return (1.1 * dz * d["gamma"].abs().to(dz.dtype).reshape(1, 1, G, C // G)).reshape(B, L, C)
+    return (1.1 * dz * gamma.abs().to(dz.dtype).reshape(1, 1, G, C // G)).reshape(B, L, C)
 
 
-def check(c, y, ref, extra_atol=0.0):
+def check(c, y, ref, extra_atol=0.0, s=None):
     """(ok, largest error as a fraction of the bound, message) for the stored output ``y`` (fp32, bf16 widened) of case
-    ``c`` against the exact result ``ref``"""
+    ``c`` against the exact result ``ref``; ``s``: max(1, mean |ref|) of the whole output when ``ref`` is a part of it"""
     ref = ref.to(torch.float64)
     yd = y.to(torch.float64)
     if not torch.isfinite(yd).all():
         return False, float("inf"), "non-finite output"
-    s = max(1.0, ref.abs().mean().item())
+    s = max(1.0, ref.abs().mean().item()) if s is None else s
     bound = ATOL * s + extra_atol + RTOL[c["out_dtype"]] * ref.abs()
     frac = ((yd - ref).abs() / bound).max().item()
     if c["out_dtype"] == cabi.TF32 and int((y.contiguous().view(torch.int32) & 0x1FFF).abs().max()) != 0:

@@ -9,6 +9,7 @@ import pytest
 import torch
 
 import chi_cases as cc
+import emulator
 import mha_cases as mc
 import mha_ref
 from cleandiffuser_b200.diffusion import DDPM, DiscreteDiffusionSDE
@@ -57,7 +58,8 @@ def test_module_forward_matches_reference(gold, name):
 @pytest.fixture
 def emulate(monkeypatch):
     monkeypatch.setattr(runtime, "_device_ok", lambda device: True)
-    monkeypatch.setattr(runtime, "_make_handle", lambda device, ops, n: mha_ref.Handle(ops, n))
+    owners = emulator.record_owners(monkeypatch)      # every operand is bounds-checked against its owner
+    monkeypatch.setattr(runtime, "_make_handle", lambda device, ops, n: mha_ref.Handle(ops, n, owners()))
     monkeypatch.setenv("CDS_BACKEND", "cuda")       # any fallback to the PyTorch loop is a failure here
 
 

@@ -105,7 +105,7 @@ def test_conv_case_matches_fp64(name, monkeypatch):
     op = cc.descriptor(c, d)
     assert cc.choice_key(cabi.conv_choice(op.u.conv)) == c["want"]
     ref = cc.reference(c, d)
-    extra = cc.gn_offset_atol(c, d) if c["offset"] else 0.0
+    extra = cc.gn_offset_atol(cc.pre_norm(c, d), c["groups"], d["gamma"]) if c["offset"] else 0.0
     _run(c, op)
     y = d["view/out"].float().clone()
     ok, frac, msg = cc.check(c, y, ref, extra)

@@ -62,7 +62,8 @@ def test_lowered_edm_program(golden, name, math, monkeypatch):
     """The engine program of ContinuousEDM.sample (PREP -> denoiser -> CDS_UPD_EDM / _HEUN per network evaluation) on the
     numpy interpreter of the ABI."""
     monkeypatch.setattr(runtime, "_device_ok", lambda device: True)
-    monkeypatch.setattr(runtime, "_make_handle", lambda device, ops, n: emulator.Handle(ops, n))
+    owners = emulator.record_owners(monkeypatch)      # every operand is bounds-checked against its owner
+    monkeypatch.setattr(runtime, "_make_handle", lambda device, ops, n: emulator.Handle(ops, n, owners()))
     monkeypatch.setenv("CDS_BACKEND", "cuda")
     monkeypatch.setenv("CDS_MATH", math)
     spec = cases.edm_cases()[name]

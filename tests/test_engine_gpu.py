@@ -200,7 +200,9 @@ def test_cfg2_bf16_tensor_cores_full_batch(monkeypatch):
 @pytest.mark.parametrize("name", ["disc_dup_ddpm_x0", "cont_ddim_eps", "cont_sde_dpmsolverpp_2M_x0"])
 def test_sampler_bf16_tensor_cores_goldens(golden, name, monkeypatch):
     """Reverse loop on the tensor-core programs (once-cast + update-fused bf16 x_t copy + programmatic dependent launch)
-    against the reference goldens, with the stated bf16 tolerance; CDS_PDL=0 must give the same bits."""
+    against the reference goldens, with the stated bf16 tolerance; graph replay and direct launches must give the same bits
+    (both chain the kernels with programmatic dependent launch: tests/test_program_audit_gpu.py compares them with runs
+    that synchronise after every operator)."""
     monkeypatch.setenv("CDS_MATH", "bf16")
     spec = cases.sampler_cases()[name]
     outs = []

@@ -62,7 +62,8 @@ def test_legacy_ddpm_torch_path_matches_reference(golden, name, monkeypatch):
 @pytest.mark.parametrize("name", NAMES)
 def test_legacy_ddpm_lowered_program(golden, name, math, monkeypatch):
     monkeypatch.setattr(runtime, "_device_ok", lambda device: True)
-    monkeypatch.setattr(runtime, "_make_handle", lambda device, ops, n: emulator.Handle(ops, n))
+    owners = emulator.record_owners(monkeypatch)      # every operand is bounds-checked against its owner
+    monkeypatch.setattr(runtime, "_make_handle", lambda device, ops, n: emulator.Handle(ops, n, owners()))
     monkeypatch.setenv("CDS_BACKEND", "cuda")
     monkeypatch.setenv("CDS_MATH", math)
     spec = cases.legacy_cases()[name]
@@ -142,7 +143,8 @@ def test_legacy_edm_torch_path_matches_reference(golden, name, monkeypatch):
 @pytest.mark.parametrize("name", EDM_NAMES)
 def test_legacy_edm_lowered_program(golden, name, math, monkeypatch):
     monkeypatch.setattr(runtime, "_device_ok", lambda device: True)
-    monkeypatch.setattr(runtime, "_make_handle", lambda device, ops, n: emulator.Handle(ops, n))
+    owners = emulator.record_owners(monkeypatch)      # every operand is bounds-checked against its owner
+    monkeypatch.setattr(runtime, "_make_handle", lambda device, ops, n: emulator.Handle(ops, n, owners()))
     monkeypatch.setenv("CDS_BACKEND", "cuda")
     monkeypatch.setenv("CDS_MATH", math)
     spec = cases.legacy_edm_cases()[name]

@@ -45,7 +45,8 @@ def test_rf_torch_path_matches_reference(golden, name, monkeypatch):
 @pytest.mark.parametrize("name", NAMES)
 def test_rf_lowered_program(golden, name, math, monkeypatch):
     monkeypatch.setattr(runtime, "_device_ok", lambda device: True)
-    monkeypatch.setattr(runtime, "_make_handle", lambda device, ops, n: emulator.Handle(ops, n))
+    owners = emulator.record_owners(monkeypatch)      # every operand is bounds-checked against its owner
+    monkeypatch.setattr(runtime, "_make_handle", lambda device, ops, n: emulator.Handle(ops, n, owners()))
     monkeypatch.setenv("CDS_BACKEND", "cuda")
     monkeypatch.setenv("CDS_MATH", math)
     agent, inp, kw = build(cases.rf_cases()[name])
