@@ -13,7 +13,6 @@
 #include "conv_tc.cuh"
 #include "conv_ps.cuh"
 #include "attention_tma.cuh"
-#include "linear_ln.cuh"
 #include "elementwise.cuh"
 #include "mha.cuh"
 
@@ -60,17 +59,11 @@ struct Step {            // one validated operator + its kernel choice
   bool tc = false;       // tensor-core conv: tensor maps + launch geometry prepared at append time
   cds::ConvTcLaunch tcl;
   int branch = 0;        // (op.flags >> 8) & 0xff
-  bool skip = false;     // operator folded into another launch by a finalize-time peephole (none at present)
   bool ps = false;       // ... served by the position-sliced kernel (short sequences, conv_ps.cuh)
   cds::ConvPsLaunch psl;
   int attn_family = 0, attn_param = 0;   // attention: attn_pick's kernel family and template parameter
   int mha_hpl = 0;       // CDS_OP_MHA: head_dim / 32 (mha_pick)
   cds::AttnTmaLaunch attl;   // TF32 attention: tensor maps of the persistent TMA-fed kernel (attention_tma.cuh)
-  // gated Linear directly followed by the LayerNorm+modulate that reads its output: ONE launch of linear_ln_kernel when both
-  // operators are in the executed range (the LNMOD step then carries fused_into_prev and is not launched)
-  bool fuse_ln = false;
-  bool fused_into_prev = false;
-  cds::LinLnLaunch lll;
 };
 
 int elementwise_grid(int64_t total, int sm_count) {
@@ -222,11 +215,10 @@ int validate(const cds_op& op, Step* out) {
   }
 }
 
-int launch(const Step& s, const int* iter_ptr, int sm_count, cudaStream_t st, int* advance = nullptr, bool fused = false) {
+int launch(const Step& s, const int* iter_ptr, int sm_count, cudaStream_t st, int* advance = nullptr) {
   switch (s.op.kind) {
     case CDS_OP_CONV:
-      if (fused && s.fuse_ln) CDS_CUDA(cds::linear_ln_launch(s.lll, iter_ptr, sm_count, st));
-      else if (s.ps) CDS_CUDA(cds::conv_ps_launch(s.psl, iter_ptr, st));
+      if (s.ps) CDS_CUDA(cds::conv_ps_launch(s.psl, iter_ptr, st));
       else if (s.tc) CDS_CUDA(cds::conv_tc_launch(s.tcl, iter_ptr, st));
       else CDS_CUDA(cds::conv_simt_launch(s.op.u.conv, s.conv_bn, iter_ptr, st));
       return CDS_OK;
@@ -283,7 +275,6 @@ int preload_kernels() {
   CDS_CUDA(cudaFuncGetAttributes(&a, cds::attention_mma_tf32_hd32_kernel));
   CDS_CUDA(cds::attention_tma_preload_all());
   CDS_CUDA(cds::mha_preload_all());
-  CDS_CUDA(cds::linear_ln_preload_all());
   CDS_CUDA(cudaFuncGetAttributes(&a, cds::solver_update_kernel));
   CDS_CUDA(cudaFuncGetAttributes(&a, cds::cm_prep_kernel));
   CDS_CUDA(cudaFuncGetAttributes(&a, cds::cast_pad_kernel));
@@ -464,19 +455,6 @@ int cds_plan_finalize(cds_plan* p, int32_t n_iters) {
     // the branches share the machine: one CTA per SM and kernel, so that kernels of different branches co-reside
     for (Step& s : p->steps) if (s.tc && !s.ps) s.tcl.max_ctas_per_sm = 1;
   }
-  // peephole: gated Linear + the LayerNorm that consumes it -> one launch (linear_ln.cuh)
-  if (p->n_branches == 1) {
-    for (size_t i = 0; i + 1 < p->steps.size(); ++i) {
-      Step& a = p->steps[i];
-      Step& b = p->steps[i + 1];
-      if (a.op.kind != CDS_OP_CONV || b.op.kind != CDS_OP_LNMOD || !a.tc || a.ps) continue;
-      if ((a.op.flags & CDS_OPF_ONCE) || (b.op.flags & CDS_OPF_ONCE)) continue;
-      if (!cds::linear_ln_eligible(a.op.u.conv, b.op.u.lnmod)) continue;
-      if (!cds::linear_ln_prepare(a.op.u.conv, b.op.u.lnmod, &a.lll)) continue;
-      a.fuse_ln = true;
-      b.fused_into_prev = true;
-    }
-  }
   p->finalized = true;
   return CDS_OK;
 }
@@ -506,8 +484,8 @@ static int enqueue_iteration(cds_plan* p, cudaStream_t st) {
     for (int i = 0; i < (int)p->steps.size(); ++i) if (!(p->steps[i].op.flags & CDS_OPF_ONCE)) last = i;
     for (int i = 0; i < (int)p->steps.size(); ++i) {
       const Step& s = p->steps[i];
-      if ((s.op.flags & CDS_OPF_ONCE) || s.skip || s.fused_into_prev) continue;
-      int rc = launch(s, p->d_iter, p->sm_count, st, (fused && i == last) ? p->d_iter : nullptr, true);
+      if (s.op.flags & CDS_OPF_ONCE) continue;
+      int rc = launch(s, p->d_iter, p->sm_count, st, (fused && i == last) ? p->d_iter : nullptr);
       if (rc != CDS_OK) return rc;
     }
   } else {
@@ -518,7 +496,7 @@ static int enqueue_iteration(cds_plan* p, cudaStream_t st) {
     std::vector<std::vector<int>> per(p->n_branches);
     for (int i = 0; i < (int)p->steps.size(); ++i) {
       const Step& s = p->steps[i];
-      if (!(s.op.flags & CDS_OPF_ONCE) && !s.skip) per[s.branch].push_back(i);
+      if (!(s.op.flags & CDS_OPF_ONCE)) per[s.branch].push_back(i);
     }
     for (size_t k = 0;; ++k) {
       bool any = false;
@@ -600,11 +578,8 @@ int cds_plan_run_range(cds_plan* p, int32_t iter, int32_t op_first, int32_t op_c
   CDS_CUDA(cudaGetLastError());
   for (int i = op_first; i < op_first + op_count; ++i) {
     const Step& s = p->steps[i];
-    if ((s.op.flags & CDS_OPF_ONCE) || s.skip) continue;
-    // a fused pair runs as one launch only when the range holds both halves
-    if (s.fused_into_prev && i > op_first) continue;
-    const bool both = s.fuse_ln && i + 1 < op_first + op_count;
-    int rc = launch(s, p->d_iter, p->sm_count, st, nullptr, both);
+    if (s.op.flags & CDS_OPF_ONCE) continue;
+    int rc = launch(s, p->d_iter, p->sm_count, st);
     if (rc != CDS_OK) return rc;
   }
   return CDS_OK;
@@ -624,10 +599,8 @@ int cds_plan_profile(cds_plan* p, int32_t iter, void* stream, float* ms_per_op, 
       const bool once = (p->steps[i].op.flags & CDS_OPF_ONCE) != 0;
       if (once != (pass == 0)) continue;
       CDS_CUDA(cudaEventRecord(ev[2 * i], st));
-      if (!p->steps[i].skip && !p->steps[i].fused_into_prev) {
-        int rc = launch(p->steps[i], p->d_iter, p->sm_count, st, nullptr, true);
-        if (rc != CDS_OK) return rc;
-      }
+      int rc = launch(p->steps[i], p->d_iter, p->sm_count, st);
+      if (rc != CDS_OK) return rc;
       CDS_CUDA(cudaEventRecord(ev[2 * i + 1], st));
     }
   }
@@ -640,7 +613,7 @@ int cds_plan_profile(cds_plan* p, int32_t iter, void* stream, float* ms_per_op, 
 int cds_plan_launches_per_iter(const cds_plan* p) {
   if (!p) return 0;
   int n = advance_fused(p) ? 0 : 1;
-  for (const Step& s : p->steps) if (!(s.op.flags & CDS_OPF_ONCE) && !s.skip && !s.fused_into_prev) ++n;
+  for (const Step& s : p->steps) if (!(s.op.flags & CDS_OPF_ONCE)) ++n;
   return n;
 }
 

@@ -11,9 +11,7 @@ checks:
     mha_cases.bound, the LNMOD bound of tests/test_elementwise_gpu.py; UPDATE / PREP / CAST bit for bit against the
     interpreter run on host copies of their operands;
   - that nothing outside its declared outputs changed: every other owner keeps its fingerprint, and inside the owner of an
-    output view the elements outside the view keep theirs;
-  - every adjacent CONV -> LNMOD pair once more as ``run_range(it, i, 2)`` from the same inputs (one linear_ln launch when
-    the plan fused the pair): X against fp64, Y against the LayerNorm of the X the kernel stored.
+    output view the elements outside the view keep theirs.
 The largest error as a fraction of the bound is recorded per (program, kernel instantiation).
 Never imported by the product.
 """
@@ -98,12 +96,6 @@ def instantiation(op):
     return KIND_NAME[op.kind]
 
 
-def is_pair(ops, i):
-    """operators i, i + 1 are an adjacent CONV -> LNMOD pair of the iteration program"""
-    return (i + 1 < len(ops) and ops[i].kind == cabi.OP_CONV and ops[i + 1].kind == cabi.OP_LNMOD
-            and not (ops[i].flags | ops[i + 1].flags) & cabi.OPF_ONCE)
-
-
 def _bits(t):
     flat = t.detach().reshape(-1)
     return flat.view({1: torch.int8, 2: torch.int16, 4: torch.int32, 8: torch.int64}[flat.element_size()])
@@ -143,7 +135,6 @@ class Auditor:
         self.name, self.ops, self.handle, self.stream, self.sync = name, list(ops), handle, stream, sync
         self.mem = emulator.Owned(owners)
         self.worst = {}                       # instantiation -> (largest fraction of the bound, where)
-        self.pairs = 0                        # CONV -> LNMOD pairs run as one range
         self.failures = []
 
     # ---- bookkeeping ---------------------------------------------------------------------------------------------------
@@ -185,15 +176,15 @@ class Auditor:
         return after
 
     # ---- references (computed from the state before the launch); each returns check() -> [(frac, label)] --------------
-    def _conv(self, c, it, lazy=True):
-        """``lazy``: the fp64 reference is computed chunk by chunk after the launch (a first pass before it only sums |ref| for
-        the bound's scale s) -- possible when the launch cannot change the conv's operands, i.e. no operand shares a tensor
-        with the output; otherwise every chunk is computed before the launch and kept (in host memory when large)."""
+    def _conv(self, c, it):
+        """The fp64 reference is computed chunk by chunk after the launch (a first pass before it only sums |ref| for the
+        bound's scale s) when the launch cannot change the conv's operands, i.e. no operand shares a tensor with the output;
+        otherwise every chunk is computed before the launch and kept (in host memory when large)."""
         x, w, kw, out = emulator.conv_operands(c, it, self.mem)
         B, div = c.batch, kw["sample_row_div"]
         gn = c.groups > 0 and c.math in cabi.TC_MODES
         inputs = [t for t in (x, kw.get("res"), kw.get("res_in")) if t is not None]
-        lazy = lazy and all(t.untyped_storage().data_ptr() != out.untyped_storage().data_ptr() for t in inputs)
+        lazy = all(t.untyped_storage().data_ptr() != out.untyped_storage().data_ptr() for t in inputs)
 
         def chunk(b0, b1):
             k = dict(kw, batch=b1 - b0)
@@ -309,9 +300,9 @@ class Auditor:
                     for j, (g, w) in enumerate(zip(got, want))]
         return check
 
-    def reference(self, op, it, lazy=True):
+    def reference(self, op, it):
         if op.kind == cabi.OP_CONV:
-            return self._conv(op.u.conv, it, lazy)
+            return self._conv(op.u.conv, it)
         if op.kind == cabi.OP_LNMOD:
             return self._lnmod(op.u.lnmod)
         if op.kind == cabi.OP_ATTN:
@@ -340,46 +331,18 @@ class Auditor:
         self._stray_writes(before, once, sums, "once ops")
 
     def audit_iteration(self, it):
-        """every operator of iteration ``it`` alone, then every CONV -> LNMOD pair as one range; leaves the state of the
-        iteration's end"""
-        ops = self.ops
+        """every operator of iteration ``it`` alone; leaves the state of the iteration's end"""
         fp = self._fingerprints()
-        pair_in = None                                 # (conv index, saved outputs of both, conv check) of an open pair
-        for i, op in enumerate(ops):
+        for i, op in enumerate(self.ops):
             if op.flags & cabi.OPF_ONCE:
                 continue
             where = f"it {it} op {i} ({KIND_NAME[op.kind]})"
-            if is_pair(ops, i):
-                pair_in = (i, [v.clone() for o in (op, ops[i + 1]) for v in self._views(o)], None)
-            check = self.reference(op, it, lazy=not is_pair(ops, i))     # a pair's conv check is used again after the pair
+            check = self.reference(op, it)
             sums = self._sums([op])
             self._launch(it, i, 1)
             for frac, label in check():
                 self._record(instantiation(op), frac, f"{where} {label}")
             fp = self._stray_writes(fp, [op], sums, where)
-            if pair_in is not None and pair_in[0] == i:
-                pair_in = (i, pair_in[1], check)
-            elif pair_in is not None and pair_in[0] == i - 1:
-                fp = self._pair(it, i - 1, pair_in, fp)
-                pair_in = None
-
-    def _pair(self, it, i, pair_in, fp):
-        """operators i, i + 1 once more as one range from the inputs they had: X against the fp64 reference of the conv
-        (computed before operator i ran), Y against the LayerNorm of the X the kernel stored"""
-        ops = self.ops
-        _, saved, conv_check = pair_in
-        views = [v for o in (ops[i], ops[i + 1]) for v in self._views(o)]
-        for v, s in zip(views, saved):
-            v.copy_(s)
-        before, sums = self._fingerprints(), self._sums([ops[i], ops[i + 1]])
-        self._launch(it, i, 2)
-        self.pairs += 1
-        where = f"it {it} ops {i},{i + 1} (conv -> lnmod as one range)"
-        for frac, label in conv_check():
-            self._record(instantiation(ops[i]) + " [pair]", frac, f"{where} X {label}")
-        for frac, label in self._lnmod(ops[i + 1].u.lnmod)():
-            self._record(instantiation(ops[i + 1]) + " [pair]", frac, f"{where} Y {label}")
-        return self._stray_writes(before, [ops[i], ops[i + 1]], sums, where)
 
 
 # ---- whole iterations -------------------------------------------------------------------------------------------------
@@ -392,33 +355,27 @@ def written_owners(mem, ops):
     return sorted(idx)
 
 
-def run_op_by_op(handle, ops, first, count, stream, sync, pairs):
+def run_op_by_op(handle, ops, first, count, stream, sync):
     """iterations [first, first + count) one operator at a time with a synchronisation after each (the CDS_OPF_ONCE operators
-    first, as cds_plan_run does); ``pairs``: adjacent CONV -> LNMOD pairs run as one range (one launch where the plan fused
-    them)"""
+    first, as cds_plan_run does)"""
     if any(op.flags & cabi.OPF_ONCE for op in ops):
         handle.run(first, 0, stream, False)
         sync()
     for it in range(first, first + count):
-        i = 0
-        while i < len(ops):
-            if ops[i].flags & cabi.OPF_ONCE:
-                i += 1
+        for i, op in enumerate(ops):
+            if op.flags & cabi.OPF_ONCE:
                 continue
-            n = 2 if pairs and is_pair(ops, i) else 1
-            handle.run_range(it, i, n, stream)
+            handle.run_range(it, i, 1, stream)
             sync()
-            i += n
 
 
-def fused_pairs(handle, ops):
-    """number of CONV -> LNMOD pairs the plan runs as one launch, from launches_per_iter(): one launch per operator of the
-    iteration program, one fewer per fused pair, and one more for the iteration-counter advance unless the last operator,
-    a solver update of a single-branch program, advances it itself"""
+def launches_per_iter(ops):
+    """the launches of one iteration of ``ops``: one per operator of the iteration program, and one more for the
+    iteration-counter advance unless the last operator, a solver update of a single-branch program, advances it itself"""
     body = [op for op in ops if not op.flags & cabi.OPF_ONCE]
     branches = 1 + max((op.flags & 0xFF00) >> cabi.OPF_BRANCH_SHIFT for op in ops)
     advance = 0 if (branches == 1 and body and body[-1].kind == cabi.OP_UPDATE) else 1
-    return len(body) + advance - handle.launches_per_iter()
+    return len(body) + advance
 
 
 def report_lines(worst):

@@ -4,7 +4,7 @@ calls against the PyTorch loop.
 - Every case of tests/mha_cases.py runs through ``cds_run_op`` with each input dtype, each value pattern and each output
   dtype, under the term-by-term bound of mha_cases.bound; NaN padding around the output stays untouched, two runs give the
   same bits, and a sub-batch starting at trajectory 1 (odd element offsets) gives the same bits.
-- ``engine_forward`` at the pipeline shapes and the edge shape in all three math modes, with CDS_FUSE_LN on and off.
+- ``engine_forward`` at the pipeline shapes and the edge shape in all three math modes, with and without a condition.
 - ``sample()`` through the legacy DDPM class (the dp_* pipelines' agent) and DiscreteDiffusionSDE at the three pipeline
   shapes, per-GPU batch 2048 and batch 1, against the PyTorch loop on the same noise; the engine must serve every call.
 - A model in train mode with dropout falls back to the PyTorch loop and gives its result.
@@ -120,11 +120,10 @@ def _net(ctor, seed=0):
 FWD_SHAPES = ["pusht", "kitchen", "edge"]
 
 
-@pytest.mark.parametrize("fuse", ["1", "0"])
+@pytest.mark.parametrize("conditioned", [True, False], ids=["cond", "uncond"])
 @pytest.mark.parametrize("math", ["tf32", "bf16", "fp32"])
 @pytest.mark.parametrize("name", FWD_SHAPES)
-def test_engine_forward_matches_module(name, math, fuse, monkeypatch):
-    monkeypatch.setenv("CDS_FUSE_LN", fuse)
+def test_engine_forward_matches_module(name, math, conditioned):
     torch.backends.cuda.matmul.allow_tf32 = False
     ctor = cc.NETS[name]
     net = _net(ctor)
@@ -134,16 +133,16 @@ def test_engine_forward_matches_module(name, math, fuse, monkeypatch):
     cond = torch.randn(B, ctor["To"], ctor["obs_dim"], generator=g).to(DEV)
     t = torch.tensor([17], device=DEV)
     mode = {"tf32": cabi.MATH_TF32_TC, "bf16": cabi.MATH_BF16_TC, "fp32": cabi.MATH_FP32}[math]
-    for c in (cond, None):
-        with torch.no_grad():
-            want = net(x, t.expand(B), c)
-        got = runtime.engine_forward(net, x, t, c, math=mode)
-        scale = max(1.0, want.abs().mean().item())
-        err = (got - want).abs() / scale
-        assert torch.isfinite(got).all()
-        mx, mean = err.max().item(), err.mean().item()
-        _record(f"forward {math}", mx / TOL[math][0], f"{name} fuse={fuse} cond={c is not None}")
-        assert mx < TOL[math][0] and mean < TOL[math][1], (mx, mean)
+    c = cond if conditioned else None
+    with torch.no_grad():
+        want = net(x, t.expand(B), c)
+    got = runtime.engine_forward(net, x, t, c, math=mode)
+    scale = max(1.0, want.abs().mean().item())
+    err = (got - want).abs() / scale
+    assert torch.isfinite(got).all()
+    mx, mean = err.max().item(), err.mean().item()
+    _record(f"forward {math}", mx / TOL[math][0], f"{name} cond={conditioned}")
+    assert mx < TOL[math][0] and mean < TOL[math][1], (mx, mean)
 
 
 # ---------------------------------------------------------------------------------------------------------------- sample()

@@ -3,7 +3,7 @@
 UPDATE, PREP and CAST promise fp32 results identical to the operation-by-operation fp32 mirror in tests/emulator.py, so
 they are compared bit for bit: every descriptor is built from one dict of buffers twice, over CPU tensors for the emulator
 and over their GPU copies for ``cds_run_op``, and every buffer (NaN guards included) must come out with the same bits.
-LNMOD is compared with tests/opref.py's fp64 LayerNorm under the bound of tests/test_linear_ln_gpu.py."""
+LNMOD is compared with tests/opref.py's fp64 LayerNorm under the bound of tests/test_linear_layernorm_plan_gpu.py."""
 import pytest
 import torch
 

@@ -306,9 +306,9 @@ def test_dit_tf32_program_keeps_attention_on_tensor_cores(monkeypatch):
     assert sorted((c.C_in, c.C_out) for c in tc if c.batch == B) == [(320, 320), (320, 4480)]
     attn = [op.u.attn for op in p.ops if op.kind == cabi.OP_ATTN]
     assert len(attn) == 2 and all(a.qkv_dtype == cabi.TF32 and a.out_dtype == cabi.TF32 for a in attn)
-    # the form libcds fuses into one launch at plan-finalize time (csrc/linear_ln.cuh::linear_ln_eligible): a gated Linear with a
-    # dense fp32 residual, directly followed by the LayerNorm+modulate that reads its output, one vector set per L tokens
-    fusable = 0
+    # the form conv_tc's gated epilogue lane serves: a gated Linear with a dense fp32 residual, directly followed by the
+    # LayerNorm+modulate that reads its output, one vector set per L tokens
+    gated = 0
     for a, b in zip(p.ops[:-1], p.ops[1:]):
         if a.kind != cabi.OP_CONV or b.kind != cabi.OP_LNMOD:
             continue
@@ -317,8 +317,8 @@ def test_dit_tf32_program_keeps_attention_on_tensor_cores(monkeypatch):
                 and c.taps == 1 and c.L_in == 1 and c.C_out == 320 and c.C_in % 32 == 0 and c.sample_row_div == L
                 and c.out_dtype != cabi.BF16 and c.res_dtype != cabi.BF16 and c.bias.step and not c.bias.sample
                 and ln.in_ == c.out and ln.C == c.C_out and ln.batch * ln.L == c.batch and ln.L == L and ln.out_dtype != cabi.BF16):
-            fusable += 1
-    assert fusable == 4                                      # attention out-projection and second MLP Linear of both blocks
+            gated += 1
+    assert gated == 4                                    # attention out-projection and second MLP Linear of both blocks
     g = torch.Generator().manual_seed(2)
     x, cond, t = torch.randn(B, L, 29, generator=g), torch.randn(B, 128, generator=g), torch.tensor([0.37])
     with torch.no_grad():

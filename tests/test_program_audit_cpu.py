@@ -88,8 +88,6 @@ def test_every_operator_passes(which, monkeypatch):
     kinds = {op.kind for op in plan.program.ops}
     assert {cabi.OP_CONV, cabi.OP_UPDATE} <= kinds and (which == "cfg2" or {cabi.OP_MHA, cabi.OP_LNMOD} <= kinds)
     assert aud.worst and max(f for f, _ in aud.worst.values()) <= PASS_FRAC, aud.worst
-    if which == "chi":
-        assert aud.pairs > 0                    # the out-projections and their LayerNorms ran once more as one range
 
 
 def test_a_corrupted_element_is_pinned_on_its_operator(monkeypatch):

@@ -2,15 +2,15 @@
 
 Programs: cfg2 (fp32, tf32, bf16), cfg3 / cfg4 / cfg5 (tf32, bf16) from cleandiffuser_b200/workloads.py, and the
 ChiTransformer kitchen shape (tests/golden/chi_cases.py) at batch 2048 as scripts/chitransformer_bench.py builds it (tf32,
-bf16).  None of them launches linear_ln (csrc/linear_ln.cuh serves 256 output channels only: cfg4's d_model is 320, and
-ChiTransformer's Linear layers are not gated), so "dit256" adds cfg4 with a DiT1d whose widths it serves -- d_model 256 and
-x_t of 96 channels, so that x_proj, which reads x_t shared by the two CFG halves (in_batch_mod), is fused as well.  Each
-is built by one ``sample()``, so that the plan, its tables and its per-call fills are what production builds; its handle
-is then driven directly.
+bf16).  "dit256" adds cfg4 with a DiT1d of d_model 256 over x_t of 96 channels: the only audited program with 256-wide
+gated Linears (attention out-projection, second MLP Linear) and a 256-wide x_proj that reads x_t shared by the two CFG
+halves (in_batch_mod), i.e. conv_tc's gated and table epilogue lanes, each followed by a LayerNorm, at a width other than
+cfg4's 320.  Each is built by one ``sample()``, so that the plan, its tables and its per-call fills are what production builds; its
+handle is then driven directly.
 
 - Every operator of iterations 0, 1, the middle one (loops of 50 steps or more) and the last, reached by graph replay, is
   run alone and checked on every trajectory against fp64 under its kernel family's bound, and for writes outside its
-  outputs; every CONV -> LNMOD pair once more as one range (the fused linear_ln launch where the plan fused it).
+  outputs; one iteration is one launch per operator, plus the iteration-counter advance.
 - ``min(12, n_iters - f)`` whole iterations from a snapshot at iteration f give the same bits operator by operator (with a
   synchronisation after each: no launch overlaps another), by graph replay (the 10-iteration graph plus single graphs)
   and by direct launches.
@@ -37,28 +37,20 @@ pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
 PROGRAMS = ["cfg2-fp32", "cfg2-tf32", "cfg2-bf16", "cfg3-tf32", "cfg3-bf16", "cfg4-tf32", "cfg4-bf16", "cfg5-tf32",
             "cfg5-bf16", "chi-tf32", "chi-bf16", "dit256-tf32"]
-# CONV -> LNMOD pairs per iteration the plan runs as one linear_ln launch: dit256's x_proj -> LN and, per block, the gated
-# out-projection -> LN and fc2 -> LN (the last one feeding the final LayerNorm); no other program reaches linear_ln (see above),
-# and bf16 / fp32 programs never fuse.  Not every CONV -> LNMOD pair fuses: cfg4's and ChiTransformer's widths are not served,
-# ChiTransformer's out-projections have no gate, and x_proj reads x_t padded to 32 channels (fewer than linear_ln's 96).
-FUSED_EXPECTED = {"dit256-tf32": 5}
 CHI_BATCH, CHI_STEPS = 2048, 50
-WORST, COST, FUSED = {}, {}, {}
+WORST, COST = {}, {}
 
 
 @pytest.fixture(scope="module", autouse=True)
 def _report(request):
     WORST.clear()
     COST.clear()
-    FUSED.clear()
     yield
     capman = request.config.pluginmanager.getplugin("capturemanager")
     with capman.global_and_fixture_disabled():
         print(f"\n[audit] {torch.cuda.get_device_name(0)}: largest error as a fraction of the bound")
         for line in pa.report_lines(WORST):
             print("[audit] " + line)
-        for k, (fused, pairs) in sorted(FUSED.items()):
-            print(f"[audit] {k}: {pairs} CONV -> LNMOD pairs per iteration, {fused} of them fused into one linear_ln launch")
         for k, (sec, extra, base) in sorted(COST.items()):
             print(f"[audit] {k}: {sec:.1f} s, peak {extra / 2 ** 30:.2f} GB on top of the program's {base / 2 ** 30:.2f} GB")
 
@@ -172,12 +164,8 @@ def test_every_operator_matches_fp64(prog, monkeypatch):
     for inst, (frac, where) in aud.worst.items():
         WORST[(prog, inst)] = (frac, where)
     assert not aud.failures, "\n".join(aud.failures[:20])
-    pairs = [i for i in range(len(ops)) if pa.is_pair(ops, i)]
-    assert aud.pairs == len(pairs) * len(its)
-    # launches_per_iter() says how many pairs the plan fused; every pair ran as one range above, so each fused launch was checked
-    fused = pa.fused_pairs(plan.handle, ops)
-    FUSED[prog] = (fused, len(pairs))
-    assert fused == FUSED_EXPECTED.get(prog, 0), (fused, len(pairs))
+    # every launch of an iteration is one of the operators checked above, or the counter advance
+    assert plan.handle.launches_per_iter() == pa.launches_per_iter(ops)
 
 
 @pytest.mark.parametrize("prog", PROGRAMS)
@@ -198,7 +186,7 @@ def test_replay_gives_the_bits_of_operator_by_operator_runs(prog, monkeypatch):
             for t, s in zip(written, snap):
                 t.copy_(s)
             if mode == "op by op":
-                pa.run_op_by_op(plan.handle, ops, f, K, st, torch.cuda.synchronize, pairs=True)
+                pa.run_op_by_op(plan.handle, ops, f, K, st, torch.cuda.synchronize)
             else:
                 plan.handle.run(f, K, st, mode == "graph")
             torch.cuda.synchronize()
@@ -213,8 +201,8 @@ def test_replay_gives_the_bits_of_operator_by_operator_runs(prog, monkeypatch):
 
 @pytest.mark.parametrize("prog,branches", [("cfg2-tf32", 2), ("cfg2-tf32", 4), ("cfg4-tf32", 2)])
 def test_parallel_branches_give_the_operator_by_operator_bits(prog, branches, monkeypatch):
-    """Branch programs cap conv_tc at one CTA per SM and never fuse linear_ln: their whole iterations must give the bits of
-    the single-branch program run one operator at a time (no pair fused)"""
+    """Branch programs cap conv_tc at one CTA per SM: their whole iterations must give the bits of the single-branch program
+    run one operator at a time"""
     agent, plan = _build(prog, monkeypatch)
     ops, n, st = plan.program.ops, plan.n_iters, _stream()
     f = min(1, n - 1)
@@ -224,7 +212,7 @@ def test_parallel_branches_give_the_operator_by_operator_bits(prog, branches, mo
     plan.handle.run(0, f, st, True)
     torch.cuda.synchronize()
     state = {k: getattr(plan, k).clone() for k in carried if getattr(plan, k) is not None}
-    pa.run_op_by_op(plan.handle, ops, f, K, st, torch.cuda.synchronize, pairs=False)
+    pa.run_op_by_op(plan.handle, ops, f, K, st, torch.cuda.synchronize)
     torch.cuda.synchronize()
     want = {k: getattr(plan, k).clone() for k in state}
     plan.close()
