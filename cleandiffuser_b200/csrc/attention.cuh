@@ -193,135 +193,10 @@ __global__ void __launch_bounds__(128) attention_mma_hd32_kernel(const cds_attn_
   }
 }
 
-// ---------------------------------------------------------------------------------------------------------------------
-// TF32 tensor-core path (fp32 q/k/v storage rounded to TF32 = cds_dtype CDS_TF32, head_dim 32, L <= 128): the same structure on
-// mma.sync.m16n8k8 (tf32 operands, fp32 accumulate).  The S accumulator layout (row = lane/4 (+8), columns 2c, 2c+1 with
-// c = lane%4) becomes the A operand of P V by RENAMING the summation index: MMA k-slot c stands for key 2c, slot c+4 for key
-// 2c+1 of the 8-key tile, and the V fragment is fetched with the same renaming (one 64-bit load of V^T[dim][2c..2c+1]) -- no
-// shuffles.  K row-major with a 36-float pitch, V transposed with a 136-float pitch: conflict-free fragment loads.
-// Algorithmic HBM bytes per (trajectory, head): 4*L*32*3 (q, k, v) + L*32*4 (out).
-__device__ __forceinline__ void mma_tf32_1688(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
-  asm volatile("mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
-               : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
-__device__ __forceinline__ uint32_t to_tf32(float x) { uint32_t u; asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(u) : "f"(x)); return u; }
-
-constexpr int kAttnKPitchF = 36;                     // floats per K row (32 + 4 pad)
-constexpr int kAttnVPitchF = kAttnMaxL + 8;          // floats per V^T row
-
-__global__ void __launch_bounds__(128) attention_mma_tf32_hd32_kernel(const cds_attn_op p) {
-  constexpr int HD = 32;
-  __shared__ __align__(16) float Ks[kAttnMaxL * kAttnKPitchF];
-  __shared__ __align__(16) float Vt[HD * kAttnVPitchF];
-  const int b = blockIdx.x / p.heads, h = blockIdx.x - b * p.heads;
-  const int L = p.L, ld = 3 * p.C;
-  const int LP = (L + 7) & ~7;                       // keys padded to whole 8-key tiles (zeros, masked below)
-  const float* base = reinterpret_cast<const float*>(p.qkv) + (int64_t)b * L * ld + h * HD;
-  for (int idx = threadIdx.x; idx < LP * 8; idx += blockDim.x) {
-    const int j = idx >> 3, c4 = (idx & 7) * 4;      // key row, first of 4 channels
-    float4 kq = make_float4(0.f, 0.f, 0.f, 0.f), vq = kq;
-    if (j < L) {
-      kq = *reinterpret_cast<const float4*>(base + (int64_t)j * ld + p.C + c4);
-      vq = *reinterpret_cast<const float4*>(base + (int64_t)j * ld + 2 * p.C + c4);
-    }
-    *reinterpret_cast<float4*>(&Ks[j * kAttnKPitchF + c4]) = kq;
-    Vt[(c4 + 0) * kAttnVPitchF + j] = vq.x; Vt[(c4 + 1) * kAttnVPitchF + j] = vq.y;
-    Vt[(c4 + 2) * kAttnVPitchF + j] = vq.z; Vt[(c4 + 3) * kAttnVPitchF + j] = vq.w;
-  }
-  __syncthreads();
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int gr = lane >> 2, c = lane & 3;             // fragment row (0..7), k-slot / column-pair index (0..3)
-  const float scale_log2e = rsqrtf((float)HD) * 1.4426950408889634f;
-  constexpr int NT_MAX = kAttnMaxL / 8;
-  const int NT = LP / 8;
-  for (int qt = warp; qt * 16 < L; qt += 4) {
-    const int r0 = qt * 16 + gr, r1 = r0 + 8;
-    uint32_t aq[4][4];                                // 4 K steps of 8 dims
-#pragma unroll
-    for (int ks = 0; ks < 4; ++ks) {
-      const int d0 = ks * 8 + c;
-      aq[ks][0] = r0 < L ? __float_as_uint(base[(int64_t)r0 * ld + d0]) : 0u;
-      aq[ks][1] = r1 < L ? __float_as_uint(base[(int64_t)r1 * ld + d0]) : 0u;
-      aq[ks][2] = r0 < L ? __float_as_uint(base[(int64_t)r0 * ld + d0 + 4]) : 0u;
-      aq[ks][3] = r1 < L ? __float_as_uint(base[(int64_t)r1 * ld + d0 + 4]) : 0u;
-    }
-    float s[NT_MAX][4];
-#pragma unroll
-    for (int nt = 0; nt < NT_MAX; ++nt) {
-      s[nt][0] = s[nt][1] = s[nt][2] = s[nt][3] = 0.f;
-      if (nt < NT) {
-#pragma unroll
-        for (int ks = 0; ks < 4; ++ks) {
-          const float* kp = &Ks[(nt * 8 + gr) * kAttnKPitchF + ks * 8 + c];        // B[k = dim][n = key]: n = lane/4, k = lane%4 (+4)
-          mma_tf32_1688(s[nt], aq[ks], __float_as_uint(kp[0]), __float_as_uint(kp[4]));
-        }
-      }
-    }
-    float m0 = -INFINITY, m1 = -INFINITY;
-#pragma unroll
-    for (int nt = 0; nt < NT_MAX; ++nt) {
-      if (nt < NT) {
-        const int j = nt * 8 + 2 * c;
-        if (j >= L) s[nt][0] = s[nt][2] = -INFINITY;
-        if (j + 1 >= L) s[nt][1] = s[nt][3] = -INFINITY;
-        m0 = fmaxf(m0, fmaxf(s[nt][0], s[nt][1]));
-        m1 = fmaxf(m1, fmaxf(s[nt][2], s[nt][3]));
-      }
-    }
-    m0 = fmaxf(m0, __shfl_xor_sync(0xffffffffu, m0, 1)); m0 = fmaxf(m0, __shfl_xor_sync(0xffffffffu, m0, 2));
-    m1 = fmaxf(m1, __shfl_xor_sync(0xffffffffu, m1, 1)); m1 = fmaxf(m1, __shfl_xor_sync(0xffffffffu, m1, 2));
-    float d0 = 0.f, d1 = 0.f;
-    const float o0 = m0 * scale_log2e, o1 = m1 * scale_log2e;
-#pragma unroll
-    for (int nt = 0; nt < NT_MAX; ++nt) {
-      if (nt < NT) {
-        s[nt][0] = exp2f(fmaf(s[nt][0], scale_log2e, -o0)); s[nt][1] = exp2f(fmaf(s[nt][1], scale_log2e, -o0));
-        s[nt][2] = exp2f(fmaf(s[nt][2], scale_log2e, -o1)); s[nt][3] = exp2f(fmaf(s[nt][3], scale_log2e, -o1));
-        d0 += s[nt][0] + s[nt][1];
-        d1 += s[nt][2] + s[nt][3];
-      }
-    }
-    d0 += __shfl_xor_sync(0xffffffffu, d0, 1); d0 += __shfl_xor_sync(0xffffffffu, d0, 2);
-    d1 += __shfl_xor_sync(0xffffffffu, d1, 1); d1 += __shfl_xor_sync(0xffffffffu, d1, 2);
-    float o[HD / 8][4];
-#pragma unroll
-    for (int dn = 0; dn < HD / 8; ++dn) o[dn][0] = o[dn][1] = o[dn][2] = o[dn][3] = 0.f;
-#pragma unroll
-    for (int nt = 0; nt < NT_MAX; ++nt) {
-      if (nt < NT) {
-        // A k-slot c <-> key 2c, slot c+4 <-> key 2c+1 of this tile: (a0, a1, a2, a3) = (P[r0][2c], P[r1][2c], P[r0][2c+1], P[r1][2c+1])
-        uint32_t ap[4] = {to_tf32(s[nt][0]), to_tf32(s[nt][2]), to_tf32(s[nt][1]), to_tf32(s[nt][3])};
-#pragma unroll
-        for (int dn = 0; dn < HD / 8; ++dn) {
-          const float2 vv = *reinterpret_cast<const float2*>(&Vt[(dn * 8 + gr) * kAttnVPitchF + nt * 8 + 2 * c]);   // B[k-slot][n = dim]
-          mma_tf32_1688(o[dn], ap, __float_as_uint(vv.x), __float_as_uint(vv.y));
-        }
-      }
-    }
-    const float i0 = 1.f / d0, i1 = 1.f / d1;
-    float* out = reinterpret_cast<float*>(p.out);
-    const int od = p.out_dtype;
-#pragma unroll
-    for (int dn = 0; dn < HD / 8; ++dn) {
-      const int col = h * HD + dn * 8 + 2 * c;
-      if (r0 < L) *reinterpret_cast<float2*>(out + ((int64_t)b * L + r0) * p.C + col) =
-          make_float2(f32_for_store(o[dn][0] * i0, od), f32_for_store(o[dn][1] * i0, od));
-      if (r1 < L) *reinterpret_cast<float2*>(out + ((int64_t)b * L + r1) * p.C + col) =
-          make_float2(f32_for_store(o[dn][2] * i1, od), f32_for_store(o[dn][3] * i1, od));
-    }
-  }
-}
-
-// family (CDS_ATTN_F32 / _BF16_MMA / _TF32_MMA) and, for the fp32 kernel, HD: as attn_pick (cds_api.cu) chose them
+// family (CDS_ATTN_F32 / _BF16_MMA) and, for the fp32 kernel, HD: as attn_pick (cds_api.cu) chose them
 inline cudaError_t attention_launch(const cds_attn_op& p, int family, int hd, cudaStream_t st) {
   if (family == CDS_ATTN_BF16_MMA) {
     attention_mma_hd32_kernel<<<dim3(p.batch * p.heads), 128, 0, st>>>(p);
-    return cudaGetLastError();
-  }
-  if (family == CDS_ATTN_TF32_MMA) {
-    attention_mma_tf32_hd32_kernel<<<dim3(p.batch * p.heads), 128, 0, st>>>(p);
     return cudaGetLastError();
   }
   if (family != CDS_ATTN_F32) return cudaErrorInvalidValue;

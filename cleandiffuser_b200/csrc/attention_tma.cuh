@@ -1,7 +1,7 @@
 // Persistent, TMA-fed attention for the TF32 tensor-core programs (q/k/v: fp32 storage rounded to TF32, head_dim 32, L <= 128).
 //
-// Replaces, for that case, the one-CTA-per-(trajectory, head) kernel of attention.cuh, whose time went into exposed global-load
-// latency (each CTA first pulls 38 KB of strided q/k/v rows, then computes, 3-4 CTAs per SM).  Here
+// With one CTA per (trajectory, head) the time goes into exposed global-load latency (each CTA first pulls 38 KB of strided
+// q/k/v rows, then computes, 3-4 CTAs per SM).  Here
 //   * every CTA is persistent (2 per SM) and walks the (trajectory, head) work list with stride gridDim.x;
 //   * warp 7 is the producer: per work item three TMA boxes {32 channels, L rows} of the (B, L, 3C) q|k|v tensor land in a
 //     2-stage shared-memory ring (128-byte rows, SWIZZLE_128B), completion on a "full" mbarrier, slots handed back through an
@@ -11,9 +11,9 @@
 //     swizzle makes all of them bank-conflict free, V needs no transposed copy;
 //   * the normalised 16 x 32 output tile goes through a per-warp 2 KB staging tile and ONE cp.async.bulk.tensor store (full
 //     128-byte lines; rows >= L are clipped by the TMA unit).
-// Same arithmetic as attention_mma_tf32_hd32_kernel (same MMA shapes, same summation order inside a row, the same fmaf for
-// every exp2 argument), so the two agree bit for bit unless an exp2 result is subnormal (ex2.approx.ftz here flushes it, exp2f
-// there does not); the k-slot renaming of the P V product is described there.
+// The S accumulator layout of m16n8k8 (row = lane/4 (+8), columns 2c, 2c+1 with c = lane%4) becomes the A operand of P V by
+// RENAMING the summation index: MMA k-slot c stands for key 2c, slot c+4 for key 2c+1 of the 8-key tile, and the V fragment is
+// fetched with the same renaming (V rows 2c and 2c+1) -- no shuffles.
 // Reference: nn.MultiheadAttention inside DiTBlock, cleandiffuser/nn_diffusion/dit.py:10-36.
 // Algorithmic HBM bytes per (trajectory, head): 4*L*32*3 (q, k, v) + 4*L*32 (out).
 #pragma once
@@ -32,6 +32,12 @@ struct AttnTmaLaunch {
   int n_work = 0, smem_bytes = 0;
 };
 
+__device__ __forceinline__ void mma_tf32_1688(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
+  asm volatile("mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
+               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+               : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
+}
+__device__ __forceinline__ uint32_t to_tf32(float x) { uint32_t u; asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(u) : "f"(x)); return u; }
 __device__ __forceinline__ float attn_ex2(float x) {            // 2^x, flush-to-zero, no range fix-up (x <= 0 here)
   float y;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
@@ -208,12 +214,6 @@ attention_tma_tf32_hd32_kernel(const cds_attn_op p, const __grid_constant__ CUte
     if (lane == 0) ptx::mbar_arrive(&empty_bar[s]);
   }
   if (lane == 0) ptx::bulk_wait_group<0>();
-}
-
-// CDS_ATTN_TMA=0 in the environment (read once per process) sends the ops this kernel would serve to the one-CTA-per-head one
-inline bool attention_tma_enabled() {
-  static const bool off = [] { const char* e = getenv("CDS_ATTN_TMA"); return e && e[0] == '0'; }();
-  return !off;
 }
 
 inline int attention_tma_smem_bytes(int L) {

@@ -114,15 +114,12 @@ int attn_pick(const cds_attn_op& a, int* family, int* param) {
     *family = CDS_ATTN_BF16_MMA;
     return CDS_OK;
   }
-  // fp32 storage rounded to TF32 (TF32 tensor-core programs): mma.sync tf32 when the shape allows -- fed by TMA when out is
-  // 16-byte aligned as well --, else the fp32 kernel
-  const bool tf32_mma = a.qkv_dtype == CDS_TF32 && hd == 32 && a.L <= cds::kAttnMaxL && a.C % 4 == 0 && qkv % 16 == 0 &&
-                        a.out_dtype != CDS_BF16 && out % 8 == 0;
-  if (tf32_mma && out % 16 == 0 && cds::attention_tma_enabled()) {
+  // fp32 storage rounded to TF32 (TF32 tensor-core programs): the TMA-fed mma.sync tf32 kernel when the shape and the
+  // alignment of q/k/v and out allow, else the fp32 kernel
+  if (a.qkv_dtype == CDS_TF32 && hd == 32 && a.L <= cds::kAttnMaxL && a.C % 4 == 0 && qkv % 16 == 0 &&
+      a.out_dtype != CDS_BF16 && out % 16 == 0) {
     *family = CDS_ATTN_TF32_TMA;
     *param = (a.L + 7) / 8;
-  } else if (tf32_mma) {
-    *family = CDS_ATTN_TF32_MMA;
   } else {
     *family = CDS_ATTN_F32;
     *param = hd;
@@ -272,7 +269,6 @@ int preload_kernels() {
   CDS_CUDA(cudaFuncGetAttributes(&a, cds::attention_f32_kernel<32>));
   CDS_CUDA(cudaFuncGetAttributes(&a, cds::attention_f32_kernel<64>));
   CDS_CUDA(cudaFuncGetAttributes(&a, cds::attention_mma_hd32_kernel));
-  CDS_CUDA(cudaFuncGetAttributes(&a, cds::attention_mma_tf32_hd32_kernel));
   CDS_CUDA(cds::attention_tma_preload_all());
   CDS_CUDA(cds::mha_preload_all());
   CDS_CUDA(cudaFuncGetAttributes(&a, cds::solver_update_kernel));

@@ -1175,57 +1175,6 @@ inline int conv_tc_width(const cds_conv_op& c) {
   return 0;
 }
 
-// can the tensor-core kernel serve this op?  (otherwise the fp32 CUDA-core kernel runs it, any dtype)
-inline bool conv_tc_eligible(const cds_conv_op& c) {
-  if (c.math != CDS_MATH_BF16_TC && c.math != CDS_MATH_TF32_TC) return false;
-  const bool tf32 = conv_is_tf32(c);
-  // operand tensors (in, res_in) must have the mode's storage type: bf16, or fp32 (CDS_F32 / CDS_TF32 read alike)
-  auto operand_ok = [tf32](int dt) { return tf32 ? (dt == CDS_F32 || dt == CDS_TF32) : (dt == CDS_BF16); };
-  const int vec_el = tf32 ? 4 : 8;                    // elements per 16 bytes
-  const int kmin = tf32 ? 16 : 32;                    // channels in a 64-byte operand row
-  if (!operand_ok(c.in_dtype)) return false;
-  if (c.stride != 1 && c.stride != 2) return false;
-  if (c.phases != 1 && c.phases != 2) return false;
-  int L = c.L_out;                                   // tile rows = 128/L trajectories x L output positions
-  if (L > 32 || (L & (L - 1)) != 0) return false;
-  if (c.stride == 1 ? (c.L_in != L) : (c.L_in != 2 * L || c.phases != 1 || c.res_w || c.res)) return false;
-  if (conv_tc_width(c) == 0) return false;
-  if (conv_tc_width(c) > 256 && c.groups != 0 && conv_tc_pick_kc(c) != 64) return false;   // wide GN variants: KC = 64 only
-  if (c.res_w) {
-    // the main and the shortcut accumulator share one wgmma-width (256-column) tile: CTA tiles of at most 128 columns
-    const int n = conv_tc_width(c);
-    const bool fixed = n == 16 || n == 32 || n == 64 || n == 128 || n == 256 || ((n == 512 || n == 1024) && c.groups != 0);
-    const int tile = fixed ? (n > 256 ? 128 : (n >= 128 ? n / 2 : n)) : conv_tc_runtime_tile(n, conv_tc_pick_kc(c));
-    if (tile > 128) return false;
-  }
-  if (c.sample_row_div > 1 && c.L_out != 1) return false;
-  if (c.C_in % kmin != 0) return false;
-  if (c.groups != 0 && (c.groups != 8 || c.phases != 1 || c.C_out < 32)) return false;
-  if (c.phases == 2 && (c.res || c.res_w)) return false;
-  int T = 128 / L;
-  if (c.in_batch_mod > 0 && c.in_batch_mod % T != 0) return false;
-  if (c.res_batch_mod > 0 && c.res_w && c.res_batch_mod % T != 0) return false;   // (the identity residual is read row by row)
-  if (c.res_w && (!operand_ok(c.res_in_dtype) || c.res_C % kmin != 0)) return false;
-  if ((c.in_lstride % vec_el) || (c.in_bstride % vec_el) || ((uintptr_t)c.in % 16)) return false;
-  if (c.res_w && ((c.res_in_lstride % vec_el) || (c.res_in_bstride % vec_el) || ((uintptr_t)c.res_in % 16))) return false;
-  if (c.C_out % 16 == 0) {                           // vector stores
-    if (c.out_dtype == 1 ? ((c.out_lstride % 8) || ((uintptr_t)c.out % 16)) : ((c.out_lstride % 4) || ((uintptr_t)c.out % 16)))
-      return false;
-  }
-  if (c.res && (c.res_dtype == 1 ? ((c.res_lstride % 8) || ((uintptr_t)c.res % 16)) : ((c.res_lstride % 4) || ((uintptr_t)c.res % 16))))
-    return false;
-  return true;
-}
-
-struct ConvTcLaunch {
-  ConvTcParams prm;
-  bool tf32 = false;              // fp32 operands read as TF32 (CDS_MATH_TF32_TC)
-  int kc = 0, n = 0, split = 1;   // n = CTA tile width, split*n = layer width
-  int max_ctas_per_sm = 0;        // > 0: use at most this many CTAs per SM (plans with parallel branches share the SMs)
-  bool has_res = false;
-  dim3 grid;
-};
-
 // Share a layer's columns between two CTAs?  Yes for the wide layers (C_out >= 128: halves the per-CTA epilogue and main
 // loop) and for C_out = 64 when there are too few row tiles to fill the machine.
 inline int conv_tc_pick_split(const cds_conv_op& c, int n_total, int m_tiles) {
@@ -1258,6 +1207,52 @@ inline ConvTcShape conv_tc_shape(const cds_conv_op& c) {
   }
   return s;
 }
+
+// can the tensor-core kernel serve this op?  (otherwise the fp32 CUDA-core kernel runs it, any dtype)
+inline bool conv_tc_eligible(const cds_conv_op& c) {
+  if (c.math != CDS_MATH_BF16_TC && c.math != CDS_MATH_TF32_TC) return false;
+  const bool tf32 = conv_is_tf32(c);
+  // operand tensors (in, res_in) must have the mode's storage type: bf16, or fp32 (CDS_F32 / CDS_TF32 read alike)
+  auto operand_ok = [tf32](int dt) { return tf32 ? (dt == CDS_F32 || dt == CDS_TF32) : (dt == CDS_BF16); };
+  const int vec_el = tf32 ? 4 : 8;                    // elements per 16 bytes
+  const int kmin = tf32 ? 16 : 32;                    // channels in a 64-byte operand row
+  if (!operand_ok(c.in_dtype)) return false;
+  if (c.stride != 1 && c.stride != 2) return false;
+  if (c.phases != 1 && c.phases != 2) return false;
+  int L = c.L_out;                                   // tile rows = 128/L trajectories x L output positions
+  if (L > 32 || (L & (L - 1)) != 0) return false;
+  if (c.stride == 1 ? (c.L_in != L) : (c.L_in != 2 * L || c.phases != 1 || c.res_w || c.res)) return false;
+  if (conv_tc_width(c) == 0) return false;
+  if (conv_tc_width(c) > 256 && c.groups != 0 && conv_tc_pick_kc(c) != 64) return false;   // wide GN variants: KC = 64 only
+  // the main and the shortcut accumulator share one wgmma-width (256-column) tile: CTA tiles of at most 128 columns
+  if (c.res_w && conv_tc_shape(c).n > 128) return false;
+  if (c.sample_row_div > 1 && c.L_out != 1) return false;
+  if (c.C_in % kmin != 0) return false;
+  if (c.groups != 0 && (c.groups != 8 || c.phases != 1 || c.C_out < 32)) return false;
+  if (c.phases == 2 && (c.res || c.res_w)) return false;
+  int T = 128 / L;
+  if (c.in_batch_mod > 0 && c.in_batch_mod % T != 0) return false;
+  if (c.res_batch_mod > 0 && c.res_w && c.res_batch_mod % T != 0) return false;   // (the identity residual is read row by row)
+  if (c.res_w && (!operand_ok(c.res_in_dtype) || c.res_C % kmin != 0)) return false;
+  if ((c.in_lstride % vec_el) || (c.in_bstride % vec_el) || ((uintptr_t)c.in % 16)) return false;
+  if (c.res_w && ((c.res_in_lstride % vec_el) || (c.res_in_bstride % vec_el) || ((uintptr_t)c.res_in % 16))) return false;
+  if (c.C_out % 16 == 0) {                           // vector stores
+    if (c.out_dtype == 1 ? ((c.out_lstride % 8) || ((uintptr_t)c.out % 16)) : ((c.out_lstride % 4) || ((uintptr_t)c.out % 16)))
+      return false;
+  }
+  if (c.res && (c.res_dtype == 1 ? ((c.res_lstride % 8) || ((uintptr_t)c.res % 16)) : ((c.res_lstride % 4) || ((uintptr_t)c.res % 16))))
+    return false;
+  return true;
+}
+
+struct ConvTcLaunch {
+  ConvTcParams prm;
+  bool tf32 = false;              // fp32 operands read as TF32 (CDS_MATH_TF32_TC)
+  int kc = 0, n = 0, split = 1;   // n = CTA tile width, split*n = layer width
+  int max_ctas_per_sm = 0;        // > 0: use at most this many CTAs per SM (plans with parallel branches share the SMs)
+  bool has_res = false;
+  dim3 grid;
+};
 
 inline bool conv_tc_prepare(const cds_conv_op& c, ConvTcLaunch* out) {
   ConvTcLaunch& L = *out;
@@ -1373,9 +1368,7 @@ long long* conv_tc_trace_hook(int grid);
 template <int KC, int N, bool HAS_RES, int SPLIT, bool TF32>
 cudaError_t conv_tc_launch_t(const ConvTcLaunch& L, const int* iter_ptr, cudaStream_t st) {
   using Cfg = ConvTcCfg<KC, N, HAS_RES, SPLIT>;
-  if constexpr (!Cfg::kFits) {
-    return cudaErrorInvalidConfiguration;      // (never picked: conv_tc_eligible keeps shortcut tiles at <= 128 columns)
-  } else {
+  static_assert(Cfg::kFits, "conv_tc instantiation does not fit");
   static bool attr = false;
   static int resident = 0;                   // CTAs of this instantiation that fit on the device at once
   static int sm_count = 0;
@@ -1394,7 +1387,6 @@ cudaError_t conv_tc_launch_t(const ConvTcLaunch& L, const int* iter_ptr, cudaStr
     e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&want, conv_tc_kernel<KC, N, HAS_RES, SPLIT, TF32>, kTcThreads, Cfg::kSmemBytes);
     if (e != cudaSuccess) return e;
     if (want > Cfg::kMinBlocks) want = Cfg::kMinBlocks;
-    if (const char* cap = getenv("CDS_TC_MAXCTAS")) { int c = atoi(cap); if (c >= 1 && c < want) want = c; }
     if (want < 1) want = 1;
     if (getenv("CDS_DEBUG"))
       fprintf(stderr, "[cds] conv_tc<%d,%d,%d,%d,%s>: %d CTA/SM, smem %d B, %d stages\n", KC, N, (int)HAS_RES, SPLIT,
@@ -1417,44 +1409,43 @@ cudaError_t conv_tc_launch_t(const ConvTcLaunch& L, const int* iter_ptr, cudaStr
   if (pdl) { at[na].id = cudaLaunchAttributeProgrammaticStreamSerialization; at[na].val.programmaticStreamSerializationAllowed = 1; ++na; }
   cfg.attrs = at; cfg.numAttrs = na;
   return cudaLaunchKernelEx(&cfg, conv_tc_kernel<KC, N, HAS_RES, SPLIT, TF32>, prm, iter_ptr);
-  }
 }
 // touch the kernel once (module load) so that nothing lazy happens inside a stream capture
 template <int KC, int N, bool HAS_RES, int SPLIT, bool TF32>
 cudaError_t conv_tc_preload_t() {
-  if constexpr (!ConvTcCfg<KC, N, HAS_RES, SPLIT>::kFits) {
-    return cudaSuccess;
-  } else {
-    cudaFuncAttributes a;
-    return cudaFuncGetAttributes(&a, conv_tc_kernel<KC, N, HAS_RES, SPLIT, TF32>);
-  }
+  static_assert(ConvTcCfg<KC, N, HAS_RES, SPLIT>::kFits, "conv_tc instantiation does not fit");
+  cudaFuncAttributes a;
+  return cudaFuncGetAttributes(&a, conv_tc_kernel<KC, N, HAS_RES, SPLIT, TF32>);
 }
 
-// every (KC, N, SPLIT) the dispatcher can pick (each with and without the shortcut accumulator); X(kc, n, split)
-#define CDS_TC_VARIANTS(X)                                                                              \
-  X(64, 16, 1) X(64, 32, 1) X(64, 64, 1) X(64, 128, 1) X(64, 256, 1) X(64, 32, 2) X(64, 64, 2) X(64, 128, 2) \
-  X(64, 256, 2) X(64, 256, 4) X(64, 128, 4) X(64, 128, 8) X(64, 160, 1) X(64, 192, 1)                    \
-  X(32, 16, 1) X(32, 32, 1) X(32, 64, 1) X(32, 128, 1) X(32, 256, 1) X(32, 32, 2) X(32, 64, 2) X(32, 128, 2)
+// Every instantiation the dispatcher can select, X(KC, N, SPLIT, HAS_RES, TF32).  Absent by construction: N = 16 with a
+// shortcut conv (narrow heads take none), shortcut tiles wider than 128 columns (conv_tc_eligible), 128-column tiles of
+// 512 / 1024-wide layers without a shortcut and split TF32 64-wide layers (conv_tc_pick_split).
+#define CDS_TC_VARIANTS(X)                                                                                                \
+  X(64, 16, 1, 0, 0) X(64, 32, 1, 0, 0) X(64, 32, 1, 1, 0) X(64, 32, 2, 0, 0) X(64, 32, 2, 1, 0) X(64, 64, 1, 0, 0)       \
+  X(64, 64, 1, 1, 0) X(64, 64, 2, 0, 0) X(64, 64, 2, 1, 0) X(64, 128, 1, 0, 0) X(64, 128, 1, 1, 0) X(64, 128, 2, 0, 0)    \
+  X(64, 128, 2, 1, 0) X(64, 128, 4, 1, 0) X(64, 128, 8, 1, 0) X(64, 160, 1, 0, 0) X(64, 192, 1, 0, 0) X(64, 256, 1, 0, 0) \
+  X(64, 256, 2, 0, 0) X(64, 256, 4, 0, 0)                                                                                 \
+  X(32, 16, 1, 0, 0) X(32, 32, 1, 0, 0) X(32, 32, 1, 1, 0) X(32, 32, 2, 0, 0) X(32, 32, 2, 1, 0) X(32, 64, 1, 0, 0)       \
+  X(32, 64, 1, 1, 0) X(32, 64, 2, 0, 0) X(32, 64, 2, 1, 0) X(32, 128, 1, 0, 0) X(32, 128, 1, 1, 0) X(32, 128, 2, 0, 0)    \
+  X(32, 128, 2, 1, 0) X(32, 256, 1, 0, 0)                                                                                 \
+  X(64, 16, 1, 0, 1) X(64, 32, 1, 0, 1) X(64, 32, 1, 1, 1) X(64, 64, 1, 0, 1) X(64, 64, 1, 1, 1) X(64, 64, 2, 0, 1)       \
+  X(64, 64, 2, 1, 1) X(64, 128, 1, 0, 1) X(64, 128, 1, 1, 1) X(64, 128, 2, 0, 1) X(64, 128, 2, 1, 1) X(64, 128, 4, 1, 1)  \
+  X(64, 128, 8, 1, 1) X(64, 160, 1, 0, 1) X(64, 192, 1, 0, 1) X(64, 256, 1, 0, 1) X(64, 256, 2, 0, 1) X(64, 256, 4, 0, 1) \
+  X(32, 16, 1, 0, 1) X(32, 32, 1, 0, 1) X(32, 32, 1, 1, 1) X(32, 64, 1, 0, 1) X(32, 64, 1, 1, 1) X(32, 64, 2, 0, 1)       \
+  X(32, 64, 2, 1, 1) X(32, 128, 1, 0, 1) X(32, 128, 1, 1, 1) X(32, 128, 2, 0, 1) X(32, 128, 2, 1, 1) X(32, 256, 1, 0, 1)
 
 #ifndef CDS_TC_INSTANTIATE
-#define CDS_TC_EXTERN2(KC_, N_, S_, T_)                                                                                 \
-  extern template cudaError_t conv_tc_launch_t<KC_, N_, false, S_, T_>(const ConvTcLaunch&, const int*, cudaStream_t);  \
-  extern template cudaError_t conv_tc_launch_t<KC_, N_, true, S_, T_>(const ConvTcLaunch&, const int*, cudaStream_t);   \
-  extern template cudaError_t conv_tc_preload_t<KC_, N_, false, S_, T_>();                                              \
-  extern template cudaError_t conv_tc_preload_t<KC_, N_, true, S_, T_>();
-#define CDS_TC_EXTERN(KC_, N_, S_) CDS_TC_EXTERN2(KC_, N_, S_, false) CDS_TC_EXTERN2(KC_, N_, S_, true)
+#define CDS_TC_EXTERN(KC_, N_, S_, R_, T_)                                                                                \
+  extern template cudaError_t conv_tc_launch_t<KC_, N_, R_ != 0, S_, T_ != 0>(const ConvTcLaunch&, const int*, cudaStream_t); \
+  extern template cudaError_t conv_tc_preload_t<KC_, N_, R_ != 0, S_, T_ != 0>();
 CDS_TC_VARIANTS(CDS_TC_EXTERN)
 #undef CDS_TC_EXTERN
-#undef CDS_TC_EXTERN2
 
 inline cudaError_t conv_tc_launch(const ConvTcLaunch& L, const int* iter_ptr, cudaStream_t st) {
-#define CDS_TC_CASE(KC_, N_, S_)                                                                                         \
-  if (L.kc == KC_ && L.n == N_ && L.split == S_) {                                                                       \
-    if (L.tf32) return L.has_res ? conv_tc_launch_t<KC_, N_, true, S_, true>(L, iter_ptr, st)                            \
-                                 : conv_tc_launch_t<KC_, N_, false, S_, true>(L, iter_ptr, st);                          \
-    return L.has_res ? conv_tc_launch_t<KC_, N_, true, S_, false>(L, iter_ptr, st)                                       \
-                     : conv_tc_launch_t<KC_, N_, false, S_, false>(L, iter_ptr, st);                                     \
-  }
+#define CDS_TC_CASE(KC_, N_, S_, R_, T_)                                                                          \
+  if (L.kc == KC_ && L.n == N_ && L.split == S_ && L.has_res == (R_ != 0) && L.tf32 == (T_ != 0))                 \
+    return conv_tc_launch_t<KC_, N_, R_ != 0, S_, T_ != 0>(L, iter_ptr, st);
   CDS_TC_VARIANTS(CDS_TC_CASE)
 #undef CDS_TC_CASE
   return cudaErrorInvalidValue;
@@ -1462,11 +1453,8 @@ inline cudaError_t conv_tc_launch(const ConvTcLaunch& L, const int* iter_ptr, cu
 
 inline cudaError_t conv_tc_preload_all() {
   cudaError_t e;
-#define CDS_TC_PRE(KC_, N_, S_)                                                              \
-  if ((e = conv_tc_preload_t<KC_, N_, false, S_, false>()) != cudaSuccess) return e;         \
-  if ((e = conv_tc_preload_t<KC_, N_, true, S_, false>()) != cudaSuccess) return e;          \
-  if ((e = conv_tc_preload_t<KC_, N_, false, S_, true>()) != cudaSuccess) return e;          \
-  if ((e = conv_tc_preload_t<KC_, N_, true, S_, true>()) != cudaSuccess) return e;
+#define CDS_TC_PRE(KC_, N_, S_, R_, T_) \
+  if ((e = conv_tc_preload_t<KC_, N_, R_ != 0, S_, T_ != 0>()) != cudaSuccess) return e;
   CDS_TC_VARIANTS(CDS_TC_PRE)
 #undef CDS_TC_PRE
   return cudaSuccess;

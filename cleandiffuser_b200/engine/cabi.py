@@ -215,16 +215,16 @@ def conv_choice(conv: ConvOp):
             "tf32": bool(info[6])}
 
 
-ATTN_F32, ATTN_BF16_MMA, ATTN_TF32_MMA, ATTN_TF32_TMA = 0, 1, 2, 3     # cds_attn_choice info[0]
+ATTN_F32, ATTN_BF16_MMA, ATTN_TF32_TMA = 0, 1, 3     # cds_attn_choice info[0]
 
 
 def attn_choice(attn: AttnOp):
     """The kernel the library would run ``attn`` on (cds_attn_choice): a dict with the family ("f32" / "bf16_mma" /
-    "tf32_mma" / "tma"), its template parameter (HD of "f32", NT of "tma", else 0), the head dim and the dynamic shared
-    memory of the launch.  Raises CdsError if the op would be refused."""
+    "tma"), its template parameter (HD of "f32", NT of "tma", else 0), the head dim and the dynamic shared memory of the
+    launch.  Raises CdsError if the op would be refused."""
     info = (C.c_int32 * 4)()
     check(load().cds_attn_choice(C.byref(attn), info))
-    fam = {ATTN_F32: "f32", ATTN_BF16_MMA: "bf16_mma", ATTN_TF32_MMA: "tf32_mma", ATTN_TF32_TMA: "tma"}[info[0]]
+    fam = {ATTN_F32: "f32", ATTN_BF16_MMA: "bf16_mma", ATTN_TF32_TMA: "tma"}[info[0]]
     return {"family": fam, "param": info[1], "hd": info[2], "smem": info[3]}
 
 

@@ -247,12 +247,11 @@ int cds_conv_choice(const cds_conv_op* op, int32_t info[8]);
 
 /* kernel families of CDS_OP_ATTN (cds_attn_choice info[0]) */
 enum { CDS_ATTN_F32 = 0 /* fp32 CUDA cores, attention_f32_kernel<HD> */, CDS_ATTN_BF16_MMA = 1 /* mma.sync bf16, head_dim 32 */,
-       CDS_ATTN_TF32_MMA = 2 /* mma.sync tf32, head_dim 32, one CTA per (trajectory, head) */,
        CDS_ATTN_TF32_TMA = 3 /* mma.sync tf32, head_dim 32, persistent and TMA-fed, attention_tma.cuh<NT> */ };
 /* The attention kernel cds_plan_append / cds_run_op would choose for `op`.  Pure host logic: only the alignment of qkv and out
- * is read (they may be NULL), and CDS_ATTN_TMA=0 is honoured.  info[0] = family; info[1] = HD (CDS_ATTN_F32), NT = ceil(L / 8)
- * (CDS_ATTN_TF32_TMA), else 0; info[2] = head_dim; info[3] = dynamic shared memory of the launch in bytes (0 for the
- * one-CTA-per-head mma.sync kernels).  Returns 0, or the negative cds_status with which the op would be refused. */
+ * is read (they may be NULL).  info[0] = family; info[1] = HD (CDS_ATTN_F32), NT = ceil(L / 8) (CDS_ATTN_TF32_TMA), else 0;
+ * info[2] = head_dim; info[3] = dynamic shared memory of the launch in bytes (0 for CDS_ATTN_BF16_MMA).  Returns 0, or the
+ * negative cds_status with which the op would be refused. */
 int cds_attn_choice(const cds_attn_op* op, int32_t info[4]);
 
 /* The CDS_OP_MHA kernel cds_plan_append / cds_run_op would run `op` on.  Pure host logic: no pointer is dereferenced (they may

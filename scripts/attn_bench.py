@@ -1,5 +1,5 @@
 """Time CDS_OP_ATTN alone at a DiT1d shape (default: cfg4's 4096 x 100 tokens, 10 heads of 32) through cds_run_op.
-usage: python scripts/attn_bench.py [batch] [L] [heads] [reps]      (CDS_ATTN_TMA=0 selects the one-CTA-per-head kernel)"""
+usage: python scripts/attn_bench.py [batch] [L] [heads] [reps]"""
 import ctypes as C
 import os
 import sys
@@ -33,4 +33,4 @@ torch.cuda.synchronize()
 us = e0.elapsed_time(e1) / reps * 1e3
 flop = 4.0 * B * H * L * L * 32
 byt = 4.0 * B * L * Cd * 4
-print(f"attn B={B} L={L} heads={H} tma={os.environ.get('CDS_ATTN_TMA', '1')}: {us:.1f} us  {flop / us / 1e6:.1f} TFLOP/s  {byt / us / 1e3:.0f} GB/s (algorithmic)")
+print(f"attn B={B} L={L} heads={H}: {us:.1f} us  {flop / us / 1e6:.1f} TFLOP/s  {byt / us / 1e3:.0f} GB/s (algorithmic)")

@@ -2,12 +2,12 @@
 kernel.
 
 Every case names the kernel instantiation it must reach (``want``, in the form ``choice_key`` gives ``cabi.attn_choice``):
-("f32", HD), ("bf16_mma", 0), ("tf32_mma", 0) or ("tma", NT).  tests/test_attn_dispatch_cpu.py checks on the CPU that
+("f32", HD), ("bf16_mma", 0) or ("tma", NT).  tests/test_attn_dispatch_cpu.py checks on the CPU that
 each case reaches it, that the table covers every instantiation, and that ``check`` accepts the fp64 reference and rejects
 typical kernel faults; tests/test_attention_gpu.py runs every case through ``cds_run_op`` against tests/opref.py.
 
-``out_off`` places the output that many floats into its buffer: 2 floats (8 bytes) is how the one-CTA-per-head TF32
-kernel is reached, since the persistent TMA kernel needs a 16-byte aligned output.
+``out_off`` places the output that many floats into its buffer: at 2 floats (8 bytes) TF32 q/k/v with head_dim 32 and
+L <= 128 run on the fp32 kernel, since the persistent TMA kernel needs a 16-byte aligned output (the "_out8" cases).
 """
 import math
 import zlib
@@ -21,7 +21,7 @@ TORCH_DT = {cabi.F32: torch.float32, cabi.TF32: torch.float32, cabi.BF16: torch.
 F64 = torch.float64
 LOG2E = 1.0 / math.log(2.0)
 # P is rounded to the MMA operand type before P V: unit roundoff of bf16 (8 significant bits) and of TF32 (cvt.rna, 11)
-U_P = {"f32": 0.0, "bf16_mma": 2.0 ** -8, "tf32_mma": 2.0 ** -11, "tma": 2.0 ** -11}
+U_P = {"f32": 0.0, "bf16_mma": 2.0 ** -8, "tma": 2.0 ** -11}
 # relative rounding of the stored output, as in tests/test_conv_kernels_gpu.py
 R_OUT = {cabi.F32: 0.0, cabi.TF32: 2.0 ** -10, cabi.BF16: 2.0 ** -8}
 # value patterns every case runs with (see ``make``)
@@ -52,14 +52,18 @@ for L in (1, 10, 19, 28, 37, 46, 55, 64, 65, 74, 83, 92, 101, 110, *range(113, 1
     CASES.append(case(f"tma_L{L}", key("tma", (L + 7) // 8), B=3, L=L, heads=2 + L % 3))
 for L in (1, 64, 113, 128):
     CASES.append(case(f"tma_L{L}_ring", key("tma", (L + 7) // 8), B=3 * 2 * SMS // 8 + 1, L=L, heads=8))
-# ---- one-CTA-per-head TF32 mma.sync: out 8- but not 16-byte aligned
+# ---- TF32 q/k/v in the TMA kernel's shapes with the output 8- but not 16-byte aligned: the fp32 kernel serves them.  Seven
+# shapes of their own, and the shape of every TMA case above (the "_out8" twins)
 for L in (1, 7, 16, 33, 100, 113, 128):
-    CASES.append(case(f"tf32mma_L{L}", key("tf32_mma"), B=3, L=L, heads=3, out_off=2))
+    CASES.append(case(f"f32_hd32_L{L}_tf32_out8", key("f32", 32), B=3, L=L, heads=3, out_off=2))
+for c in [c for c in CASES if c["want"][0] == "tma"]:
+    CASES.append(dict(c, name=f"f32_{c['name']}_out8", want=key("f32", 32), out_off=2))
 # ---- bf16 mma.sync (every bf16 DiT program)
 for L in (1, 15, 16, 17, 100, 127, 128):
     CASES.append(case(f"bf16mma_L{L}", key("bf16_mma"), B=3, L=L, heads=1 + L % 4, qkv_dtype=cabi.BF16, outs=ALL_OUTS))
 # ---- fp32 kernel: head_dim 16 / 32 / 64, L up to the largest accepted (K and V above 48 KB of shared memory from
-# L * hd > 6144 on), q/k/v fp32 or TF32-rounded.  TF32 q/k/v with head_dim 32 and L <= 128 reaches it only with bf16 output.
+# L * hd > 6144 on), q/k/v fp32 or TF32-rounded.  With TF32 q/k/v, head_dim 32, L <= 128 and a 16-byte aligned output
+# only a bf16 output reaches it.
 for hd in (16, 32, 64):
     for L in (1, 100, 129, 300, MAX_L[hd]):
         for qd in (cabi.F32, cabi.TF32):

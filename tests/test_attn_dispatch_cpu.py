@@ -1,11 +1,9 @@
 """CPU checks of the operator-level attention case table (tests/attn_cases.py): every case reaches the kernel instantiation
-it names (cds_attn_choice, pure host logic), the table covers all 21 instantiations, the refusals hold, and the checker of
+it names (cds_attn_choice, pure host logic), the table covers all 20 instantiations, the refusals hold, and the checker of
 tests/test_attention_gpu.py accepts the fp64 reference and rejects three typical kernel faults."""
 import math
 import os
 import re
-import subprocess
-import sys
 
 import pytest
 import torch
@@ -21,8 +19,7 @@ CSRC = os.path.join(ROOT, "cleandiffuser_b200", "csrc")
 def _instantiations():
     f32 = re.findall(r"CDS_ATTN_CASE\((\d+)\)\n", open(os.path.join(CSRC, "attention.cuh")).read())
     nt = re.findall(r"CDS_ATTN_NT\((\d+)\)", open(os.path.join(CSRC, "attention_tma.cuh")).read())
-    return ({ac.key("f32", int(h)) for h in f32} | {ac.key("tma", int(n)) for n in nt} |
-            {ac.key("bf16_mma"), ac.key("tf32_mma")})
+    return {ac.key("f32", int(h)) for h in f32} | {ac.key("tma", int(n)) for n in nt} | {ac.key("bf16_mma")}
 
 
 @pytest.mark.parametrize("name", list(ac.CASES))
@@ -34,7 +31,7 @@ def test_case_reaches_its_instantiation(name):
 
 def test_cases_cover_every_instantiation():
     inst = _instantiations()
-    assert len(inst) == 21
+    assert len(inst) == 20
     assert {c["want"] for c in ac.CASES.values()} == inst
 
 
@@ -78,17 +75,6 @@ def test_refusals():
 
 
 ERR_INVALID, ERR_UNSUPPORTED = -1, -3      # cds_status
-
-
-def test_tma_switch_sends_the_tma_cases_to_the_tf32_mma_kernel():
-    """CDS_ATTN_TMA=0 (read once per process, hence a fresh interpreter)"""
-    code = ("import sys; sys.path[:0] = [%r, %r]\n"
-            "import attn_cases as ac\nfrom cleandiffuser_b200.engine import cabi\n"
-            "print(sorted({cabi.attn_choice(ac.fake_descriptor(c).u.attn)['family'] for c in ac.CASES.values() "
-            "if c['want'][0] == 'tma'}))") % (ROOT, os.path.join(ROOT, "tests"))
-    out = subprocess.run([sys.executable, "-c", code], env=dict(os.environ, CDS_ATTN_TMA="0"), capture_output=True,
-                         text=True, check=True).stdout
-    assert out.strip() == "['tf32_mma']"
 
 
 # ---- the checker itself, with the fp64 reference standing in for the kernel (one trajectory, CPU)

@@ -13,27 +13,14 @@ from cleandiffuser_b200.engine import cabi
 
 CSRC = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "cleandiffuser_b200", "csrc")
 
-# instantiations that eligibility can never select, with the reason
-UNREACHABLE = {
-    **{cc.tc(kc, 16, 1, 1, tf): "N = 16 serves narrow 1x1 heads only, which take no shortcut conv (conv_tc_width)"
-       for kc in (32, 64) for tf in (0, 1)},
-    **{cc.tc(kc, 256, 1, 1, tf): "a shortcut conv needs CTA tiles of at most 128 columns (conv_tc_eligible)"
-       for kc in (32, 64) for tf in (0, 1)},
-    **{cc.tc(64, n, s, 1, tf): "a shortcut conv needs CTA tiles of at most 128 columns (conv_tc_eligible)"
-       for n, s in ((160, 1), (192, 1), (256, 2), (256, 4)) for tf in (0, 1)},
-    **{cc.tc(64, 128, s, 0, tf): "512 / 1024-wide GroupNorm layers without a shortcut use 256-column tiles "
-       "(conv_tc_pick_split)" for s in (4, 8) for tf in (0, 1)},
-    **{cc.tc(kc, 32, 2, r, 1): "TF32 64-wide layers are never split (conv_tc_pick_split)" for kc in (32, 64) for r in (0, 1)},
-}
-
 
 def _instantiations():
     tc_src = open(os.path.join(CSRC, "conv_tc.cuh")).read()
     ps_src = open(os.path.join(CSRC, "conv_ps.cuh")).read()
     body = lambda src, name: re.search(r"#define %s\(X\)(.*?)\n\n" % name, src, re.S).group(1)
     out = set()
-    for kc, n, s in re.findall(r"X\((\d+),\s*(\d+),\s*(\d+)\)", body(tc_src, "CDS_TC_VARIANTS")):
-        out |= {cc.tc(int(kc), int(n), int(s), r, tf) for r in (0, 1) for tf in (0, 1)}
+    for kc, n, s, r, tf in re.findall(r"X\((\d+),\s*(\d+),\s*(\d+),\s*([01]),\s*([01])\)", body(tc_src, "CDS_TC_VARIANTS")):
+        out.add(cc.tc(int(kc), int(n), int(s), int(r), int(tf)))
     for n, r, tf in re.findall(r"X\((\d+),\s*(true|false),\s*(true|false)\)", body(ps_src, "CDS_PS_VARIANTS")):
         out.add(cc.ps(int(n), r == "true", tf == "true"))
     return out
@@ -45,17 +32,16 @@ def test_case_reaches_its_variant(name):
     assert cc.choice_key(cabi.conv_choice(cc.descriptor(c).u.conv)) == c["want"]
 
 
-def test_cases_cover_every_selectable_instantiation():
+def test_cases_cover_every_instantiation():
     inst = _instantiations()
-    assert len(inst) == 22 * 4 + 6
-    assert set(UNREACHABLE) <= inst
+    assert len(inst) == 64 + 6
     reached = {c["want"] for c in cc.CASES.values() if c["want"][0] != "simt"}
-    assert reached == inst - set(UNREACHABLE), (sorted(inst - set(UNREACHABLE) - reached), sorted(reached - inst))
+    assert reached == inst, (sorted(inst - reached), sorted(reached - inst))
     assert {c["want"] for c in cc.CASES.values() if c["want"][0] == "simt"} == {cc.simt(32), cc.simt(64), cc.simt(128)}
 
 
-def test_every_tc_variant_runs_three_tiles_per_cta():
-    """the persistent tile loop of conv_tc: for every reachable instantiation some case gives each resident CTA (at most
+def test_every_tc_instantiation_runs_three_tiles_per_cta():
+    """the persistent tile loop of conv_tc: for every instantiation some case gives each resident CTA (at most
     2 per SM, or 1 in a plan with parallel branches) three or more tiles, counted from cds_conv_choice's SPLIT / column
     tiles"""
     best = {}
@@ -66,7 +52,7 @@ def test_every_tc_variant_runs_three_tiles_per_cta():
         tiles = -(-c["B"] * c["L"] // 128) * (ch["split"] if ch["split"] > 1 else ch["col_tiles"])
         assert tiles == cc.num_tiles(c), c["name"]
         best[c["want"]] = max(best.get(c["want"], 0), tiles / cc.resident_ctas(c))
-    tc_variants = {k for k in _instantiations() - set(UNREACHABLE) if k[0] == "tc"}
+    tc_variants = {k for k in _instantiations() if k[0] == "tc"}
     assert set(best) == tc_variants
     assert all(v >= 3 for v in best.values()), sorted((v, k) for k, v in best.items() if v < 3)
 
