@@ -14,6 +14,7 @@
 #include "conv_ps.cuh"
 #include "attention_tma.cuh"
 #include "elementwise.cuh"
+#include "grad.cuh"
 #include "mha.cuh"
 
 namespace {
@@ -207,6 +208,33 @@ int validate(const cds_op& op, Step* out) {
         return fail(CDS_ERR_INVALID, "cast: bad arguments");
       return CDS_OK;
     }
+    case CDS_OP_STASH: {
+      const cds_stash_op& t = op.u.stash;
+      if (t.n <= 0 || !t.src || !t.dst) return fail(CDS_ERR_INVALID, "stash: bad arguments");
+      if (t.act_out && t.act != CDS_ACT_NONE && t.act != CDS_ACT_MISH) return fail(CDS_ERR_UNSUPPORTED, "stash: act %d", t.act);
+      return CDS_OK;
+    }
+    case CDS_OP_UPDATE_BWD: {
+      const cds_update_bwd_op& u = op.u.update_bwd;
+      if (u.batch <= 0 || u.row <= 0 || !u.gx || !u.gpred || !u.x || !u.pred || !u.coef)
+        return fail(CDS_ERR_INVALID, "update_bwd: bad arguments");
+      return CDS_OK;
+    }
+    case CDS_OP_DGRAD: {
+      const cds_dgrad_op& d = op.u.dgrad;
+      if (d.rows <= 0 || d.N <= 0 || d.K <= 0 || !d.dz || !d.w || !d.out || d.ldz < d.N || d.ldw < d.K || d.ldo < d.K)
+        return fail(CDS_ERR_INVALID, "dgrad: bad arguments");
+      if (d.act != CDS_ACT_NONE && d.act != CDS_ACT_MISH) return fail(CDS_ERR_UNSUPPORTED, "dgrad: act %d", d.act);
+      if (d.act == CDS_ACT_MISH && !d.z) return fail(CDS_ERR_INVALID, "dgrad: Mish derivative without a pre-activation");
+      return CDS_OK;
+    }
+    case CDS_OP_WGRAD: {
+      const cds_wgrad_op& w = op.u.wgrad;
+      if (w.rows <= 0 || w.N <= 0 || w.K <= 0 || !w.dz || !w.h || !w.dw || w.ldz < w.N || w.ldh < w.K || w.lddw < w.K)
+        return fail(CDS_ERR_INVALID, "wgrad: bad arguments");
+      if (w.act != CDS_ACT_NONE && w.act != CDS_ACT_MISH) return fail(CDS_ERR_UNSUPPORTED, "wgrad: act %d", w.act);
+      return CDS_OK;
+    }
     default:
       return fail(CDS_ERR_INVALID, "unknown operator kind %d", op.kind);
   }
@@ -253,6 +281,26 @@ int launch(const Step& s, const int* iter_ptr, int sm_count, cudaStream_t st, in
       CDS_CUDA(cudaGetLastError());
       return CDS_OK;
     }
+    case CDS_OP_STASH: {
+      const cds_stash_op& t = s.op.u.stash;
+      cds::stash_kernel<<<elementwise_grid(t.n, sm_count), 256, 0, st>>>(t, iter_ptr);
+      CDS_CUDA(cudaGetLastError());
+      return CDS_OK;
+    }
+    case CDS_OP_UPDATE_BWD: {
+      const cds_update_bwd_op& u = s.op.u.update_bwd;
+      cds::update_bwd_kernel<<<elementwise_grid((int64_t)u.batch * u.row, sm_count), 256, 0, st>>>(u, iter_ptr);
+      CDS_CUDA(cudaGetLastError());
+      return CDS_OK;
+    }
+    case CDS_OP_DGRAD:
+      cds::dgrad_kernel<<<cds::dgrad_grid(s.op.u.dgrad), 256, 0, st>>>(s.op.u.dgrad, iter_ptr);
+      CDS_CUDA(cudaGetLastError());
+      return CDS_OK;
+    case CDS_OP_WGRAD:
+      cds::wgrad_kernel<<<cds::wgrad_grid(s.op.u.wgrad), 256, 0, st>>>(s.op.u.wgrad, iter_ptr);
+      CDS_CUDA(cudaGetLastError());
+      return CDS_OK;
   }
   return fail(CDS_ERR_INVALID, "unknown operator kind");
 }
@@ -275,6 +323,10 @@ int preload_kernels() {
   CDS_CUDA(cudaFuncGetAttributes(&a, cds::cm_prep_kernel));
   CDS_CUDA(cudaFuncGetAttributes(&a, cds::cast_pad_kernel));
   CDS_CUDA(cudaFuncGetAttributes(&a, cds::ln_modulate_kernel));
+  CDS_CUDA(cudaFuncGetAttributes(&a, cds::stash_kernel));
+  CDS_CUDA(cudaFuncGetAttributes(&a, cds::update_bwd_kernel));
+  CDS_CUDA(cudaFuncGetAttributes(&a, cds::dgrad_kernel));
+  CDS_CUDA(cudaFuncGetAttributes(&a, cds::wgrad_kernel));
   CDS_CUDA(cudaFuncGetAttributes(&a, cds::set_iter_kernel));
   CDS_CUDA(cudaFuncGetAttributes(&a, cds::advance_iter_kernel));
   return CDS_OK;
@@ -298,6 +350,10 @@ long long* conv_tc_trace_hook(int grid) {
 
 // CDS_OP_MHA was added without a layout change: the union keeps its size
 static_assert(sizeof(cds_mha_op) <= sizeof(cds_conv_op), "cds_mha_op must not grow the cds_op union");
+// ... and neither do the backward operators (the ABI version was bumped for the new kinds, not for a new layout)
+static_assert(sizeof(cds_stash_op) <= sizeof(cds_conv_op) && sizeof(cds_update_bwd_op) <= sizeof(cds_conv_op) &&
+              sizeof(cds_dgrad_op) <= sizeof(cds_conv_op) && sizeof(cds_wgrad_op) <= sizeof(cds_conv_op),
+              "backward operators must not grow the cds_op union");
 
 struct cds_plan {
   int device = 0;

@@ -237,6 +237,8 @@ class ContinuousConsistencyModel(DiffusionModel):
         order = list(reversed([1] * diffusion_x_sampling_steps + list(range(1, sample_steps))))
 
         from ..engine import runtime
+        if requires_grad:
+            runtime.grad_fallback(self)
         if not (requires_grad or preserve_history) and runtime._device_ok(torch.device(self.device)):
             out = runtime.try_sample_consistency(self, model=model, xt=xt, prior=prior, sigmas=sigmas, order=order,
                                                  cond_emb=cvec, n_samples=n_samples,

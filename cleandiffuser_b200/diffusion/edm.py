@@ -158,6 +158,8 @@ class ContinuousEDM(DiffusionModel):
         guided = self.classifier is not None and w_cg != 0.0 and condition_cg is not None
         from ..engine import runtime
         done = False
+        if requires_grad:
+            runtime.grad_fallback(self)
         if not (requires_grad or preserve_history or guided) and runtime._device_ok(torch.device(self.device)):
             out = runtime.try_sample_edm(self, model=model, xt=xt, prior=prior, solver=solver, sigmas=sigmas, order=order,
                                          cond_emb=cvec, w_cfg=w_cfg, n_samples=n_samples,

@@ -177,6 +177,8 @@ class DDPM(DiffusionModel):
 
         guided = self.classifier is not None and w_cg != 0.0 and condition_cg is not None
         from ..engine import runtime
+        if requires_grad:
+            runtime.grad_fallback(self)
         if not (requires_grad or preserve_history or guided) and runtime._device_ok(torch.device(self.device)):
             rows, slots, t_all = self._engine_table(extra_sample_steps)
             out = runtime.try_sample(self, model=model, xt=xt, prior=prior.to(self.device), solver="legacy_ddpm",

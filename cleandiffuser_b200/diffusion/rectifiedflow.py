@@ -73,6 +73,8 @@ class _RectifiedFlow(DiffusionModel):
         """``t_of(i)`` = the network's time input of loop index i, ``dt_of(i)`` = t_i - t_{i-1} (0-d tensors)."""
         order = list(reversed([1] * diffusion_x_sampling_steps + list(range(1, sample_steps + 1))))
         from ..engine import runtime
+        if requires_grad:
+            runtime.grad_fallback(self)
         if not (requires_grad or preserve_history) and runtime._device_ok(torch.device(self.device)):
             rows = torch.zeros((len(order), S.ROW), dtype=torch.float32)
             for n, i in enumerate(order):

@@ -4,13 +4,14 @@ Same constructor / ``sample()`` / ``update()`` / ``loss()`` / ``add_noise()`` su
 cleandiffuser/diffusion/diffusionsde.py (:35-245 base, :247-606 discrete, :609-952 continuous).
 
 ``sample()`` is a dispatcher.  When the model lives on a CUDA device, the backbone is one the
-engine can lower (JannerUNet1d / ChiUNet1d / DiT1d / DQLMlp), gradients are not requested and no
-per-step Python hook is needed (classifier guidance, history capture), the whole reverse loop
-runs as one replayed CUDA-graph of hand-written sm_90a kernels with x_t resident on the device
-(``engine/runtime.py``).  Everything else -- CPU tensors, user-defined backbones,
-``requires_grad=True`` (Diffusion-QL back-propagates through the loop), classifier guidance,
-``preserve_history`` -- takes the PyTorch loop below, which is step-for-step the reference
-algorithm and is pinned against the reference's goldens on CPU (tests/test_host_golden.py).
+engine can lower (JannerUNet1d / ChiUNet1d / DiT1d / DQLMlp) and no per-step Python hook is needed
+(history capture), the whole reverse loop runs as one replayed CUDA-graph of hand-written sm_90a
+kernels with x_t resident on the device (``engine/runtime.py``).  ``requires_grad=True`` (Diffusion-QL
+back-propagates through the loop) runs on the engine for DQLMlp with the first-order solvers, a
+forward and a backward program (``runtime.try_sample_grad``).  Everything else -- CPU tensors,
+user-defined backbones, other ``requires_grad=True`` requests, ``preserve_history`` -- takes the
+PyTorch loop below, which is step-for-step the reference algorithm and is pinned against the
+reference's goldens on CPU (tests/test_host_golden.py).
 """
 from typing import Callable, Dict, Optional, Union
 
@@ -164,7 +165,16 @@ class BaseDiffusionSDE(DiffusionModel):
         hs, stds = S.schedule_tables(alphas, sigmas, sample_steps, self.device)
         order = S.loop_indices(sample_steps, diffusion_x_sampling_steps)
 
-        if engine_ok:
+        if engine_ok and requires_grad:
+            # differentiable loop on the engine (Diffusion-QL's actor loss): x0 comes back connected to autograd
+            from ..engine import runtime
+            out = runtime.try_sample_grad(self, model=model, xt=xt, prior=prior, solver=solver, sample_steps=sample_steps,
+                                          order=order, step_values=step_values, alphas=alphas, sigmas=sigmas, hs=hs, stds=stds,
+                                          cond_emb=condition_vec_cfg, w_cfg=w_cfg, n_samples=n_samples,
+                                          guided=self.classifier is not None and w_cg != 0.0, sched_id=sched_id)
+            if out is not None:
+                return out
+        elif engine_ok:
             from ..engine import runtime
             guide = None
             if self.classifier is not None and w_cg != 0.0:
@@ -202,7 +212,7 @@ class BaseDiffusionSDE(DiffusionModel):
 
     def _engine_candidate(self, requires_grad, preserve_history, w_cg, warm_start_reference):
         """Cheap host-side screen; the detailed backbone/shape screen lives in engine/runtime.py."""
-        if requires_grad or preserve_history:
+        if preserve_history:
             return False
         from ..engine import runtime
         return runtime._device_ok(torch.device(self.device))

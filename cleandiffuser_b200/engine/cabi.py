@@ -10,10 +10,11 @@ import os
 
 _LIB_PATH = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "csrc", "libcds.so")
 
-ABI_VERSION = 5
+ABI_VERSION = 6
 OPF_BRANCH_SHIFT = 8   # cds_op.flags bits 8..15: branch index (independent chains run on parallel streams)
 OPF_ONCE = 1          # cds_op.flags: run once per plan run (before its first iteration), not in every iteration
 OP_CONV, OP_UPDATE, OP_LNMOD, OP_ATTN, OP_PREP, OP_CAST, OP_MHA = range(7)
+OP_STASH, OP_UPDATE_BWD, OP_DGRAD, OP_WGRAD = 7, 8, 9, 10      # backward operators of a differentiable loop (csrc/grad.cuh)
 ACT_NONE, ACT_MISH, ACT_SILU, ACT_GELU_TANH, ACT_MISH_SILU, ACT_LEAKY_RELU, ACT_GELU_ERF = range(7)
 MATH_FP32, MATH_BF16_TC, MATH_TF32_TC = 0, 1, 2
 TC_MODES = (MATH_BF16_TC, MATH_TF32_TC)
@@ -90,9 +91,34 @@ class UpdateOp(C.Structure):
     ]
 
 
+class StashOp(C.Structure):
+    _fields_ = [("n", C.c_int64), ("act", C.c_int32), ("src", _f32p), ("dst", _f32p), ("dst_iter_stride", C.c_int64),
+                ("act_out", _f32p)]
+
+
+class UpdateBwdOp(C.Structure):
+    _fields_ = [("batch", C.c_int32), ("row", C.c_int32), ("gx", _f32p), ("gpred", _f32p),
+                ("x", _f32p), ("x_iter_stride", C.c_int64), ("pred", _f32p), ("pred_iter_stride", C.c_int64),
+                ("mask", _f32p), ("x_min", _f32p), ("x_max", _f32p), ("coef", _f32p), ("coef_iter_stride", C.c_int64),
+                ("predict_noise", C.c_int32)]
+
+
+class DgradOp(C.Structure):
+    _fields_ = [("rows", C.c_int32), ("N", C.c_int32), ("K", C.c_int32), ("dz", _f32p), ("ldz", C.c_int32),
+                ("w", _f32p), ("ldw", C.c_int32), ("z", _f32p), ("z_iter_stride", C.c_int64),
+                ("act", C.c_int32), ("accumulate", C.c_int32), ("out", _f32p), ("ldo", C.c_int32), ("out_sum", _f32p)]
+
+
+class WgradOp(C.Structure):
+    _fields_ = [("rows", C.c_int32), ("N", C.c_int32), ("K", C.c_int32), ("dz", _f32p), ("ldz", C.c_int32),
+                ("h", _f32p), ("h_iter_stride", C.c_int64), ("ldh", C.c_int32), ("act", C.c_int32),
+                ("dw", _f32p), ("lddw", C.c_int32), ("db", _f32p), ("db_iter_stride", C.c_int64), ("accumulate", C.c_int32)]
+
+
 class _OpUnion(C.Union):
     _fields_ = [("conv", ConvOp), ("update", UpdateOp), ("lnmod", LnModOp), ("attn", AttnOp), ("prep", PrepOp),
-                ("cast", CastOp), ("mha", MhaOp)]
+                ("cast", CastOp), ("mha", MhaOp), ("stash", StashOp), ("update_bwd", UpdateBwdOp), ("dgrad", DgradOp),
+                ("wgrad", WgradOp)]
 
 
 class Op(C.Structure):

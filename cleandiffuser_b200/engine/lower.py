@@ -570,6 +570,108 @@ def lower_dql(p: Program, net: nn.Module, x: View, has_cond: bool, in_batch_mod:
     return p.conv(h, w_linear(fl.weight), out, bias=_const_vec(p.packed(lambda: fl.bias)))
 
 
+# =============================================================================== DQLMlp, differentiable
+def _rev(stash: torch.Tensor):
+    """(pointer, signed stride) that walks the [n_iters, ...] stash from its last slot to its first: backward iteration m reads
+    the slot of forward iteration n_iters - 1 - m."""
+    per = stash[0].numel()
+    return stash.data_ptr() + 4 * per * (stash.shape[0] - 1), -per
+
+
+class DQLGrad:
+    """DQLMlp under ``sample(requires_grad=True)``: a forward program that keeps what the backward needs and the backward
+    program over the same buffers.
+
+    Forward, per iteration n (the reverse loop's network evaluation; the runtime appends the solver update):
+        stash x_n;  z1 = W_x x_n + step_tab[n] + samp_tab[b]  (Linear, no activation);  stash z1, h1 = Mish(z1)  (one operator);
+        z2, z3 alike;  pred = W_f h3 + b_f;  stash pred  (raw: clip_prediction happens in the update)
+    Backward, per iteration m = n_iters-1 .. 0 walking the stashes in reverse (the runtime puts the update's backward first; it
+    turns d x_{n+1} in ``gx`` into d pred in ``gpred`` and the direct part of d x_n in ``gx``):
+        d W_f, d b_f += Mish(z3)^T gpred;  dz3 = (gpred W_f) Mish'(z3);  ... layer 3, layer 2 alike ... ;
+        d step_tab[n] = sum_rows dz1 (with d W_x += x_n^T dz1: W_x's "bias" is the per-iteration table row);
+        d samp_tab += dz1;  gx += dz1 W_x
+    ``step_tab`` / ``samp_tab`` are filled by the caller (they are autograd inputs: d step_tab carries into time_mlp, the time
+    columns of mid_layer[0] and its bias, d samp_tab into the observation columns and the condition)."""
+
+    def __init__(self, p: Program, bp: Program, net: nn.Module, x: View):
+        R, n, a = p.rows, p.n_iters, x.C
+        lins = [net.mid_layer[0], net.mid_layer[2], net.mid_layer[4], net.final_layer]
+        widths = [lin.out_features for lin in lins[:3]]
+        self.step_tab, self.samp_tab = p.buf(n, widths[0]), p.buf(R, widths[0])
+        self.xs, self.ps = p.buf(n, R, a), p.buf(n, R, a)
+        self.zs = [p.buf(n, R, w) for w in widths]
+
+        def stash(src: View, dst: torch.Tensor, act_out: Optional[View] = None):
+            op = cabi.Op()
+            op.kind = cabi.OP_STASH
+            s = op.u.stash
+            s.n, s.src, s.dst, s.dst_iter_stride = R * src.C, src.ptr, dst.data_ptr(), dst[0].numel()
+            if act_out is not None:
+                s.act_out, s.act = act_out.ptr, cabi.ACT_MISH
+            p.ops.append(op)
+
+        stash(x, self.xs)
+        h = x
+        for k, lin in enumerate(lins[:3]):
+            z = View(p.buf(R, 1, widths[k]), 1, widths[k])
+            if k == 0:
+                p.conv(x, w_linear(lin.weight, slice(0, a)), z, bias=_vec(self.step_tab, self.samp_tab))
+            else:
+                p.conv(h, w_linear(lin.weight), z, bias=_const_vec(p.packed(lambda m=lin: m.bias)))
+            h = View(p.buf(R, 1, widths[k]), 1, widths[k])
+            stash(z, self.zs[k], h)
+        fl = lins[3]
+        self.pred = View(p.buf(R, 1, a), 1, a)
+        p.conv(h, w_linear(fl.weight), self.pred, bias=_const_vec(p.packed(lambda: fl.bias)))
+        stash(self.pred, self.ps)
+
+        # ---- backward program
+        self.gx, self.gpred = bp.buf(R, a), bp.buf(R, a)
+        dz = [bp.buf(R, w) for w in widths]
+        wts = [bp.packed(lambda: lins[0].weight[:, :a])] + [bp.packed(lambda m=lin: m.weight) for lin in lins[1:]]
+        self.g_w = [bp.buf(*w.shape) for w in wts]                        # d W_x, d W2, d W3, d W_f
+        self.g_b = [None] + [bp.buf(lin.out_features) for lin in lins[1:]]
+        self.g_step, self.g_samp = bp.buf(n, widths[0]), bp.buf(R, widths[0])
+        self.accumulators = self.g_w + self.g_b[1:] + [self.g_step, self.g_samp]
+
+        def wgrad(k: int, dzk: torch.Tensor, h_src: torch.Tensor, act: int):
+            op = cabi.Op()
+            op.kind = cabi.OP_WGRAD
+            g = op.u.wgrad
+            N, K = wts[k].shape
+            g.rows, g.N, g.K, g.dz, g.ldz = R, N, K, dzk.data_ptr(), N
+            g.h, g.h_iter_stride = _rev(h_src)
+            g.ldh, g.act = K, act
+            g.dw, g.lddw, g.accumulate = self.g_w[k].data_ptr(), K, 1
+            if k == 0:
+                g.db, g.db_iter_stride = _rev(self.g_step)
+            else:
+                g.db, g.db_iter_stride = self.g_b[k].data_ptr(), 0
+            bp.ops.append(op)
+
+        def dgrad(k: int, dzk: torch.Tensor, out: torch.Tensor, z_src: Optional[torch.Tensor], accumulate=0, out_sum=None):
+            op = cabi.Op()
+            op.kind = cabi.OP_DGRAD
+            d = op.u.dgrad
+            N, K = wts[k].shape
+            d.rows, d.N, d.K, d.dz, d.ldz, d.w, d.ldw = R, N, K, dzk.data_ptr(), N, wts[k].data_ptr(), K
+            if z_src is not None:
+                d.z, d.z_iter_stride = _rev(z_src)
+                d.act = cabi.ACT_MISH
+            d.accumulate, d.out, d.ldo = accumulate, out.data_ptr(), K
+            if out_sum is not None:
+                d.out_sum = out_sum.data_ptr()
+            bp.ops.append(op)
+
+        upstream = self.gpred
+        for k in (3, 2, 1):
+            wgrad(k, upstream, self.zs[k - 1], cabi.ACT_MISH)
+            dgrad(k, upstream, dz[k - 1], self.zs[k - 1], out_sum=self.g_samp if k == 1 else None)
+            upstream = dz[k - 1]
+        wgrad(0, upstream, self.xs, cabi.ACT_NONE)
+        dgrad(0, upstream, self.gx, None, accumulate=1)
+
+
 # =============================================================================== IDQLMlp
 def lower_idql(p: Program, net: nn.Module, x: View, has_cond: bool, in_batch_mod: int) -> View:
     """idqlmlp.py:21-65.  affine_in over cat[x, time_mlp(t), obs] splits like DQLMlp's first Linear (per-iteration row +

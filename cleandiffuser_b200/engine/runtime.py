@@ -26,9 +26,10 @@ import types
 from typing import Optional
 
 import torch
+import torch.nn.functional as F
 
 from . import cabi
-from .lower import Program, Unsupported, View, lower_denoiser
+from .lower import DQLGrad, Program, Unsupported, View, _rev, lower_denoiser
 from ..diffusion import solvers as S
 
 STATS = {"engine_calls": 0, "fallbacks": 0, "last_fallback_reason": None, "launches": 0}
@@ -372,6 +373,57 @@ def try_sample(agent, *, model, xt, prior, solver, sample_steps, order, step_val
         # the update operator combines the two CFG branches itself; a guidance term would have to enter after that combine
         return _fallback("classifier guidance together with two-branch classifier-free guidance")
 
+    table, n_slots, t_cpu, sched_key, order, table_given = _step_table(
+        agent, solver=solver, sample_steps=sample_steps, order=order, step_values=step_values, alphas=alphas, sigmas=sigmas,
+        hs=hs, stds=stds, table=table, sched_id=sched_id)
+    keep_history = (not table_given) and S.solver_keeps_history(solver)
+    has_mask = isinstance(agent.fix_mask, torch.Tensor)
+    has_min, has_max = (agent.x_min is not None and clip_in_loop), (agent.x_max is not None and clip_in_loop)
+    pn = bool(agent.predict_noise) if predict_noise is None else bool(predict_noise)
+    math = _math_mode()
+    row_elems = 1
+    for s_ in x_shape:
+        row_elems *= s_
+    # noise tape: all draws of the loop up front when they fit the budget, else as many slots as fit (the loop then runs in
+    # chunks with the tape refilled in between -- O(budget) memory instead of O(sample_steps x batch x row))
+    tape_slots = min(n_slots, max(1, _tape_budget_bytes() // (4 * batch * row_elems))) if n_slots > 0 else 0
+    key = ("sde", id(net), batch, x_shape, len(order), tape_slots, cfg_mode, pn, has_mask,
+           has_min, has_max, keep_history, math, float(w_cfg) if cfg_mode == 2 else 0.0)
+
+    def factory():
+        plan = SamplerPlan(device, net, batch, x_shape, len(order), tape_slots, cfg_mode=cfg_mode,
+                           predict_noise=pn, has_mask=has_mask, has_min=has_min, has_max=has_max,
+                           keep_history=keep_history, math=math)
+        plan.build(w_cfg)
+        return plan
+
+    try:
+        plan = _get_plan(agent, key, factory)
+    except Unsupported as e:
+        return _fallback(str(e))
+    except cabi.CdsError as e:
+        if e.code == -3:
+            return _fallback(str(e))
+        raise
+
+    t_all = _load_resident(agent, plan, xt, prior, table, sched_key, tape_slots, n_slots, x_shape, order, t_cpu, device)
+    # the loop's draws: same calls, same order, same shapes as the reference loop's (diffusionsde.py:548,571,...)
+    t_key = (t_cpu.numpy().tobytes(), tuple(order))
+    if guide is not None:
+        if plan.n_branches != 1 or getattr(plan, "pred", None) is None:
+            return _fallback("guided sampling needs a single-branch program with a dense prediction buffer")
+        slots = plan.coef[:, S.R_NOISE].cpu().tolist()              # tape slot per iteration as the update kernel sees it
+        plan.run_guided(t_all, cond_emb, xt, slots, lambda n, x, p: guide(n, order[n], x, p), t_key=t_key)
+    else:
+        plan.run_chunked(t_all, cond_emb, xt, (table[:, S.R_NOISE] > 0).tolist(),
+                         use_graph=os.environ.get("CDS_GRAPH", "1") != "0", t_key=t_key)
+    STATS["engine_calls"] += 1
+    return plan.x.clone()
+
+
+def _step_table(agent, *, solver, sample_steps, order, step_values, alphas, sigmas, hs, stds, table, sched_id):
+    """The coefficient table of one ``sample()`` call -> ``(table [n_iters, ROW], number of noise slots, time per step (CPU),
+    schedule key, iteration order, table_given)``."""
     # ---- per-iteration scalars (host, reference op order); identical requests reuse the table (building it costs ~10 ms
     # of Python scalar arithmetic for 100 steps -- more than a tenth of a whole cfg2 sample() on the engine) ---------------
     table_given = table is not None
@@ -416,37 +468,11 @@ def try_sample(agent, *, model, xt, prior, solver, sample_steps, order, step_val
         agent._engine_tables[sched_key] = (table, n_slots)
     else:
         table, n_slots = cached
-    keep_history = (not table_given) and S.solver_keeps_history(solver)
-    has_mask = isinstance(agent.fix_mask, torch.Tensor)
-    has_min, has_max = (agent.x_min is not None and clip_in_loop), (agent.x_max is not None and clip_in_loop)
-    pn = bool(agent.predict_noise) if predict_noise is None else bool(predict_noise)
-    math = _math_mode()
-    row_elems = 1
-    for s_ in x_shape:
-        row_elems *= s_
-    # noise tape: all draws of the loop up front when they fit the budget, else as many slots as fit (the loop then runs in
-    # chunks with the tape refilled in between -- O(budget) memory instead of O(sample_steps x batch x row))
-    tape_slots = min(n_slots, max(1, _tape_budget_bytes() // (4 * batch * row_elems))) if n_slots > 0 else 0
-    key = ("sde", id(net), batch, x_shape, len(order), tape_slots, cfg_mode, pn, has_mask,
-           has_min, has_max, keep_history, math, float(w_cfg) if cfg_mode == 2 else 0.0)
+    return table, n_slots, t_cpu, sched_key, order, table_given
 
-    def factory():
-        plan = SamplerPlan(device, net, batch, x_shape, len(order), tape_slots, cfg_mode=cfg_mode,
-                           predict_noise=pn, has_mask=has_mask, has_min=has_min, has_max=has_max,
-                           keep_history=keep_history, math=math)
-        plan.build(w_cfg)
-        return plan
 
-    try:
-        plan = _get_plan(agent, key, factory)
-    except Unsupported as e:
-        return _fallback(str(e))
-    except cabi.CdsError as e:
-        if e.code == -3:
-            return _fallback(str(e))
-        raise
-
-    # ---- fill the resident buffers ----------------------------------------------------------------------
+def _load_resident(agent, plan, xt, prior, table, sched_key, tape_slots, n_slots, x_shape, order, t_cpu, device):
+    """Fill the plan's resident buffers (x_t, coefficient rows, mask, clip bounds) -> the time value of every iteration."""
     with torch.no_grad():
         plan.x.copy_(xt)
         if getattr(plan, "_coef_key", None) != sched_key:
@@ -458,27 +484,15 @@ def try_sample(agent, *, model, xt, prior, solver, sample_steps, order, step_val
             else:
                 plan.coef.copy_(table)
             plan._coef_key = sched_key
-        if has_mask:
+        if plan.mask is not None:
             plan.prior.copy_(prior)
             plan.mask.copy_(_row(agent.fix_mask, x_shape, device))
-        if has_min:
+        if plan.x_min is not None:
             plan.x_min.copy_(_row(agent.x_min, x_shape, device))
-        if has_max:
+        if plan.x_max is not None:
             plan.x_max.copy_(_row(agent.x_max, x_shape, device))
         idx = torch.as_tensor(order, dtype=torch.long)
-        t_all = t_cpu[idx].to(device)      # int64 (discrete) or float32 (continuous), one entry per iteration
-    # the loop's draws: same calls, same order, same shapes as the reference loop's (diffusionsde.py:548,571,...)
-    t_key = (t_cpu.numpy().tobytes(), tuple(order))
-    if guide is not None:
-        if plan.n_branches != 1 or getattr(plan, "pred", None) is None:
-            return _fallback("guided sampling needs a single-branch program with a dense prediction buffer")
-        slots = plan.coef[:, S.R_NOISE].cpu().tolist()              # tape slot per iteration as the update kernel sees it
-        plan.run_guided(t_all, cond_emb, xt, slots, lambda n, x, p: guide(n, order[n], x, p), t_key=t_key)
-    else:
-        plan.run_chunked(t_all, cond_emb, xt, (table[:, S.R_NOISE] > 0).tolist(),
-                         use_graph=os.environ.get("CDS_GRAPH", "1") != "0", t_key=t_key)
-    STATS["engine_calls"] += 1
-    return plan.x.clone()
+        return t_cpu[idx].to(device)      # int64 (discrete) or float32 (continuous), one entry per iteration
 
 
 def try_sample_consistency(agent, *, model, xt, prior, sigmas, order, cond_emb, n_samples, sched_id=None):
@@ -647,6 +661,195 @@ def try_sample_edm(agent, *, model, xt, prior, solver, sigmas, order, cond_emb, 
     plan.run(t_all, cond_emb, use_graph=os.environ.get("CDS_GRAPH", "1") != "0")
     STATS["engine_calls"] += 1
     return plan.x.clone()
+
+
+# ============================================================================ differentiable sampling (requires_grad=True)
+class GradSamplerPlan(SamplerPlan):
+    """The resident state of ``sample(requires_grad=True)`` over DQLMlp: a forward program (``lower.DQLGrad``'s network
+    operators, which stash x_n, the hidden pre-activations and the raw prediction of every iteration, then the solver update)
+    and a backward program that walks the iterations in reverse.  Each is one cds_plan replayed from a CUDA graph.  One branch,
+    no CFG combine, no solver history."""
+
+    def __init__(self, device, net, batch, x_shape, n_iters, n_slots, *, predict_noise, has_mask, has_min, has_max, math):
+        self.device, self.net, self.batch, self.x_shape = device, net, batch, tuple(x_shape)
+        row = x_shape[0]
+        self.row, self.n_iters, self.cfg_mode, self.n_branches = row, n_iters, 1, 1
+        root = Program(device, batch, n_iters, math)
+        back = Program(device, batch, n_iters, math)
+        self.program, self.back = root, back
+        self.x = root.buf(batch, row)
+        self.prior = root.buf(batch, row) if has_mask else None
+        self.mask = root.buf(row) if has_mask else None
+        self.x_min = root.buf(row) if has_min else None
+        self.x_max = root.buf(row) if has_max else None
+        self.coef = root.buf(n_iters, cabi.ROW_FLOATS)
+        self.noise = root.buf(max(n_slots, 1), batch, row) if n_slots > 0 else None
+        self.grad = g = DQLGrad(root, back, net, View(self.x, 1, row))
+        self.pred = g.pred.t
+
+        op = cabi.Op()
+        op.kind = cabi.OP_UPDATE
+        u = op.u.update
+        u.batch, u.row, u.x, u.pred = batch, row, self.x.data_ptr(), g.pred.ptr
+        if self.noise is not None:
+            u.noise, u.noise_slot_stride = self.noise.data_ptr(), batch * row
+        u.prior = self.prior.data_ptr() if has_mask else None
+        u.mask = self.mask.data_ptr() if has_mask else None
+        u.x_min = self.x_min.data_ptr() if has_min else None
+        u.x_max = self.x_max.data_ptr() if has_max else None
+        u.coef = self.coef.data_ptr()
+        u.predict_noise = 1 if predict_noise else 0
+        root.ops.append(op)
+        self._update_ops = [op]
+
+        bop = cabi.Op()                                      # the update's backward opens every backward iteration
+        bop.kind = cabi.OP_UPDATE_BWD
+        b = bop.u.update_bwd
+        b.batch, b.row, b.gx, b.gpred = batch, row, g.gx.data_ptr(), g.gpred.data_ptr()
+        b.x, b.x_iter_stride = _rev(g.xs)
+        b.pred, b.pred_iter_stride = _rev(g.ps)
+        b.mask = u.mask
+        b.x_min, b.x_max = u.x_min, u.x_max
+        b.coef, b.coef_iter_stride = _rev(self.coef)
+        b.predict_noise = u.predict_noise
+        back.ops.insert(0, bop)
+
+        self._fillers = []                 # the tables are autograd inputs, copied in by _GradSampleFn
+        self.handle: Optional[cabi.Plan] = None
+        self.back_handle: Optional[cabi.Plan] = None
+        self.version = None
+        self.generation = 0                # forward runs so far: a backward must belong to the latest one
+
+    def build(self, w_cfg: float):
+        super().build(w_cfg)
+        self.back_handle = _make_handle(self.device, self.back.ops, self.n_iters)
+
+    def refresh_weights(self, epoch: int = 0):
+        v = _weights_version(self.net, epoch)
+        if self.version is None:
+            self.version = v
+        elif v != self.version:
+            for fn in self.program.packers + self.back.packers:
+                fn()
+            self.version = v
+
+    def close(self):
+        super().close()
+        if self.back_handle is not None:
+            self.back_handle.close()
+            self.back_handle = None
+
+    def backward(self, grad_x0, generation):
+        """d x0 -> the gradients of the Function's inputs (step_tab, samp_tab, W_x, W2, b2, W3, b3, W_f, b_f)."""
+        if generation != self.generation:
+            raise RuntimeError("the engine's saved iterations of this sample(requires_grad=True) call were overwritten by a later "
+                               "call with the same shapes; call backward() before sampling again")
+        g = self.grad
+        with torch.no_grad():
+            for t in g.accumulators:
+                t.zero_()
+            g.gx.copy_(grad_x0.reshape(g.gx.shape))
+        stream = torch.cuda.current_stream(self.device).cuda_stream if self.device.type == "cuda" else 0
+        self.back_handle.run(0, self.n_iters, stream, os.environ.get("CDS_GRAPH", "1") != "0")
+        STATS["backward_launches"] = self.back_handle.launches_per_iter() * self.n_iters + 1
+        return (g.g_step.clone(), g.g_samp.clone(), g.g_w[0].clone(), g.g_w[1].clone(), g.g_b[1].clone(),
+                g.g_w[2].clone(), g.g_b[2].clone(), g.g_w[3].clone(), g.g_b[3].clone())
+
+
+class _GradSampleFn(torch.autograd.Function):
+    """x0 of the engine's reverse loop as a function of the per-call tables and the DQLMlp weights the loop reads."""
+
+    @staticmethod
+    def forward(ctx, plan, run, step_tab, samp_tab, w_x, w2, b2, w3, b3, w_f, b_f):
+        plan.grad.step_tab.copy_(step_tab)
+        plan.grad.samp_tab.copy_(samp_tab)
+        run()
+        plan.generation += 1
+        ctx.plan, ctx.generation = plan, plan.generation
+        return plan.x.clone()
+
+    @staticmethod
+    def backward(ctx, grad_x0):
+        return (None, None) + ctx.plan.backward(grad_x0, ctx.generation)
+
+
+def grad_fallback(agent):
+    """``requires_grad=True`` on a sampler class that has no differentiable engine program: recorded (raised under
+    CDS_BACKEND=cuda) like every other fallback; the caller then runs its PyTorch loop, which autograd differentiates."""
+    if _backend() != "torch" and _device_ok(_device_of(agent)):
+        return _fallback(f"requires_grad=True: {type(agent).__name__} has no differentiable engine program")
+    return None
+
+
+def try_sample_grad(agent, *, model, xt, prior, solver, sample_steps, order, step_values, alphas, sigmas, hs, stds,
+                    cond_emb, w_cfg, n_samples, guided=False, sched_id=None):
+    """``sample(requires_grad=True)`` on the engine: x0 connected to autograd through ``_GradSampleFn``.  Covers DQLMlp with
+    the DDPM / DDIM / first-order DPM-Solver updates, one CFG branch and CDS_MATH = fp32 | tf32; everything else takes the
+    PyTorch loop (which autograd differentiates) through ``_fallback``."""
+    if _backend() == "torch":
+        return None
+    device = _device_of(agent)
+    if not _device_ok(device) or xt.dtype != torch.float32:
+        return None
+    net = model["diffusion"]
+    name = type(net).__name__
+    if name != "DQLMlp" or xt.dim() != 2:
+        return _fallback(f"requires_grad=True: backbone {name} has no differentiable engine program (DQLMlp only)")
+    if S.solver_keeps_history(solver):
+        return _fallback(f"requires_grad=True with the multistep solver {solver} (history)")
+    cfg_mode = _cfg_mode(w_cfg, cond_emb)
+    if cfg_mode is None or cfg_mode == 2:
+        return _fallback("requires_grad=True with two-branch classifier-free guidance")
+    if guided:
+        return _fallback("requires_grad=True with classifier guidance")
+    math = _math_mode()
+    if math == cabi.MATH_BF16_TC:
+        return _fallback("requires_grad=True with CDS_MATH=bf16 (fp32 and tf32 only)")
+    batch, x_shape = xt.shape[0], tuple(xt.shape[1:])
+    if n_samples != batch:
+        return _fallback("n_samples != prior.shape[0]")
+
+    table, n_slots, t_cpu, sched_key, order, _ = _step_table(
+        agent, solver=solver, sample_steps=sample_steps, order=order, step_values=step_values, alphas=alphas, sigmas=sigmas,
+        hs=hs, stds=stds, table=None, sched_id=sched_id)
+    has_mask = isinstance(agent.fix_mask, torch.Tensor)
+    has_min, has_max = agent.x_min is not None, agent.x_max is not None
+    pn = bool(agent.predict_noise)
+    tape_slots = min(n_slots, max(1, _tape_budget_bytes() // (4 * batch * x_shape[0]))) if n_slots > 0 else 0
+    key = ("sde", id(net), batch, x_shape, len(order), tape_slots, cfg_mode, pn, has_mask, has_min, has_max, False, math, 0.0,
+           "grad")
+
+    def factory():
+        plan = GradSamplerPlan(device, net, batch, x_shape, len(order), tape_slots, predict_noise=pn, has_mask=has_mask,
+                               has_min=has_min, has_max=has_max, math=math)
+        plan.build(1.0)
+        return plan
+
+    try:
+        plan = _get_plan(agent, key, factory)
+    except Unsupported as e:
+        return _fallback(str(e))
+    except cabi.CdsError as e:
+        if e.code == -3:
+            return _fallback(str(e))
+        raise
+
+    t_all = _load_resident(agent, plan, xt, prior, table, sched_key, tape_slots, n_slots, x_shape, order, t_cpu, device)
+    lin1, fl = net.mid_layer[0], net.final_layer
+    a, e = x_shape[0], net.time_mlp[2].out_features
+    with torch.enable_grad():
+        # the per-call tables with autograd: Linear over cat[x, time_mlp(map_noise(t)), obs] = W_x x + (W_t temb + b) + W_o obs
+        step_tab = F.linear(net.time_mlp(net.map_noise(t_all)), lin1.weight[:, a:a + e], lin1.bias)
+        if cfg_mode == 1:
+            samp_tab = F.linear(_cond_rows(cfg_mode, cond_emb), lin1.weight[:, a + e:])
+        else:
+            samp_tab = torch.zeros((batch, lin1.out_features), device=device)
+        noise_rows = (table[:, S.R_NOISE] > 0).tolist()
+        run = lambda: plan.run_chunked(t_all, None, xt, noise_rows, use_graph=os.environ.get("CDS_GRAPH", "1") != "0")  # noqa: E731
+        x0 = _GradSampleFn.apply(plan, run, step_tab, samp_tab, lin1.weight[:, :a], net.mid_layer[2].weight,
+                                 net.mid_layer[2].bias, net.mid_layer[4].weight, net.mid_layer[4].bias, fl.weight, fl.bias)
+    STATS["engine_calls"] += 1
+    return x0
 
 
 def engine_forward(net, x, t, cond_emb=None, math=None, use_graph=False):

@@ -21,6 +21,8 @@
  *                       (diffusionsde.py:202,208-223,539-592) and the CM skip/out combine (consistency_model.py:257-262)
  *   CDS_OP_MHA          the attention core of nn.TransformerDecoderLayer's causal self-attention and masked cross-attention
  *                       (chitransformer.py: decoder with tgt_mask / memory_mask), q and k|v from separate strided sources
+ *   CDS_OP_STASH ..     the backward of sample(requires_grad=True) over DQLMlp (diffusionsde.py:525-594 under autograd): per-
+ *   CDS_OP_WGRAD        iteration stashes, the update's backward, Linear data / weight gradients (declared further down)
  *
  * Conventions
  *  - every function returns 0 on success, a negative cds_status otherwise; cds_last_error() gives the
@@ -47,7 +49,7 @@
 extern "C" {
 #endif
 
-#define CDS_ABI_VERSION 5
+#define CDS_ABI_VERSION 6
 
 typedef enum cds_status {
   CDS_OK = 0,
@@ -58,7 +60,9 @@ typedef enum cds_status {
 } cds_status;
 
 typedef enum cds_op_kind { CDS_OP_CONV = 0, CDS_OP_UPDATE = 1, CDS_OP_LNMOD = 2, CDS_OP_ATTN = 3, CDS_OP_PREP = 4,
-                           CDS_OP_CAST = 5, CDS_OP_MHA = 6 } cds_op_kind;
+                           CDS_OP_CAST = 5, CDS_OP_MHA = 6,
+                           /* differentiable sampling (sample(requires_grad=True) over DQLMlp, csrc/grad.cuh) */
+                           CDS_OP_STASH = 7, CDS_OP_UPDATE_BWD = 8, CDS_OP_DGRAD = 9, CDS_OP_WGRAD = 10 } cds_op_kind;
 typedef enum cds_act { CDS_ACT_NONE = 0, CDS_ACT_MISH = 1, CDS_ACT_SILU = 2, CDS_ACT_GELU_TANH = 3,
                        CDS_ACT_MISH_SILU = 4 /* silu(mish(x)): DiT's map_emb tail feeding every adaLN (dit.py:26,43,71) */,
                        CDS_ACT_LEAKY_RELU = 5 /* negative slope 0.01 (nn.LeakyReLU default; pearcemlp.py:44) */,
@@ -205,6 +209,67 @@ typedef struct cds_update_op {
   int32_t x_cast_dtype;          /* cds_dtype of x_cast */
 } cds_update_op;
 
+/* ---- backward operators of a differentiable reverse loop ------------------------------------------------------------
+ * A differentiable program keeps, per iteration n, what its backward reads in "stashes": [n_iters][...] buffers written at
+ * slot iter by the forward.  Every iteration-indexed operand below is `base + iter*iter_stride` (floats) with a SIGNED stride:
+ * the backward program walks the forward iterations in reverse by pointing at the last slot with a negative stride, so that
+ * one captured graph serves every backward iteration like it does every forward one. */
+
+/* dst[iter*dst_iter_stride + i] = src[i];  act_out[i] = act(src[i]) when act_out != NULL (i < n).  act: CDS_ACT_NONE / MISH */
+typedef struct cds_stash_op {
+  int64_t n;
+  int32_t act;
+  const float* src;
+  float* dst; int64_t dst_iter_stride;
+  float* act_out;
+} cds_stash_op;
+
+/* Backward of CDS_OP_UPDATE for kinds DDPM, DDIM, EPS and X with a single prediction (no CFG combine, no history):
+ *   in:  gx = d x_{n+1} (batch, row); the forward's operands x_n and the raw prediction from their stashes
+ *   out: gpred = d pred;  gx <- the direct part of d x_n (through the update and clip_prediction's x_t-dependent bounds;
+ *        the part through the network is added by the operators that follow)
+ * fix_mask: d out = gx * (1 - mask).  clip_prediction follows torch.clip's tensor-bound gradient: an element equal to a bound
+ * is not clipped (its gradient goes to pred), a clipped element's gradient goes to the bound, and an eps-prediction bound
+ * (x - alpha*x_lim)/sigma passes it to x_t divided by sigma. */
+typedef struct cds_update_bwd_op {
+  int32_t batch, row;
+  float* gx; float* gpred;
+  const float* x; int64_t x_iter_stride;
+  const float* pred; int64_t pred_iter_stride;
+  const float* mask;                       /* `row` floats or NULL */
+  const float* x_min; const float* x_max;  /* `row` floats or NULL */
+  const float* coef; int64_t coef_iter_stride;   /* row of iteration iter: coef + iter*coef_iter_stride (CDS_ROW_FLOATS) */
+  int32_t predict_noise;
+} cds_update_bwd_op;
+
+/* Data gradient of a Linear layer:  out(r, k) [+]= (sum_n dz(r, n) W(n, k)) * act'(z(r, k))
+ * dz (rows, N) row stride ldz; W (N, K) row stride ldw (a PyTorch [out, in] weight or a column block of one);
+ * z = the stashed pre-activation of the layer's input (z + iter*z_iter_stride, dense (rows, K)), required when act = MISH;
+ * out (rows, K) row stride ldo, overwritten (accumulate = 0) or added to (1); out_sum (dense (rows, K), optional) += result.
+ * fp32 CUDA cores; deterministic (every output is one thread's fixed-order sum). */
+typedef struct cds_dgrad_op {
+  int32_t rows, N, K;
+  const float* dz; int32_t ldz;
+  const float* w; int32_t ldw;
+  const float* z; int64_t z_iter_stride;
+  int32_t act, accumulate;
+  float* out; int32_t ldo;
+  float* out_sum;
+} cds_dgrad_op;
+
+/* Weight gradient of a Linear layer:  dw(n, k) [+]= sum_r dz(r, n) act(h(r, k));  db(n) [+]= sum_r dz(r, n)
+ * dz (rows, N) row stride ldz; h = h + iter*h_iter_stride, (rows, K) row stride ldh, read through act (CDS_ACT_NONE or MISH:
+ * the layer input recomputed from its stashed pre-activation); dw (N, K) row stride lddw; db + iter*db_iter_stride or NULL.
+ * Deterministic: each output is summed over the rows in a fixed order by one thread, no atomics, so two runs are bitwise equal. */
+typedef struct cds_wgrad_op {
+  int32_t rows, N, K;
+  const float* dz; int32_t ldz;
+  const float* h; int64_t h_iter_stride; int32_t ldh; int32_t act;
+  float* dw; int32_t lddw;
+  float* db; int64_t db_iter_stride;
+  int32_t accumulate;
+} cds_wgrad_op;
+
 /* cds_op.flags */
 enum { CDS_OPF_ONCE = 1 /* run once per cds_plan_run, before its first iteration, instead of in every iteration */,
        CDS_OPF_BRANCH_SHIFT = 8, CDS_OPF_BRANCH_MASK = 0xff00
@@ -216,7 +281,7 @@ typedef struct cds_op {
   int32_t kind;                  /* cds_op_kind */
   int32_t flags;
   union { cds_conv_op conv; cds_update_op update; cds_lnmod_op lnmod; cds_attn_op attn; cds_prep_op prep; cds_cast_op cast;
-          cds_mha_op mha; } u;
+          cds_mha_op mha; cds_stash_op stash; cds_update_bwd_op update_bwd; cds_dgrad_op dgrad; cds_wgrad_op wgrad; } u;
 } cds_op;
 
 typedef struct cds_plan cds_plan;
