@@ -1,0 +1,91 @@
+"""Classifiers for classifier guidance: ``logp(x, noise, c)`` and its input gradient ``gradients(x, noise, c)``.
+
+Same surface as the reference's (cleandiffuser/classifier/base.py, rew_classifiers.py): ``model`` is trained, ``model_ema`` (an
+eval-mode copy updated by ``ema_update``) is what ``logp`` evaluates.  When a ``CumRewClassifier`` over ``HalfJannerUNet1d``
+guides ``sample()``, the engine evaluates the input gradient inside the replayed loop and ``gradients`` is not called.
+"""
+from copy import deepcopy
+from typing import Optional
+
+import torch
+
+
+class BaseClassifier:
+    def __init__(self, nn_classifier: torch.nn.Module, ema_rate: float = 0.995, grad_clip_norm: Optional[float] = None,
+                 optim_params: Optional[dict] = None, device: str = "cpu"):
+        if optim_params is None:
+            optim_params = {"lr": 2e-4, "weight_decay": 1e-4}
+        self.device = device
+        self.ema_rate, self.grad_clip_norm = ema_rate, grad_clip_norm
+        self.model = nn_classifier.to(device)
+        self.model_ema = deepcopy(self.model).eval()
+        self.optim = torch.optim.Adam(self.model.parameters(), **optim_params)
+
+    def eval(self):
+        self.model.eval()
+        self.model_ema.eval()
+
+    def train(self):
+        self.model.train()
+
+    def ema_update(self):
+        """model_ema <- rate * model_ema + (1 - rate) * model, written through ``.data``"""
+        with torch.no_grad():
+            for p, p_ema in zip(self.model.parameters(), self.model_ema.parameters()):
+                p_ema.data.mul_(self.ema_rate).add_(p.data, alpha=1. - self.ema_rate)
+
+    def loss(self, x: torch.Tensor, noise: torch.Tensor, y: torch.Tensor):
+        raise NotImplementedError
+
+    def update(self, x: torch.Tensor, noise: torch.Tensor, y: torch.Tensor, update_ema: bool = True):
+        loss = self.loss(x, noise, y)
+        self.optim.zero_grad()
+        loss.backward()
+        grad_norm = None
+        if isinstance(self.grad_clip_norm, float):
+            grad_norm = torch.nn.utils.clip_grad_norm_(self.model.parameters(), self.grad_clip_norm).item()
+        self.optim.step()
+        if update_ema:
+            self.ema_update()
+        return {"loss": loss.item(), "grad_norm": grad_norm}
+
+    def logp(self, x: torch.Tensor, noise: torch.Tensor, c: torch.Tensor):
+        """log p(c | x_t, noise) + const, (batch, 1)"""
+        raise NotImplementedError
+
+    def gradients(self, x: torch.Tensor, noise: torch.Tensor, c: torch.Tensor):
+        """(logp, d sum(logp) / d x), both detached"""
+        x.requires_grad_()
+        logp = self.logp(x, noise, c)
+        grad = torch.autograd.grad([logp.sum()], [x])[0]
+        x.detach()
+        return logp.detach(), grad.detach()
+
+    def save(self, path):
+        torch.save({"model": self.model.state_dict(), "model_ema": self.model_ema.state_dict()}, path)
+
+    def load(self, path):
+        ckpt = torch.load(path, map_location=self.device)
+        self.model.load_state_dict(ckpt["model"])
+        self.model_ema.load_state_dict(ckpt["model_ema"])
+
+
+class CumRewClassifier(BaseClassifier):
+    """Regresses the cumulative reward R of a trajectory: ``loss = mean((model(x, noise) - R)^2)``, ``logp = model_ema(x, noise)``."""
+
+    def __init__(self, nn_classifier: torch.nn.Module, device: str = "cpu", optim_params: Optional[dict] = None):
+        super().__init__(nn_classifier, 0.995, None, optim_params, device)
+
+    def loss(self, x, noise, R):
+        return ((self.model(x, noise, None) - R) ** 2).mean()
+
+    def update(self, x, noise, R):
+        self.optim.zero_grad()
+        loss = self.loss(x, noise, R)
+        loss.backward()
+        self.optim.step()
+        self.ema_update()
+        return {"loss": loss.item()}
+
+    def logp(self, x, noise, c=None):
+        return self.model_ema(x, noise)

@@ -14,6 +14,7 @@
 #include "conv_ps.cuh"
 #include "attention_tma.cuh"
 #include "elementwise.cuh"
+#include "classifier.cuh"
 #include "grad.cuh"
 #include "mha.cuh"
 
@@ -235,6 +236,29 @@ int validate(const cds_op& op, Step* out) {
       if (w.act != CDS_ACT_NONE && w.act != CDS_ACT_MISH) return fail(CDS_ERR_UNSUPPORTED, "wgrad: act %d", w.act);
       return CDS_OK;
     }
+    case CDS_OP_GN: {
+      const cds_gn_op& g = op.u.gn;
+      if (g.batch <= 0 || g.L <= 0 || g.C <= 0 || g.groups <= 0 || g.C % g.groups != 0 || !g.h || !g.gamma || !g.beta || !g.out)
+        return fail(CDS_ERR_INVALID, "gn: bad arguments");
+      if (g.act != CDS_ACT_NONE && g.act != CDS_ACT_MISH) return fail(CDS_ERR_UNSUPPORTED, "gn: act %d", g.act);
+      if (g.out_dtype != CDS_F32 && g.out_dtype != CDS_TF32) return fail(CDS_ERR_UNSUPPORTED, "gn: out dtype %d", g.out_dtype);
+      return CDS_OK;
+    }
+    case CDS_OP_GN_BWD: {
+      const cds_gn_bwd_op& g = op.u.gn_bwd;
+      if (g.batch <= 0 || g.L <= 0 || g.C <= 0 || g.groups <= 0 || g.C % g.groups != 0 || !g.h || !g.gamma || !g.beta ||
+          !g.dout || !g.dh)
+        return fail(CDS_ERR_INVALID, "gn_bwd: bad arguments");
+      if (g.act != CDS_ACT_NONE && g.act != CDS_ACT_MISH) return fail(CDS_ERR_UNSUPPORTED, "gn_bwd: act %d", g.act);
+      if (g.dh_dtype != CDS_F32 && g.dh_dtype != CDS_TF32) return fail(CDS_ERR_UNSUPPORTED, "gn_bwd: dh dtype %d", g.dh_dtype);
+      return CDS_OK;
+    }
+    case CDS_OP_GUIDE: {
+      const cds_guide_op& g = op.u.guide;
+      if (g.batch <= 0 || g.L <= 0 || g.C <= 0 || !g.pred || !g.g || !g.s || g.g_lstride < g.C)
+        return fail(CDS_ERR_INVALID, "guide: bad arguments");
+      return CDS_OK;
+    }
     default:
       return fail(CDS_ERR_INVALID, "unknown operator kind %d", op.kind);
   }
@@ -301,6 +325,20 @@ int launch(const Step& s, const int* iter_ptr, int sm_count, cudaStream_t st, in
       cds::wgrad_kernel<<<cds::wgrad_grid(s.op.u.wgrad), 256, 0, st>>>(s.op.u.wgrad, iter_ptr);
       CDS_CUDA(cudaGetLastError());
       return CDS_OK;
+    case CDS_OP_GN:
+      cds::gn_kernel<<<cds::gn_grid(s.op.u.gn.batch, s.op.u.gn.groups), 256, 0, st>>>(s.op.u.gn, iter_ptr);
+      CDS_CUDA(cudaGetLastError());
+      return CDS_OK;
+    case CDS_OP_GN_BWD:
+      cds::gn_bwd_kernel<<<cds::gn_grid(s.op.u.gn_bwd.batch, s.op.u.gn_bwd.groups), 256, 0, st>>>(s.op.u.gn_bwd);
+      CDS_CUDA(cudaGetLastError());
+      return CDS_OK;
+    case CDS_OP_GUIDE: {
+      const cds_guide_op& g = s.op.u.guide;
+      cds::guide_kernel<<<elementwise_grid((int64_t)g.batch * g.L * g.C, sm_count), 256, 0, st>>>(g, iter_ptr);
+      CDS_CUDA(cudaGetLastError());
+      return CDS_OK;
+    }
   }
   return fail(CDS_ERR_INVALID, "unknown operator kind");
 }
@@ -327,6 +365,9 @@ int preload_kernels() {
   CDS_CUDA(cudaFuncGetAttributes(&a, cds::update_bwd_kernel));
   CDS_CUDA(cudaFuncGetAttributes(&a, cds::dgrad_kernel));
   CDS_CUDA(cudaFuncGetAttributes(&a, cds::wgrad_kernel));
+  CDS_CUDA(cudaFuncGetAttributes(&a, cds::gn_kernel));
+  CDS_CUDA(cudaFuncGetAttributes(&a, cds::gn_bwd_kernel));
+  CDS_CUDA(cudaFuncGetAttributes(&a, cds::guide_kernel));
   CDS_CUDA(cudaFuncGetAttributes(&a, cds::set_iter_kernel));
   CDS_CUDA(cudaFuncGetAttributes(&a, cds::advance_iter_kernel));
   return CDS_OK;
@@ -354,6 +395,9 @@ static_assert(sizeof(cds_mha_op) <= sizeof(cds_conv_op), "cds_mha_op must not gr
 static_assert(sizeof(cds_stash_op) <= sizeof(cds_conv_op) && sizeof(cds_update_bwd_op) <= sizeof(cds_conv_op) &&
               sizeof(cds_dgrad_op) <= sizeof(cds_conv_op) && sizeof(cds_wgrad_op) <= sizeof(cds_conv_op),
               "backward operators must not grow the cds_op union");
+// ... nor do the classifier-guidance operators
+static_assert(sizeof(cds_gn_op) <= sizeof(cds_conv_op) && sizeof(cds_gn_bwd_op) <= sizeof(cds_conv_op) &&
+              sizeof(cds_guide_op) <= sizeof(cds_conv_op), "classifier-guidance operators must not grow the cds_op union");
 
 struct cds_plan {
   int device = 0;

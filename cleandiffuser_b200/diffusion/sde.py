@@ -102,7 +102,9 @@ class BaseDiffusionSDE(DiffusionModel):
 
     def update_classifier(self, x0, condition):
         xt, t, _ = self.add_noise(x0)
-        return self.classifier.update(xt, t, condition)
+        out = self.classifier.update(xt, t, condition)
+        self._weights_epoch += 1        # the EMA update writes through .data: no version counter moves
+        return out
 
     # ------------------------------------------------------------------ guidance
     def classifier_free_guidance(self, xt, t, model, condition=None, w: float = 1.0,
@@ -178,9 +180,10 @@ class BaseDiffusionSDE(DiffusionModel):
             from ..engine import runtime
             guide = None
             if self.classifier is not None and w_cg != 0.0:
-                # classifier guidance on the engine, step by step: the engine evaluates the denoiser, this callback adds the
-                # guidance term to the prediction in place (same tensor expression as classifier_guidance above), the engine
-                # applies the update.  The classifier's forward + input gradient stay PyTorch autograd.
+                # classifier guidance on the engine.  A CumRewClassifier over HalfJannerUNet1d is lowered into the replayed
+                # program (runtime.try_sample); any other classifier runs step by step: the engine evaluates the denoiser, this
+                # callback adds the guidance term to the prediction in place (same tensor expression as classifier_guidance
+                # above), the engine applies the update.
                 def guide(n, i, x_t, pred):
                     t = self._t_vector(n_samples, step_values[i])
                     with torch.enable_grad():
@@ -193,7 +196,8 @@ class BaseDiffusionSDE(DiffusionModel):
             out = runtime.try_sample(self, model=model, xt=xt, prior=prior, solver=solver,
                                      sample_steps=sample_steps, order=order, step_values=step_values,
                                      alphas=alphas, sigmas=sigmas, hs=hs, stds=stds,
-                                     cond_emb=condition_vec_cfg, w_cfg=w_cfg, n_samples=n_samples, guide=guide, sched_id=sched_id)
+                                     cond_emb=condition_vec_cfg, w_cfg=w_cfg, n_samples=n_samples, guide=guide, sched_id=sched_id,
+                                     classifier=self.classifier, w_cg=w_cg)
             if out is not None:
                 return out
 

@@ -10,11 +10,12 @@ import os
 
 _LIB_PATH = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "csrc", "libcds.so")
 
-ABI_VERSION = 6
+ABI_VERSION = 7
 OPF_BRANCH_SHIFT = 8   # cds_op.flags bits 8..15: branch index (independent chains run on parallel streams)
 OPF_ONCE = 1          # cds_op.flags: run once per plan run (before its first iteration), not in every iteration
 OP_CONV, OP_UPDATE, OP_LNMOD, OP_ATTN, OP_PREP, OP_CAST, OP_MHA = range(7)
 OP_STASH, OP_UPDATE_BWD, OP_DGRAD, OP_WGRAD = 7, 8, 9, 10      # backward operators of a differentiable loop (csrc/grad.cuh)
+OP_GN, OP_GN_BWD, OP_GUIDE = 11, 12, 13       # classifier guidance inside the loop (csrc/classifier.cuh)
 ACT_NONE, ACT_MISH, ACT_SILU, ACT_GELU_TANH, ACT_MISH_SILU, ACT_LEAKY_RELU, ACT_GELU_ERF = range(7)
 MATH_FP32, MATH_BF16_TC, MATH_TF32_TC = 0, 1, 2
 TC_MODES = (MATH_BF16_TC, MATH_TF32_TC)
@@ -115,10 +116,31 @@ class WgradOp(C.Structure):
                 ("dw", _f32p), ("lddw", C.c_int32), ("db", _f32p), ("db_iter_stride", C.c_int64), ("accumulate", C.c_int32)]
 
 
+class GnOp(C.Structure):
+    _fields_ = [("batch", C.c_int32), ("L", C.c_int32), ("C", C.c_int32), ("groups", C.c_int32), ("eps", C.c_float),
+                ("act", C.c_int32), ("h", _f32p), ("h_bstride", C.c_int64), ("h_lstride", C.c_int32),
+                ("gamma", _f32p), ("beta", _f32p), ("vec", Vec),
+                ("res", _f32p), ("res_bstride", C.c_int64), ("res_lstride", C.c_int32),
+                ("out", _f32p), ("out_bstride", C.c_int64), ("out_lstride", C.c_int32), ("out_dtype", C.c_int32)]
+
+
+class GnBwdOp(C.Structure):
+    _fields_ = [("batch", C.c_int32), ("L", C.c_int32), ("C", C.c_int32), ("groups", C.c_int32), ("eps", C.c_float),
+                ("act", C.c_int32), ("h", _f32p), ("h_bstride", C.c_int64), ("h_lstride", C.c_int32),
+                ("gamma", _f32p), ("beta", _f32p),
+                ("dout", _f32p), ("dout_bstride", C.c_int64), ("dout_lstride", C.c_int32),
+                ("dh", _f32p), ("dh_bstride", C.c_int64), ("dh_lstride", C.c_int32), ("dh_dtype", C.c_int32)]
+
+
+class GuideOp(C.Structure):
+    _fields_ = [("batch", C.c_int32), ("L", C.c_int32), ("C", C.c_int32), ("pred", _f32p),
+                ("g", _f32p), ("g_bstride", C.c_int64), ("g_lstride", C.c_int32), ("s", _f32p)]
+
+
 class _OpUnion(C.Union):
     _fields_ = [("conv", ConvOp), ("update", UpdateOp), ("lnmod", LnModOp), ("attn", AttnOp), ("prep", PrepOp),
                 ("cast", CastOp), ("mha", MhaOp), ("stash", StashOp), ("update_bwd", UpdateBwdOp), ("dgrad", DgradOp),
-                ("wgrad", WgradOp)]
+                ("wgrad", WgradOp), ("gn", GnOp), ("gn_bwd", GnBwdOp), ("guide", GuideOp)]
 
 
 class Op(C.Structure):

@@ -1035,3 +1035,200 @@ def lower_denoiser(p: Program, net: nn.Module, x: View, x_shape, has_cond: bool,
     if name == "IDQLMlp" and len(x_shape) == 1:
         return lower_idql(p, net, x, has_cond, in_batch_mod)
     raise Unsupported(f"backbone {name} with x_shape {tuple(x_shape)}")
+
+
+# =============================================================================== classifier guidance: HalfJannerUNet1d's input gradient
+def half_janner_guidable(clf, x_shape) -> Optional[str]:
+    """None when ``clf`` is a CumRewClassifier over a HalfJannerUNet1d whose input gradient ``lower_half_janner_grad`` can put
+    into the loop (recognised structurally, so that the reference's own instances qualify), else the reason it cannot."""
+    if type(clf).__name__ != "CumRewClassifier":
+        return f"classifier {type(clf).__name__} (CumRewClassifier only)"
+    net = getattr(clf, "model_ema", None)
+    if type(net).__name__ != "HalfJannerUNet1d":
+        return f"classifier network {type(net).__name__} (HalfJannerUNet1d only)"
+    if net.training:
+        return "classifier model_ema in train mode"
+    if len(x_shape) != 2 or x_shape[0] & (x_shape[0] - 1):
+        return "classifier horizon must be 2^n"
+    blocks = [b for s in net.downs for b in (s[0], s[1])] + [net.mid_block1[0], net.mid_block2[0]]
+    if not all(_is_groupnorm(b.conv1[1]) and _is_groupnorm(b.conv2[1]) for b in blocks):
+        return "classifier norm_type other than groupnorm"
+    if blocks[0].conv1[0].in_channels != x_shape[1]:
+        return "classifier in_dim does not match x"
+    L = max(x_shape[0] >> (len(net.downs) + 1), 1)
+    if net.final_block[0].in_features != L * blocks[-1].conv1[0].out_channels + net.map_emb[2].out_features:
+        return "classifier final_block does not match its feature map"
+    return None
+
+
+def _gn(p: Program, h: View, gn: nn.Module, out: View, vec: Optional[cabi.Vec] = None, res: Optional[View] = None):
+    """CDS_OP_GN: out = Mish(GroupNorm(h) gamma + beta) [+ vec] [+ res]"""
+    op = cabi.Op()
+    op.kind = cabi.OP_GN
+    g = op.u.gn
+    g.batch, g.L, g.C, g.groups, g.eps, g.act = p.rows, h.L, h.C, int(gn.num_groups), float(gn.eps), cabi.ACT_MISH
+    g.h, g.h_bstride, g.h_lstride = h.ptr, h.bstride, h.lstride
+    g.gamma, g.beta = p.packed(lambda: gn.weight).data_ptr(), p.packed(lambda: gn.bias).data_ptr()
+    if vec is not None:
+        g.vec = vec
+    if res is not None:
+        g.res, g.res_bstride, g.res_lstride = res.ptr, res.bstride, res.lstride
+    g.out, g.out_bstride, g.out_lstride, g.out_dtype = out.ptr, out.bstride, out.lstride, out.dtype
+    p.ops.append(op)
+    return out
+
+
+def _gn_bwd(p: Program, h: View, gn: nn.Module, dout: View, dh: View):
+    """CDS_OP_GN_BWD: dh = d h of Mish(GroupNorm(h) gamma + beta) given the output gradient dout"""
+    op = cabi.Op()
+    op.kind = cabi.OP_GN_BWD
+    g = op.u.gn_bwd
+    g.batch, g.L, g.C, g.groups, g.eps, g.act = p.rows, h.L, h.C, int(gn.num_groups), float(gn.eps), cabi.ACT_MISH
+    g.h, g.h_bstride, g.h_lstride = h.ptr, h.bstride, h.lstride
+    g.gamma, g.beta = p.packed(lambda: gn.weight).data_ptr(), p.packed(lambda: gn.bias).data_ptr()
+    g.dout, g.dout_bstride, g.dout_lstride = dout.ptr, dout.bstride, dout.lstride
+    g.dh, g.dh_bstride, g.dh_lstride, g.dh_dtype = dh.ptr, dh.bstride, dh.lstride, dh.dtype
+    p.ops.append(op)
+    return dh
+
+
+def _as_conv(make: Callable[[], torch.Tensor]) -> WSpec:
+    """WSpec of a weight given as a Conv1d weight [C_out, C_in, taps] (packed like ``w_conv``)"""
+    return WSpec(lambda: (lambda w: w.permute(2, 1, 0).reshape(-1, w.shape[0]))(make()), lambda: make().permute(2, 0, 1))
+
+
+def w_conv_dgrad(conv: nn.Conv1d, cin: Optional[int] = None) -> WSpec:
+    """Data gradient of a stride-1 Conv1d(k, padding k // 2) as a conv of the output gradient with the same padding:
+    W'[c_in][c_out][tap] = W[c_out][c_in][k - 1 - tap] (input channels zero-padded to ``cin``: their gradient is zero)."""
+    return _as_conv(lambda: _pad_cin(conv.weight, cin).permute(1, 0, 2).flip(2))
+
+
+def w_down_dgrad(conv: nn.Conv1d) -> WSpec:
+    """Data gradient of Downsample1d (k = 3, stride 2, padding 1, L_in = 2 L_out) as ``w_convT``'s two-phase 3-tap form:
+    dx[2m] = W1^T d[m]  (phase 0, tap 1),   dx[2m+1] = W2^T d[m] + W0^T d[m+1]  (phase 1, taps 1 and 2)."""
+    def make():                                              # [3][C_out of the conv = gradient input][2 * C_in]
+        w = conv.weight                                      # [Cout, Cin, 3]
+        cout, cin, _ = w.shape
+        q = torch.zeros(3, cout, 2 * cin, device=w.device, dtype=w.dtype)
+        q[1, :, :cin] = w[:, :, 1]
+        q[1, :, cin:] = w[:, :, 2]
+        q[2, :, cin:] = w[:, :, 0]
+        return q
+    return WSpec(lambda: make().reshape(-1, 2 * conv.weight.shape[1]), lambda: make().permute(0, 2, 1))
+
+
+def lower_half_janner_grad(p: Program, clf, x: View) -> View:
+    """Append the input gradient d sum(logp) / d x of ``clf.model_ema`` (a HalfJannerUNet1d; ``half_janner_guidable``) at x_t
+    to the iteration program -> the gradient as a (rows, horizon, x.C) fp32 view (x.C may include zero padding channels).
+
+    Forward, per ResidualBlock: conv1 -> h1;  m = CDS_OP_GN(h1) + time row;  conv2 -> h2;  [1x1 shortcut conv -> s];
+    out = CDS_OP_GN(h2) + shortcut.  The Downsample convs as in the denoiser.  z1 = W1 [flatten(x), emb] + b1 (the emb half and
+    b1 are a per-iteration table row; the columns of W1 permuted from the channel-major flatten(1) to the (l, c) order).
+    Backward: dz1 = (1 W2) Mish'(z1) and d flatten = dz1 W1 (CDS_OP_DGRAD), then per block in reverse CDS_OP_GN_BWD, conv2's
+    data gradient, CDS_OP_GN_BWD, conv1's data gradient with the shortcut's added in the same CDS_OP_CONV.  Final Linear2's
+    value is not needed for the gradient."""
+    net = clf.model_ema
+    R = p.rows
+    stages = [(s[0], s[1], s[2]) for s in net.downs] + [(net.mid_block1[0], None, net.mid_block1[1]),
+                                                         (net.mid_block2[0], None, net.mid_block2[1])]
+    blocks = [b for st in stages for b in st[:2] if b is not None]
+    widths = [b.emb_mlp[1].out_features for b in blocks]
+    offs = [sum(widths[:i]) for i in range(len(widths))]
+    lin1, lin2 = net.final_block[0], net.final_block[2]
+    f2 = lin1.out_features
+    table = p.buf(p.n_iters, sum(widths) + f2)
+
+    def fill(ctx):
+        emb = net.map_emb(net.map_noise(ctx.t_all))
+        fc = lin1.in_features - emb.shape[1]
+        table.copy_(torch.cat([b.emb_mlp(emb) for b in blocks] + [F.linear(emb, lin1.weight[:, fc:], lin1.bias)], dim=1))
+    fill.time_only = True
+    p.per_call.append(fill)
+    row_of = {id(b): _vec(step=table, col=o) for b, o in zip(blocks, offs)}
+
+    # ---- forward
+    tape = []                                    # ("block", blk, x, h1, h2, k) / ("down", conv, x) in forward order
+    h = x
+    for res1, res2, down in stages:
+        for blk in (res1, res2):
+            if blk is None:
+                continue
+            k = blk.conv1[0].kernel_size[0]
+            c1, c2, C = blk.conv1[0], blk.conv2[0], blk.conv1[0].out_channels
+            h1, m, h2, out = p.act(h.L, C), p.act(h.L, C), p.act(h.L, C), p.act(h.L, C)
+            p.conv(h, w_conv(c1, h.C), h1, taps=k, pad=k // 2, bias=_const_vec(p.packed(lambda c=c1: c.bias)))
+            _gn(p, h1, blk.conv1[1], m, vec=row_of[id(blk)])
+            p.conv(m, w_conv(c2), h2, taps=k, pad=k // 2, bias=_const_vec(p.packed(lambda c=c2: c.bias)))
+            if isinstance(blk.residual_conv, nn.Conv1d):
+                rc = blk.residual_conv
+                res = p.conv(h, w_rows(lambda r=rc, cin=h.C: _pad_cin(r.weight, cin)[:, :, 0]), p.act(h.L, C),
+                           bias=_const_vec(p.packed(lambda r=rc: r.bias)))
+            else:
+                res = h
+            _gn(p, h2, blk.conv2[1], out, res=res)
+            tape.append(("block", blk, h, h1, h2, k))
+            h = out
+        if not isinstance(down, nn.Identity):
+            out = p.act((h.L + 1) // 2, h.C)
+            p.conv(h, w_conv(down.conv), out, taps=3, stride=2, pad=1, bias=_const_vec(p.packed(lambda d=down: d.conv.bias)))
+            tape.append(("down", down.conv, h))
+            h = out
+    fc = h.L * h.C
+    z1 = View(p.buf(R, 1, f2), 1, f2)
+    w1 = lambda: lin1.weight[:, :fc].reshape(f2, h.C, h.L).permute(0, 2, 1).reshape(f2, fc)     # noqa: E731
+    p.conv(View(h.t, 1, fc, h.offset, h.bstride, fc, h.tf32), w_rows(w1), z1, bias=_vec(step=table, col=sum(widths)))
+
+    # ---- backward
+    ones = p.buf(R, lin2.out_features)
+    ones.fill_(1.0)
+    dz1, dflat = p.buf(R, f2), p.buf(R, h.L, h.C)
+    for dz, w, n, k, z, out in ((ones, p.packed(lambda: lin2.weight), lin2.out_features, f2, z1, dz1),
+                                (dz1, p.packed(w1), f2, fc, None, dflat)):
+        op = cabi.Op()
+        op.kind = cabi.OP_DGRAD
+        d = op.u.dgrad
+        d.rows, d.N, d.K, d.dz, d.ldz, d.w, d.ldw = R, n, k, dz.data_ptr(), n, w.data_ptr(), k
+        if z is not None:
+            d.z, d.z_iter_stride, d.act = z.ptr, 0, cabi.ACT_MISH
+        d.out, d.ldo = out.data_ptr(), k
+        p.ops.append(op)
+    g = View(dflat, h.L, h.C)
+    for i in range(len(tape) - 1, -1, -1):
+        entry = tape[i]
+        if entry[0] == "down":
+            _, dconv, xin = entry
+            dx = p.act(xin.L, xin.C)
+            if xin.L == 1:                           # length 1 -> 1: only the centre tap sees the input
+                p.conv(g, w_rows(lambda c=dconv: c.weight[:, :, 1].t()), dx)
+            else:
+                p.conv(g, w_down_dgrad(dconv), dx, taps=3, stride=1, pad=1, phases=2, L_out=g.L)
+            g = dx
+            continue
+        _, blk, xin, h1, h2, k = entry
+        C = h1.C
+        d2, dm, d1 = p.act(h1.L, C), p.act(h1.L, C), p.act(h1.L, C)
+        _gn_bwd(p, h2, blk.conv2[1], g, d2)
+        p.conv(d2, w_conv_dgrad(blk.conv2[0]), dm, taps=k, pad=k // 2)
+        _gn_bwd(p, h1, blk.conv1[1], dm, d1)
+        first = i == 0
+        dx = p.act(xin.L, xin.C, torch.float32 if first else None)      # the input gradient itself stays exact fp32
+        if isinstance(blk.residual_conv, nn.Conv1d):
+            rc = blk.residual_conv
+            short = dict(res_conv=(g, w_rows(lambda r=rc, cin=xin.C: _pad_cin(r.weight, cin)[:, :, 0].t()),
+                                   lambda cin=xin.C: torch.zeros(cin)))
+        else:
+            short = dict(res=g)
+        p.conv(d1, w_conv_dgrad(blk.conv1[0], xin.C), dx, taps=k, pad=k // 2, **short)
+        g = dx
+    return g
+
+
+def guide(p: Program, pred: View, g: View, scale: torch.Tensor):
+    """CDS_OP_GUIDE: pred += scale[iter] * g  (pred dense fp32)"""
+    assert pred.lstride == pred.C and pred.bstride == pred.L * pred.C and pred.t.dtype == torch.float32
+    op = cabi.Op()
+    op.kind = cabi.OP_GUIDE
+    q = op.u.guide
+    q.batch, q.L, q.C, q.pred = p.rows, pred.L, pred.C, pred.ptr
+    q.g, q.g_bstride, q.g_lstride, q.s = g.ptr, g.bstride, g.lstride, scale.data_ptr()
+    p.ops.append(op)

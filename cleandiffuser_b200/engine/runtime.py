@@ -29,10 +29,15 @@ import torch
 import torch.nn.functional as F
 
 from . import cabi
-from .lower import DQLGrad, Program, Unsupported, View, _rev, lower_denoiser
+from .lower import (DQLGrad, Program, Unsupported, View, _rev, guide as emit_guide, half_janner_guidable, lower_denoiser,
+                    lower_half_janner_grad)
 from ..diffusion import solvers as S
 
-STATS = {"engine_calls": 0, "fallbacks": 0, "last_fallback_reason": None, "launches": 0}
+# guidance_path: how the latest engine call with classifier guidance was served -- "graph" (the classifier's input gradient is
+# part of the replayed program) or "callback" (step by step, PyTorch autograd between the denoiser and the update); None when
+# the latest call had no guidance.  guidance_reason: why a guided call took the callback path.
+STATS = {"engine_calls": 0, "fallbacks": 0, "last_fallback_reason": None, "launches": 0, "guidance_path": None,
+         "guidance_reason": None}
 
 
 def _backend():
@@ -127,11 +132,14 @@ class SamplerPlan:
     """Everything resident on the device for one (model, batch, x_shape, option set)."""
 
     def __init__(self, device, net, batch, x_shape, n_iters, n_slots, *, cfg_mode, predict_noise, has_mask,
-                 has_min, has_max, keep_history, math, consistency=False, aux_history=False):
-        """consistency: the EDM-preconditioned family (ContinuousConsistencyModel, ContinuousEDM): a CDS_OP_PREP in front of the
+                 has_min, has_max, keep_history, math, consistency=False, aux_history=False, classifier=None):
+        """classifier: a CumRewClassifier over HalfJannerUNet1d (``half_janner_guidable``) whose input gradient at x_t enters the
+        prediction between the denoiser and the update of every iteration (``pred += cg_scale[iter] * grad``).
+        consistency: the EDM-preconditioned family (ContinuousConsistencyModel, ContinuousEDM): a CDS_OP_PREP in front of the
         denoiser (re-noise + c_in scaling) and the c_skip / c_out combine in the update; aux_history: second history buffer (the
         EDM Heun corrector needs the predictor's x_t and slope)."""
         self.device, self.net, self.batch, self.x_shape = device, net, batch, tuple(x_shape)
+        self.classifier = classifier
         row = 1
         for s in x_shape:
             row *= s
@@ -177,6 +185,11 @@ class SamplerPlan:
             pred = lower_denoiser(p, net, xview, x_shape, cfg_mode != 0, sub if cfg_mode == 2 else 0)
             if K == 1:                 # the prediction buffer, for host callbacks between denoiser and update (guidance)
                 self.pred = pred.t if (pred.offset == 0 and pred.lstride == pred.C and pred.bstride == pred.L * pred.C) else None
+            if classifier is not None:
+                assert K == 1 and cfg_mode != 2
+                grad = lower_half_janner_grad(p, classifier, _input_view(p, n_before, xview))
+                self.cg_scale = root.buf(n_iters)           # per-iteration guidance scale, filled by every guided call
+                emit_guide(p, pred, grad, self.cg_scale)
 
             op = cabi.Op()
             op.kind = cabi.OP_UPDATE
@@ -224,6 +237,8 @@ class SamplerPlan:
 
     def refresh_weights(self, epoch: int = 0):
         v = _weights_version(self.net, epoch)
+        if self.classifier is not None:
+            v = _weights_version(self.classifier.model_ema, v)
         if self.version is None:         # packed at construction
             self.version = v
         elif v != self.version:
@@ -303,6 +318,17 @@ class SamplerPlan:
             STATS.setdefault("loop_events", []).append((e0, e1))
 
 
+def _input_view(p: Program, n_before: int, x: View) -> View:
+    """x_t as the denoiser's operators read it: the channel-padded copy of a CDS_OP_CAST appended since ``n_before`` when there
+    is one (tensor-core programs), else ``x``"""
+    for op in p.ops[n_before:]:
+        k = op.u.cast
+        if op.kind == cabi.OP_CAST and k.in_ == x.ptr:
+            t = next(t for t in p.keep if t.data_ptr() == k.out)
+            return View(t, k.L, k.C_out, tf32=k.out_dtype == cabi.TF32)
+    return x
+
+
 def _row(t, x_shape, device):
     return torch.broadcast_to(t.to(device=device, dtype=torch.float32), (1, *x_shape)).reshape(-1)
 
@@ -349,14 +375,18 @@ def _cond_rows(cfg_mode, cond_emb):
 
 
 def try_sample(agent, *, model, xt, prior, solver, sample_steps, order, step_values, alphas, sigmas, hs, stds,
-               cond_emb, w_cfg, n_samples, guide=None, table=None, clip_in_loop=True, predict_noise=None, sched_id=None):
+               cond_emb, w_cfg, n_samples, guide=None, table=None, clip_in_loop=True, predict_noise=None, sched_id=None,
+               classifier=None, w_cg=0.0):
     """``table``: optional ready-made ``(coefficient rows [n_iters, ROW], number of noise slots, int64/float32 time per iteration)``
     for samplers that are "the same update kernel with another coefficient table" (the legacy DDPM class, RectifiedFlow's Euler
     step): ``solver`` / ``alphas`` / ``sigmas`` / ``hs`` / ``stds`` / ``step_values`` are then unused.
     ``clip_in_loop=False``: the sampler clips only its final sample (RectifiedFlow); ``predict_noise``: overrides
     ``agent.predict_noise`` (classes without that attribute).
     ``guide``: optional host callback ``guide(n, i, x_t, pred)`` (n = iteration, i = its loop index) run between the denoiser
-    and the update of every iteration (classifier guidance); the loop then runs step by step instead of as a replayed graph."""
+    and the update of every iteration (classifier guidance); the loop then runs step by step instead of as a replayed graph --
+    unless ``classifier`` (the one ``guide`` evaluates, with weight ``w_cg``) is a CumRewClassifier over HalfJannerUNet1d under
+    CDS_MATH = fp32 | tf32 with one sub-batch chain: its input gradient and the guidance term are then operators of the replayed
+    program, and ``guide`` is not called."""
     if _backend() == "torch":
         return None
     device = _device_of(agent)
@@ -384,16 +414,25 @@ def try_sample(agent, *, model, xt, prior, solver, sample_steps, order, step_val
     row_elems = 1
     for s_ in x_shape:
         row_elems *= s_
+    cg_reason = None                       # why a guided call keeps the host callback (None: the graph serves it)
+    if guide is not None:
+        cg_reason = "no classifier" if classifier is None else half_janner_guidable(classifier, x_shape)
+        if cg_reason is None and math == cabi.MATH_BF16_TC:
+            cg_reason = "CDS_MATH=bf16"
+        if cg_reason is None and _n_branches(batch, row_elems, False) != 1:
+            cg_reason = "more than one sub-batch chain (CDS_BRANCHES)"
+    lowered_cg = guide is not None and cg_reason is None
     # noise tape: all draws of the loop up front when they fit the budget, else as many slots as fit (the loop then runs in
     # chunks with the tape refilled in between -- O(budget) memory instead of O(sample_steps x batch x row))
     tape_slots = min(n_slots, max(1, _tape_budget_bytes() // (4 * batch * row_elems))) if n_slots > 0 else 0
     key = ("sde", id(net), batch, x_shape, len(order), tape_slots, cfg_mode, pn, has_mask,
-           has_min, has_max, keep_history, math, float(w_cfg) if cfg_mode == 2 else 0.0)
+           has_min, has_max, keep_history, math, float(w_cfg) if cfg_mode == 2 else 0.0,
+           id(classifier.model_ema) if lowered_cg else None)
 
     def factory():
         plan = SamplerPlan(device, net, batch, x_shape, len(order), tape_slots, cfg_mode=cfg_mode,
                            predict_noise=pn, has_mask=has_mask, has_min=has_min, has_max=has_max,
-                           keep_history=keep_history, math=math)
+                           keep_history=keep_history, math=math, classifier=classifier if lowered_cg else None)
         plan.build(w_cfg)
         return plan
 
@@ -409,7 +448,17 @@ def try_sample(agent, *, model, xt, prior, solver, sample_steps, order, step_val
     t_all = _load_resident(agent, plan, xt, prior, table, sched_key, tape_slots, n_slots, x_shape, order, t_cpu, device)
     # the loop's draws: same calls, same order, same shapes as the reference loop's (diffusionsde.py:548,571,...)
     t_key = (t_cpu.numpy().tobytes(), tuple(order))
+    STATS["guidance_path"], STATS["guidance_reason"] = None, cg_reason
+    if lowered_cg:
+        # the guidance scale of every iteration, the reference's own expression (classifier_guidance), evaluated on the device
+        with torch.no_grad():
+            idx = torch.as_tensor(order, dtype=torch.long).to(device)
+            sig = sigmas.to(device)[idx]
+            plan.cg_scale.copy_(-(w_cg * sig) if pn else w_cg * ((sig ** 2) / alphas.to(device)[idx]))
+        STATS["guidance_path"] = "graph"
+        guide = None
     if guide is not None:
+        STATS["guidance_path"] = "callback"
         if plan.n_branches != 1 or getattr(plan, "pred", None) is None:
             return _fallback("guided sampling needs a single-branch program with a dense prediction buffer")
         slots = plan.coef[:, S.R_NOISE].cpu().tolist()              # tape slot per iteration as the update kernel sees it

@@ -1,0 +1,63 @@
+"""``nn_classifier`` plugin surface: networks ``(x, noise[, condition]) -> log p(y | x, t) + const`` of shape (batch, out_dim).
+
+``HalfJannerUNet1d`` is the down half of JannerUNet1d followed by a small MLP head, with the reference's constructor signature,
+parameter names and shapes (cleandiffuser/nn_classifier/half_jannerunet.py), so its checkpoints load.  Under classifier guidance
+(``CumRewClassifier``) the engine lowers its forward and input gradient into the replayed loop (``engine/lower.py``,
+``lower_half_janner_grad``); everything else about it runs in PyTorch.
+"""
+from typing import Optional, Tuple
+
+import numpy as np
+import torch
+import torch.nn as nn
+
+from ..nn_diffusion.base import BaseNNDiffusion
+from ..nn_diffusion.unets import Downsample1d, ResidualBlock
+
+
+class HalfJannerUNet1d(BaseNNDiffusion):
+    """x (b, horizon, in_dim), noise (b,), condition (b, model_dim... added to the time embedding) | None -> (b, out_dim).
+
+    Stages: two ResidualBlocks per resolution of ``dim_mult`` with a Downsample1d between resolutions, then two mid
+    ResidualBlocks (kernel 5) halving the channels, each followed by a Downsample1d, then
+    ``Linear(fc_dim + model_dim, fc_dim // 2) -> Mish -> Linear(fc_dim // 2, out_dim)`` over ``[flatten(x), emb]`` with the
+    features flattened channel-major, ``fc_dim = mid_dim // 4 * max(final length, 1)``."""
+
+    def __init__(self, horizon: int, in_dim: int, out_dim: int = 1, kernel_size: int = 3, model_dim: int = 32,
+                 emb_dim: int = 32, dim_mult: Tuple[int] = (1, 2, 2, 2), timestep_emb_type: str = "positional",
+                 norm_type: str = "groupnorm"):
+        super().__init__(emb_dim, timestep_emb_type)
+        dims = [in_dim] + [model_dim * m for m in np.cumprod(dim_mult)]
+        pairs = list(zip(dims[:-1], dims[1:]))
+        self.map_emb = nn.Sequential(nn.Linear(emb_dim, model_dim * 4), nn.Mish(), nn.Linear(model_dim * 4, model_dim))
+        self.downs = nn.ModuleList([])
+        self.ups = nn.ModuleList([])           # empty: kept so that the module tree reads like the reference's
+        length = horizon
+        for i, (cin, cout) in enumerate(pairs):
+            last = i == len(pairs) - 1
+            self.downs.append(nn.ModuleList([
+                ResidualBlock(cin, cout, model_dim, kernel_size, norm_type),
+                ResidualBlock(cout, cout, model_dim, kernel_size, norm_type),
+                nn.Identity() if last else Downsample1d(cout)]))
+            if not last:
+                length //= 2
+        mid = dims[-1]
+        self.mid_block1 = nn.ModuleList([ResidualBlock(mid, mid // 2, model_dim, kernel_size=5, norm_type=norm_type),
+                                         Downsample1d(mid // 2)])
+        self.mid_block2 = nn.ModuleList([ResidualBlock(mid // 2, mid // 4, model_dim, kernel_size=5, norm_type=norm_type),
+                                         Downsample1d(mid // 4)])
+        length = length // 4
+        fc_dim = mid // 4 * max(length, 1)
+        self.final_block = nn.Sequential(nn.Linear(fc_dim + model_dim, fc_dim // 2), nn.Mish(), nn.Linear(fc_dim // 2, out_dim))
+
+    def forward(self, x: torch.Tensor, noise: torch.Tensor, condition: Optional[torch.Tensor] = None):
+        h = x.permute(0, 2, 1)
+        emb = self.map_noise(noise)
+        if condition is not None:
+            emb = emb + condition
+        emb = self.map_emb(emb)
+        for res1, res2, down in self.downs:
+            h = down(res2(res1(h, emb), emb))
+        for block, down in (self.mid_block1, self.mid_block2):
+            h = down(block(h, emb))
+        return self.final_block(torch.cat([h.flatten(1), emb], dim=-1))

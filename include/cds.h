@@ -23,6 +23,8 @@
  *                       (chitransformer.py: decoder with tgt_mask / memory_mask), q and k|v from separate strided sources
  *   CDS_OP_STASH ..     the backward of sample(requires_grad=True) over DQLMlp (diffusionsde.py:525-594 under autograd): per-
  *   CDS_OP_WGRAD        iteration stashes, the update's backward, Linear data / weight gradients (declared further down)
+ *   CDS_OP_GN ..        classifier guidance inside the loop (diffusionsde.py:153-173 with CumRewClassifier over HalfJannerUNet1d):
+ *   CDS_OP_GUIDE        GroupNorm + Mish over a kept pre-norm input, its backward, and pred += s[iter] * grad (further down)
  *
  * Conventions
  *  - every function returns 0 on success, a negative cds_status otherwise; cds_last_error() gives the
@@ -49,7 +51,7 @@
 extern "C" {
 #endif
 
-#define CDS_ABI_VERSION 6
+#define CDS_ABI_VERSION 7
 
 typedef enum cds_status {
   CDS_OK = 0,
@@ -62,7 +64,9 @@ typedef enum cds_status {
 typedef enum cds_op_kind { CDS_OP_CONV = 0, CDS_OP_UPDATE = 1, CDS_OP_LNMOD = 2, CDS_OP_ATTN = 3, CDS_OP_PREP = 4,
                            CDS_OP_CAST = 5, CDS_OP_MHA = 6,
                            /* differentiable sampling (sample(requires_grad=True) over DQLMlp, csrc/grad.cuh) */
-                           CDS_OP_STASH = 7, CDS_OP_UPDATE_BWD = 8, CDS_OP_DGRAD = 9, CDS_OP_WGRAD = 10 } cds_op_kind;
+                           CDS_OP_STASH = 7, CDS_OP_UPDATE_BWD = 8, CDS_OP_DGRAD = 9, CDS_OP_WGRAD = 10,
+                           /* classifier guidance (the input gradient of HalfJannerUNet1d, csrc/classifier.cuh) */
+                           CDS_OP_GN = 11, CDS_OP_GN_BWD = 12, CDS_OP_GUIDE = 13 } cds_op_kind;
 typedef enum cds_act { CDS_ACT_NONE = 0, CDS_ACT_MISH = 1, CDS_ACT_SILU = 2, CDS_ACT_GELU_TANH = 3,
                        CDS_ACT_MISH_SILU = 4 /* silu(mish(x)): DiT's map_emb tail feeding every adaLN (dit.py:26,43,71) */,
                        CDS_ACT_LEAKY_RELU = 5 /* negative slope 0.01 (nn.LeakyReLU default; pearcemlp.py:44) */,
@@ -270,6 +274,46 @@ typedef struct cds_wgrad_op {
   int32_t accumulate;
 } cds_wgrad_op;
 
+/* ---- classifier guidance inside the loop ---------------------------------------------------------------------------------
+ * The classifier's forward runs its convolutions as plain CDS_OP_CONV (no GroupNorm in the epilogue) so that the pre-norm
+ * activation h survives for the backward; CDS_OP_GN normalises it.  The data gradients of the convolutions are CDS_OP_CONV with
+ * re-packed weights.  GroupNorm statistics: per (b, group) over L x C/groups elements, fp32, two passes (mean, then the mean of
+ * squared deviations), rstd = 1/sqrt(var + eps), every sum in one fixed order (no atomics): both operators compute the same
+ * mean and rstd bit for bit.  h, res and dout are fp32 storage (CDS_F32 or CDS_TF32, read alike); strides in floats. */
+
+/* out(b,l,c) = act(xhat(b,l,c) * gamma[c] + beta[c]) [+ vec(b, c)] [+ res(b,l,c)],  xhat = (h - mean) * rstd.
+ * act: CDS_ACT_NONE / MISH.  out_dtype: CDS_F32 or CDS_TF32 (rounded on store). */
+typedef struct cds_gn_op {
+  int32_t batch, L, C, groups; float eps; int32_t act;
+  const float* h; int64_t h_bstride; int32_t h_lstride;
+  const float* gamma; const float* beta;
+  cds_vec vec;
+  const float* res; int64_t res_bstride; int32_t res_lstride;
+  float* out; int64_t out_bstride; int32_t out_lstride; int32_t out_dtype;
+} cds_gn_op;
+
+/* Backward of CDS_OP_GN with respect to h (the vec and res terms do not depend on h):
+ *   dxhat = gamma * dout * act'(y),  y = xhat * gamma + beta
+ *   dh    = rstd * (dxhat - mean_g(dxhat) - xhat * mean_g(dxhat * xhat))
+ * dh_dtype: CDS_F32 or CDS_TF32. */
+typedef struct cds_gn_bwd_op {
+  int32_t batch, L, C, groups; float eps; int32_t act;
+  const float* h; int64_t h_bstride; int32_t h_lstride;
+  const float* gamma; const float* beta;
+  const float* dout; int64_t dout_bstride; int32_t dout_lstride;
+  float* dh; int64_t dh_bstride; int32_t dh_lstride; int32_t dh_dtype;
+} cds_gn_bwd_op;
+
+/* pred(b, l, c) = pred(b, l, c) + s[iter] * g(b, l, c), IEEE fp32 multiply then add (no FMA contraction): with
+ * s = -(w * sigma) this is bit for bit the reference's pred - (w * sigma) * grad.  pred dense (batch, L, C); g strided (an input
+ * gradient may carry padding channels). */
+typedef struct cds_guide_op {
+  int32_t batch, L, C;
+  float* pred;
+  const float* g; int64_t g_bstride; int32_t g_lstride;
+  const float* s;
+} cds_guide_op;
+
 /* cds_op.flags */
 enum { CDS_OPF_ONCE = 1 /* run once per cds_plan_run, before its first iteration, instead of in every iteration */,
        CDS_OPF_BRANCH_SHIFT = 8, CDS_OPF_BRANCH_MASK = 0xff00
@@ -281,7 +325,8 @@ typedef struct cds_op {
   int32_t kind;                  /* cds_op_kind */
   int32_t flags;
   union { cds_conv_op conv; cds_update_op update; cds_lnmod_op lnmod; cds_attn_op attn; cds_prep_op prep; cds_cast_op cast;
-          cds_mha_op mha; cds_stash_op stash; cds_update_bwd_op update_bwd; cds_dgrad_op dgrad; cds_wgrad_op wgrad; } u;
+          cds_mha_op mha; cds_stash_op stash; cds_update_bwd_op update_bwd; cds_dgrad_op dgrad; cds_wgrad_op wgrad;
+          cds_gn_op gn; cds_gn_bwd_op gn_bwd; cds_guide_op guide; } u;
 } cds_op;
 
 typedef struct cds_plan cds_plan;
