@@ -18,6 +18,7 @@ import torch
 import torch.nn as nn
 
 from .basic import DiffusionModel
+from . import solvers as S
 from ..utils import at_least_ndim
 
 
@@ -240,10 +241,13 @@ class ContinuousConsistencyModel(DiffusionModel):
         if requires_grad:
             runtime.grad_fallback(self)
         if not (requires_grad or preserve_history) and runtime._device_ok(torch.device(self.device)):
-            out = runtime.try_sample_consistency(self, model=model, xt=xt, prior=prior, sigmas=sigmas, order=order,
-                                                 cond_emb=cvec, n_samples=n_samples,
-                                                 sched_id=(int(sample_steps), float(self.sigma_min), float(self.sigma_max), float(self.rho),
-                                                           int(diffusion_x_sampling_steps), float(self.sigma_data)))
+            out = runtime.try_sample(self, model=model, xt=xt, prior=prior, solver="consistency", sample_steps=sample_steps,
+                                     order=order, step_values=None, alphas=None, sigmas=None, hs=None, stds=None, cond_emb=cvec,
+                                     w_cfg=1.0 if cvec is not None else 0.0, n_samples=n_samples, predict_noise=False,
+                                     consistency=True,
+                                     table=lambda: S.consistency_table(sigmas, order, self.sigma_data, self.sigma_min),
+                                     sched_id=(int(sample_steps), float(self.sigma_min), float(self.sigma_max), float(self.rho),
+                                               int(diffusion_x_sampling_steps), float(self.sigma_data)))
             if out is not None:
                 return out, log
 

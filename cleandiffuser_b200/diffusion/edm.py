@@ -16,6 +16,7 @@ import torch
 import torch.nn as nn
 
 from .basic import DiffusionModel
+from . import solvers as S
 from ..utils import at_least_ndim
 
 
@@ -161,10 +162,24 @@ class ContinuousEDM(DiffusionModel):
         if requires_grad:
             runtime.grad_fallback(self)
         if not (requires_grad or preserve_history or guided) and runtime._device_ok(torch.device(self.device)):
-            out = runtime.try_sample_edm(self, model=model, xt=xt, prior=prior, solver=solver, sigmas=sigmas, order=order,
-                                         cond_emb=cvec, w_cfg=w_cfg, n_samples=n_samples,
-                                         sched_id=(int(sample_steps), float(self.sigma_min), float(top), float(self.rho),
-                                                   float(self.sigma_data)))
+            def table():
+                # every network evaluation is one engine iteration: ``euler`` one per reverse step, ``heun`` a predictor and a
+                # corrector for every step but the last
+                sig = sigmas.detach().float().cpu()
+                evals = []                      # (sigma of the evaluation, kind, dt, predictor flag)
+                for i in order:
+                    dt = sig[i] - sig[i - 1]
+                    heun = solver == "heun" and i > 1
+                    evals.append((sig[i], S.UPD_EDM, dt, 1.0 if heun else 0.0))
+                    if heun:
+                        # the corrector evaluates at t = t_i / sigma_i * sigma_{i-1} (newedm.py:421) = sigma_{i-1} exactly (x / x == 1)
+                        evals.append((sig[i - 1], S.UPD_EDM_HEUN, dt, 0.0))
+                return S.edm_table(evals, self.sigma_data)
+            out = runtime.try_sample(self, model=model, xt=xt, prior=prior, solver=solver, sample_steps=sample_steps, order=order,
+                                     step_values=None, alphas=None, sigmas=None, hs=None, stds=None, cond_emb=cvec, w_cfg=w_cfg,
+                                     n_samples=n_samples, predict_noise=False, consistency=True, aux_history=solver == "heun",
+                                     table=table, sched_id=(int(sample_steps), float(self.sigma_min), float(top), float(self.rho),
+                                                            float(self.sigma_data)))
             if out is not None:
                 xt, done = out, True
 

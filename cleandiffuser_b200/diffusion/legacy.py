@@ -361,9 +361,11 @@ class EDM(DiffusionModel):
                 evals.append((sig[i], S.UPD_EDM, dt, 1.0 if heun else 0.0, xw[i], dw[i]))
                 if heun:
                     evals.append((sig[i + 1], S.UPD_EDM_HEUN, dt, 0.0, xw[i + 1], dw[i + 1]))
-            out = runtime.try_sample_edm(self, model=model, xt=xt, prior=prior.to(self.device),
-                                         solver="heun" if any(heun_at) else "euler", sigmas=None, order=None, cond_emb=cvec,
-                                         w_cfg=w_cfg, n_samples=n_samples, evals=evals, clip=False)
+            out = runtime.try_sample(self, model=model, xt=xt, prior=prior.to(self.device),
+                                     solver="heun" if any(heun_at) else "euler", sample_steps=N, order=list(range(len(evals))),
+                                     step_values=None, alphas=None, sigmas=None, hs=None, stds=None, cond_emb=cvec, w_cfg=w_cfg,
+                                     n_samples=n_samples, table=S.edm_table(evals, self.sigma_data), clip_in_loop=False,
+                                     predict_noise=False, consistency=True, aux_history=any(heun_at))
             if out is not None:
                 return out, {"log_p": None, "sample_history": None}
 

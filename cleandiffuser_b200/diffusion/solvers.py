@@ -164,3 +164,44 @@ def coeff_table(solver: str, order: List[int], n_steps: int, alphas, sigmas, hs,
         rows[n, R_NOISE] = 1.0 if c.noise else 0.0
         rows[n, R_T] = float(t_values[i])
     return rows
+
+
+def consistency_table(sigmas, order: List[int], sigma_data, sigma_min):
+    """ContinuousConsistencyModel.sample as engine rows -> ``(rows, n_slots, c_noise per iteration)``: iteration 0 evaluates f at
+    sigma_max, iteration n > 0 re-noises to sigma_{order[n-1]} with the draw in noise slot n and evaluates f again
+    (consistency_model.py:401-426).  The network sees c_noise = ln(sigma)/4 as its "time"."""
+    sig = sigmas.detach().float().cpu()
+    levels = [sig[-1]] + [sig[i] for i in order]
+    sd, smin = sigma_data, sigma_min
+    table = torch.zeros((len(levels), ROW), dtype=torch.float32)
+    for n, s in enumerate(levels):                     # 0-d fp32 tensors, reference op order (:241-251, :423)
+        table[n, R_K0] = float(sd ** 2 / (sd ** 2 + (s - smin) ** 2))                      # c_skip
+        table[n, R_K1] = float((s - smin) * sd / (sd ** 2 + s ** 2).sqrt())               # c_out
+        table[n, R_K3] = float(1 / (sd ** 2 + s ** 2).sqrt())                              # c_in
+        table[n, R_KIND] = float(UPD_CM)
+        if n > 0:
+            table[n, R_K2] = float((s ** 2 - smin ** 2).sqrt())                            # re-noise scale
+            table[n, R_NOISE] = float(n)
+        table[n, R_T] = float(0.25 * s.log())                                               # c_noise
+    return table, len(levels) - 1, table[:, R_T]
+
+
+def edm_table(evals, sigma_data):
+    """EDM network evaluations as engine rows -> ``(rows, 0 noise slots, c_noise per evaluation)``.  ``evals``: one
+    ``(sigma of the evaluation, kind, dt, predictor flag[, x_weight, D_weight])`` per evaluation (UPD_EDM, or UPD_EDM_HEUN for a
+    Heun corrector), 0-d fp32 tensors."""
+    sd = sigma_data
+    table = torch.zeros((len(evals), ROW), dtype=torch.float32)
+    for n, ev in enumerate(evals):                         # 0-d fp32 tensors, reference op order (newedm.py:128-148)
+        s, kind, dt, pred_flag = ev[:4]
+        if len(ev) > 4:
+            table[n, R_XW], table[n, R_DW] = float(ev[4]), float(ev[5])
+        table[n, R_K0] = float(sd ** 2 / (sd ** 2 + s ** 2))                  # c_skip
+        table[n, R_K1] = float(s * sd / (sd ** 2 + s ** 2).sqrt())            # c_out
+        table[n, R_K3] = float(1 / (sd ** 2 + s ** 2).sqrt())                 # c_in
+        table[n, R_K2] = float(dt)
+        table[n, R_K4] = pred_flag
+        table[n, R_SIGMA] = float(s)                                          # the slope divides by it
+        table[n, R_KIND] = float(kind)
+        table[n, R_T] = float(0.25 * s.log())                                 # c_noise
+    return table, 0, table[:, R_T]

@@ -1,9 +1,10 @@
-"""Host runtime of the CUDA sampling engine: plan cache, per-call table fill, graph replay.
+"""Host runtime of the CUDA sampling engine: plan cache, schedule-table cache, per-call table fill, graph replay.
 
-``try_sample`` is called by ``{Discrete,Continuous}DiffusionSDE.sample`` after the prologue (initial
+``try_sample`` is called by the ``sample()`` of every sampler family (``{Discrete,Continuous}DiffusionSDE``,
+``ContinuousConsistencyModel``, ``ContinuousEDM``, RectifiedFlow, the legacy DDPM and EDM classes) after the prologue (initial
 noise, mask, nn_condition) and replaces the whole Python reverse loop (diffusionsde.py:525-594) by
 
-    tables  <- per-iteration solver coefficients + time-conditioning rows      (host, tiny)
+    tables  <- per-iteration solver coefficients (cached per schedule) + time-conditioning rows      (host, tiny)
     noise   <- the loop's torch.randn_like draws, taken up front IN THE SAME ORDER (so a seeded run consumes
                the generator exactly like the reference loop would)
     x_t     <- one device buffer, updated in place by the last operator of every iteration
@@ -21,6 +22,7 @@ Environment switches (no flag system, pipelines stay unchanged):
   CDS_NOISE_TAPE_MB                    (cap of the pre-drawn noise tape, default 4096: longer loops are run in chunks)
   CDS_MAX_PLANS                        (plans kept per agent, default 8, least recently used evicted)
 """
+import collections
 import os
 import types
 from typing import Optional
@@ -80,10 +82,6 @@ def _device_ok(device: torch.device) -> bool:
     return cap == (9, 0) and os.path.exists(cabi.lib_path())
 
 
-def _tape_budget_bytes():
-    return int(float(os.environ.get("CDS_NOISE_TAPE_MB", "4096")) * (1 << 20))
-
-
 def _randn_is_patched():
     """True when a harness replaced torch.randn_like (tests replay recorded draws through it)."""
     return not isinstance(torch.randn_like, types.BuiltinFunctionType)
@@ -138,33 +136,17 @@ class SamplerPlan:
         consistency: the EDM-preconditioned family (ContinuousConsistencyModel, ContinuousEDM): a CDS_OP_PREP in front of the
         denoiser (re-noise + c_in scaling) and the c_skip / c_out combine in the update; aux_history: second history buffer (the
         EDM Heun corrector needs the predictor's x_t and slope)."""
-        self.device, self.net, self.batch, self.x_shape = device, net, batch, tuple(x_shape)
+        self._resident(device, net, batch, x_shape, n_iters, n_slots, cfg_mode=cfg_mode, has_mask=has_mask, has_min=has_min,
+                       has_max=has_max, keep_history=keep_history, aux_history=aux_history, math=math)
         self.classifier = classifier
-        row = 1
-        for s in x_shape:
-            row *= s
-        self.row, self.n_iters = row, n_iters
-        self.cfg_mode = cfg_mode
+        row, root = self.row, self.program
         K = _n_branches(batch, row, consistency)
         self.n_branches = K
-        root = Program(device, batch * (2 if cfg_mode == 2 else 1), n_iters, math)     # owns the shared buffers
-        self.program = root
-        self.x = root.buf(batch, *x_shape)
-        self.prior = root.buf(batch, *x_shape) if has_mask else None
-        self.mask = root.buf(row) if has_mask else None
-        self.x_min = root.buf(row) if has_min else None
-        self.x_max = root.buf(row) if has_max else None
-        self.coef = root.buf(n_iters, cabi.ROW_FLOATS)
-        self.noise = root.buf(max(n_slots, 1), batch, row) if n_slots > 0 else None
-        self.xhat_prev = root.buf(batch, row) if keep_history else None
-        self.aux = root.buf(batch, row) if (keep_history and aux_history) else None
         if consistency:
             self.xin = root.buf(batch, *x_shape)
 
         L = x_shape[0] if len(x_shape) == 2 else 1
         Cn = x_shape[-1]
-        self._update_ops = []
-        self._fillers = []                 # (per-call table filler, sub-batch slice)
         sub = batch // K
         for k in range(K):
             off = k * sub                  # first trajectory of this branch
@@ -191,24 +173,7 @@ class SamplerPlan:
                 self.cg_scale = root.buf(n_iters)           # per-iteration guidance scale, filled by every guided call
                 emit_guide(p, pred, grad, self.cg_scale)
 
-            op = cabi.Op()
-            op.kind = cabi.OP_UPDATE
-            u = op.u.update
-            u.batch, u.row, u.x = sub, row, self.x.data_ptr() + fo
-            u.pred = pred.ptr
-            if cfg_mode == 2:
-                u.pred_uncond = pred.ptr + 4 * sub * row
-            if self.noise is not None:
-                u.noise, u.noise_slot_stride = self.noise.data_ptr() + fo, batch * row
-            u.prior = self.prior.data_ptr() + fo if has_mask else None
-            u.mask = self.mask.data_ptr() if has_mask else None
-            u.x_min = self.x_min.data_ptr() if has_min else None
-            u.x_max = self.x_max.data_ptr() if has_max else None
-            u.xhat_prev = self.xhat_prev.data_ptr() + fo if keep_history else None
-            u.aux = self.aux.data_ptr() + fo if self.aux is not None else None
-            u.coef = self.coef.data_ptr()
-            u.predict_noise = 1 if predict_noise else 0
-            u.final_clip = 1 if consistency else 0
+            u = self._update_op(p, pred.ptr, sub, fo, predict_noise, consistency)
             # tensor-core UNets read x_t through a channel-padded bf16 copy (CDS_OP_CAST).  When that cast converts the very
             # buffer the update writes, the update emits the copy itself and the cast runs only once per sample() call.
             for cop in p.ops[n_before:]:
@@ -216,8 +181,6 @@ class SamplerPlan:
                     cop.flags |= cabi.OPF_ONCE
                     u.x_cast, u.cast_C_in, u.cast_C_out = cop.u.cast.out, cop.u.cast.C_in, cop.u.cast.C_out
                     u.x_cast_dtype = cop.u.cast.out_dtype
-            self._update_ops.append(op)
-            p.ops.append(op)
             self._fillers += [(fn, sl) for fn in p.per_call]
             if p is not root:
                 for o in p.ops:
@@ -226,14 +189,65 @@ class SamplerPlan:
                 root.keep += p.keep + [p]
                 root.packers += p.packers
 
+    def _resident(self, device, net, batch, x_shape, n_iters, n_slots, *, cfg_mode, has_mask, has_min, has_max, keep_history,
+                  aux_history, math):
+        """The buffers every program of the plan shares (x_t, prior and mask, clip bounds, coefficient rows, noise tape, solver
+        history), owned by the root program."""
+        self.device, self.net, self.batch, self.x_shape = device, net, batch, tuple(x_shape)
+        row = 1
+        for s in x_shape:
+            row *= s
+        self.row, self.n_iters, self.cfg_mode = row, n_iters, cfg_mode
+        root = Program(device, batch * (2 if cfg_mode == 2 else 1), n_iters, math)
+        self.program, self.back = root, None             # back: the backward program of a differentiable plan
+        self.classifier = None
+        self.x = root.buf(batch, *x_shape)
+        self.prior = root.buf(batch, *x_shape) if has_mask else None
+        self.mask = root.buf(row) if has_mask else None
+        self.x_min = root.buf(row) if has_min else None
+        self.x_max = root.buf(row) if has_max else None
+        self.coef = root.buf(n_iters, cabi.ROW_FLOATS)
+        self.noise = root.buf(max(n_slots, 1), batch, row) if n_slots > 0 else None
+        self.xhat_prev = root.buf(batch, row) if keep_history else None
+        self.aux = root.buf(batch, row) if (keep_history and aux_history) else None
+        self._update_ops = []
+        self._fillers = []                 # (per-call table filler, sub-batch slice)
         self.handle: Optional[cabi.Plan] = None
+        self.back_handle: Optional[cabi.Plan] = None
         self.version = None              # set by the first refresh_weights()
+
+    def _update_op(self, p, pred, sub, fo, predict_noise, consistency=False):
+        """Append the solver update of ``sub`` trajectories at byte offset ``fo`` of the resident buffers to ``p`` (``pred``:
+        address of their prediction, the unconditional half after it under two-branch CFG)."""
+        op = cabi.Op()
+        op.kind = cabi.OP_UPDATE
+        u = op.u.update
+        u.batch, u.row, u.x = sub, self.row, self.x.data_ptr() + fo
+        u.pred = pred
+        if self.cfg_mode == 2:
+            u.pred_uncond = pred + 4 * sub * self.row
+        if self.noise is not None:
+            u.noise, u.noise_slot_stride = self.noise.data_ptr() + fo, self.batch * self.row
+        u.prior = self.prior.data_ptr() + fo if self.prior is not None else None
+        u.mask = self.mask.data_ptr() if self.mask is not None else None
+        u.x_min = self.x_min.data_ptr() if self.x_min is not None else None
+        u.x_max = self.x_max.data_ptr() if self.x_max is not None else None
+        u.xhat_prev = self.xhat_prev.data_ptr() + fo if self.xhat_prev is not None else None
+        u.aux = self.aux.data_ptr() + fo if self.aux is not None else None
+        u.coef = self.coef.data_ptr()
+        u.predict_noise = 1 if predict_noise else 0
+        u.final_clip = 1 if consistency else 0
+        self._update_ops.append(op)
+        p.ops.append(op)
+        return u
 
     def build(self, w_cfg: float):
         for op in self._update_ops:
             op.u.update.w_cfg, op.u.update.w_uncond = float(w_cfg), float(1 - w_cfg)
         self.w_cfg = w_cfg
         self.handle = _make_handle(self.device, self.program.ops, self.n_iters)
+        if self.back is not None:
+            self.back_handle = _make_handle(self.device, self.back.ops, self.n_iters)
 
     def refresh_weights(self, epoch: int = 0):
         v = _weights_version(self.net, epoch)
@@ -242,14 +256,17 @@ class SamplerPlan:
         if self.version is None:         # packed at construction
             self.version = v
         elif v != self.version:
-            for fn in self.program.packers:
-                fn()
+            for prog in (self.program, self.back):
+                if prog is not None:
+                    for fn in prog.packers:
+                        fn()
             self.version = v
 
     def close(self):
-        if self.handle is not None:
-            self.handle.close()
-            self.handle = None
+        for h in (self.handle, self.back_handle):
+            if h is not None:
+                h.close()
+        self.handle = self.back_handle = None
 
     def fill_tables(self, t_all, cond_emb, t_key=None):
         """Per-call tables (time-conditioning rows, per-trajectory condition terms), once per ``sample()``."""
@@ -260,13 +277,6 @@ class SamplerPlan:
                 if fresh or not getattr(fn, "time_only", False):
                     fn(_Ctx(t_all, _cond_rows(self.cfg_mode, None if cond_emb is None else cond_emb[sl])))
         self._time_tables_key = (t_key, self.version) if t_key is not None else None
-
-    def run(self, t_all, cond_emb, use_graph=True, t_key=None, first=0, count=None, fill=True):
-        if fill:
-            self.fill_tables(t_all, cond_emb, t_key)
-        stream = torch.cuda.current_stream(self.device).cuda_stream if self.device.type == "cuda" else 0
-        self.handle.run(first, self.n_iters - first if count is None else count, stream, use_graph)
-        STATS["launches"] = self.handle.launches_per_iter() * self.n_iters + 1
 
     def run_guided(self, t_all, cond_emb, xt, noise_slots, guide, t_key=None):
         """The loop with a host callback between the denoiser and the update of every iteration (classifier guidance,
@@ -292,12 +302,14 @@ class SamplerPlan:
             self.handle.run_range(n, upd, 1, stream)
         STATS["launches"] = (self.handle.launches_per_iter() + 2) * self.n_iters + 1
 
-    def run_chunked(self, t_all, cond_emb, xt, noise_rows, use_graph=True, t_key=None):
+    def run_chunked(self, t_all, cond_emb, xt, noise_rows, t_key=None):
         """The whole loop, with the noise tape refilled between chunks when it is shorter than the number of draws
         (``noise_rows[n]`` = does iteration n draw?).  The draws are taken in loop order, so a seeded run consumes the
         generator like the reference loop; everything is enqueued on one stream, so a refill cannot overtake its readers."""
         cap = self.noise.shape[0] if self.noise is not None else 0
         self.fill_tables(t_all, cond_emb, t_key)
+        stream = torch.cuda.current_stream(self.device).cuda_stream if self.device.type == "cuda" else 0
+        use_graph = os.environ.get("CDS_GRAPH", "1") != "0"
         timed = STATS.get("time_loop") and self.device.type == "cuda"
         if timed:           # bench.py: device time of the reverse loop alone (noise draws + replayed iterations; events on the
             e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)    # launching stream)
@@ -308,11 +320,12 @@ class SamplerPlan:
                 draws = n < self.n_iters and bool(noise_rows[n])
                 if n == self.n_iters or (draws and used == cap):
                     if n > first:
-                        self.run(t_all, cond_emb, use_graph, t_key, first=first, count=n - first, fill=False)
+                        self.handle.run(first, n - first, stream, use_graph)
                     first, used = n, 0
                 if draws:
                     _draw_noise(self.noise[used], xt)
                     used += 1
+        STATS["launches"] = self.handle.launches_per_iter() * self.n_iters + 1
         if timed:
             e1.record()
             STATS.setdefault("loop_events", []).append((e0, e1))
@@ -351,12 +364,38 @@ def _cfg_mode(w_cfg, cond_emb):
     return 1 if w_cfg == 1.0 else 2
 
 
+def _screen(agent, xt, w_cfg, cond_emb, n_samples, decline=None):
+    """The request screen of every entry point -> ``(device, cfg_mode)`` when the engine serves the call, else None: quietly
+    under CDS_BACKEND=torch, on a device the engine does not serve and for a non-fp32 x_t (the caller's PyTorch loop runs), through
+    ``_fallback`` for a request the engine declines -- the caller's own ``decline(cfg_mode)`` reason first."""
+    if _backend() == "torch":
+        return None
+    device = _device_of(agent)
+    if not _device_ok(device) or xt.dtype != torch.float32:
+        return None
+    cfg_mode = _cfg_mode(w_cfg, cond_emb)
+    reason = decline(cfg_mode) if decline is not None else None
+    if reason is None and cfg_mode is None:
+        reason = "two-branch CFG without condition"
+    if reason is None and n_samples != xt.shape[0]:
+        reason = "n_samples != prior.shape[0]"
+    return (device, cfg_mode) if reason is None else _fallback(reason)
+
+
 def _get_plan(agent, key, factory):
-    """Plan cache of one agent: least-recently-used order, at most CDS_MAX_PLANS entries (each pins device buffers)."""
+    """Plan cache of one agent: least-recently-used order, at most CDS_MAX_PLANS entries (each pins device buffers).  A backbone
+    the lowering declines (``Unsupported``) or an option set the library refuses (``CdsError`` -3) is a fallback -> None."""
     plans = agent._engine_plans
     plan = plans.pop(key, None)
     if plan is None:
-        plan = factory()
+        try:
+            plan = factory()
+        except Unsupported as e:
+            return _fallback(str(e))
+        except cabi.CdsError as e:
+            if e.code == -3:
+                return _fallback(str(e))
+            raise
         limit = max(1, int(os.environ.get("CDS_MAX_PLANS", "8")))
         while len(plans) >= limit:
             old = plans.pop(next(iter(plans)))
@@ -374,41 +413,118 @@ def _cond_rows(cfg_mode, cond_emb):
     return torch.cat([c, torch.zeros_like(c)], 0) if cfg_mode == 2 else c
 
 
+# One schedule of an agent's table cache: the coefficient rows (noise slots numbered 1, 2, ...), the number of noise slots, the
+# time of every iteration on the device, and that column's bytes (``fill_tables`` skips the time-only fillers when they match).
+_Table = collections.namedtuple("_Table", "rows n_slots t t_key")
+
+
+def _schedule(agent, device, *, solver, sample_steps, order, step_values, alphas, sigmas, hs, stds, table, sched_id):
+    """The coefficient table of one ``sample()`` call, from the agent's table cache (cleared once it passes 16 entries).
+
+    ``table``: ``(rows, n_slots, time per iteration)``, or a zero-argument builder of it, or None for the SDE solvers (rows from
+    ``alphas`` / ``sigmas`` / ``hs`` / ``stds`` / ``step_values``).  ``sched_id``: a hashable the caller vouches for --
+    everything the table is a function of.  With it a hit skips the builder: no device->host read (each one a stream
+    synchronisation, which would keep the host from preparing call n + 1 while call n runs; 1-step samplers spend a quarter of
+    their wall time on the host), no per-step Python arithmetic (~10 ms for 100 SDE steps, more than a tenth of a cfg2
+    sample() on the engine), no host->device copy.  Without one, or for a table given by value, the cache is keyed on what the
+    table is built from."""
+    key = ("id", sched_id)
+    if table is None:                                  # the SDE solvers: the rows are a function of the schedule tensors
+        if sched_id is None:
+            key = ("content",) + tuple(z.detach().cpu().numpy().tobytes() for z in (step_values, alphas, sigmas, hs, stds))
+        table = lambda: _step_table(solver, sample_steps, order, step_values, alphas, sigmas, hs, stds)    # noqa: E731
+    elif sched_id is None or not callable(table):
+        rows, n_slots, t = table() if callable(table) else table
+        key, table = ("content", rows.numpy().tobytes(), t.detach().cpu().numpy().tobytes()), lambda: (rows, n_slots, t)
+    key += (solver, sample_steps, tuple(order), str(device))
+    cache = agent.__dict__.setdefault("_engine_tables", {})
+    entry = cache.get(key)
+    if entry is None:
+        rows, n_slots, t = table()
+        t = t.detach().cpu()
+        entry = _Table(rows, int(n_slots), t.to(device), t.numpy().tobytes())
+        if len(cache) > 16:
+            cache.clear()
+        cache[key] = entry
+    return entry
+
+
+def _step_table(solver, sample_steps, order, step_values, alphas, sigmas, hs, stds):
+    """The SDE solvers' rows (per-iteration scalars on the host, reference op order) -> ``(rows, n_slots, time per iteration)``."""
+    alphas, sigmas, hs, stds = (z.detach().float().cpu() for z in (alphas, sigmas, hs, stds))
+    step_values = step_values.detach().cpu()
+    table = S.coeff_table(solver, order, sample_steps, alphas, sigmas, hs, stds, step_values.double())
+    n_slots = 0
+    for n in range(len(order)):
+        if table[n, S.R_NOISE] > 0:
+            n_slots += 1
+            table[n, S.R_NOISE] = float(n_slots)       # 1 + slot index
+    return table, n_slots, step_values[torch.as_tensor(order, dtype=torch.long)]
+
+
+def _tape_slots(n_slots, batch, row):
+    """Noise tape: all draws of the loop up front when they fit CDS_NOISE_TAPE_MB (default 4096), else as many slots as fit (the
+    loop then runs in chunks with the tape refilled in between -- O(budget) memory instead of O(sample_steps x batch x row))."""
+    budget = int(float(os.environ.get("CDS_NOISE_TAPE_MB", "4096")) * (1 << 20))
+    return min(n_slots, max(1, budget // (4 * batch * row))) if n_slots > 0 else 0
+
+
+def _load_resident(agent, plan, xt, prior, tab: _Table, tape_slots):
+    """Fill the plan's resident buffers: x_t, the coefficient rows (when the schedule changed), prior and mask, clip bounds."""
+    with torch.no_grad():
+        plan.x.copy_(xt)
+        if getattr(plan, "_coef_of", None) is not tab:
+            rows = tab.rows
+            if tape_slots and tape_slots < tab.n_slots:      # slots are reused chunk by chunk: k-th draw -> slot k mod tape_slots
+                rows = rows.clone()
+                draws = rows[:, S.R_NOISE] > 0
+                rows[draws, S.R_NOISE] = (rows[draws, S.R_NOISE] - 1) % tape_slots + 1
+            plan.coef.copy_(rows)
+            plan._coef_of = tab
+        if plan.mask is not None:
+            plan.prior.copy_(prior)
+            plan.mask.copy_(_row(agent.fix_mask, plan.x_shape, plan.device))
+        if plan.x_min is not None:
+            plan.x_min.copy_(_row(agent.x_min, plan.x_shape, plan.device))
+        if plan.x_max is not None:
+            plan.x_max.copy_(_row(agent.x_max, plan.x_shape, plan.device))
+
+
 def try_sample(agent, *, model, xt, prior, solver, sample_steps, order, step_values, alphas, sigmas, hs, stds,
                cond_emb, w_cfg, n_samples, guide=None, table=None, clip_in_loop=True, predict_noise=None, sched_id=None,
-               classifier=None, w_cg=0.0):
-    """``table``: optional ready-made ``(coefficient rows [n_iters, ROW], number of noise slots, int64/float32 time per iteration)``
-    for samplers that are "the same update kernel with another coefficient table" (the legacy DDPM class, RectifiedFlow's Euler
-    step): ``solver`` / ``alphas`` / ``sigmas`` / ``hs`` / ``stds`` / ``step_values`` are then unused.
-    ``clip_in_loop=False``: the sampler clips only its final sample (RectifiedFlow); ``predict_noise``: overrides
-    ``agent.predict_noise`` (classes without that attribute).
+               classifier=None, w_cg=0.0, consistency=False, aux_history=False):
+    """One ``sample()`` call of any sampler family on the engine -> x0, or None when the caller's PyTorch loop must run.
+
+    ``table``: the coefficient rows for samplers that are "the same update kernel with another coefficient table" (the legacy
+    DDPM and EDM classes, RectifiedFlow's Euler step, ContinuousConsistencyModel, ContinuousEDM), see ``_schedule``;
+    ``solver`` / ``alphas`` / ``sigmas`` / ``hs`` / ``stds`` / ``step_values`` then serve only as keys or are unused.
+    ``clip_in_loop=False``: the sampler clips only its final sample (RectifiedFlow, legacy EDM); ``predict_noise``: overrides
+    ``agent.predict_noise`` (classes without that attribute).  ``consistency``: the EDM-preconditioned family (CDS_OP_PREP in
+    front of the denoiser, c_skip / c_out combine and final clip in the update); ``aux_history``: the EDM Heun corrector's
+    history buffers.
     ``guide``: optional host callback ``guide(n, i, x_t, pred)`` (n = iteration, i = its loop index) run between the denoiser
     and the update of every iteration (classifier guidance); the loop then runs step by step instead of as a replayed graph --
     unless ``classifier`` (the one ``guide`` evaluates, with weight ``w_cg``) is a CumRewClassifier over HalfJannerUNet1d under
     CDS_MATH = fp32 | tf32 with one sub-batch chain: its input gradient and the guidance term are then operators of the replayed
     program, and ``guide`` is not called."""
-    if _backend() == "torch":
+    def decline(cfg_mode):
+        if guide is not None and cfg_mode == 2:
+            # the update operator combines the two CFG branches itself; a guidance term would have to enter after that combine
+            return "classifier guidance together with two-branch classifier-free guidance"
         return None
-    device = _device_of(agent)
-    if not _device_ok(device) or xt.dtype != torch.float32:
+    screened = _screen(agent, xt, w_cfg, cond_emb, n_samples, decline)
+    if screened is None:
         return None
+    device, cfg_mode = screened
     net = model["diffusion"]
-    cfg_mode = _cfg_mode(w_cfg, cond_emb)
-    if cfg_mode is None:
-        return _fallback("two-branch CFG without condition")
     batch, x_shape = xt.shape[0], tuple(xt.shape[1:])
-    if n_samples != batch:
-        return _fallback("n_samples != prior.shape[0]")
-    if guide is not None and cfg_mode == 2:
-        # the update operator combines the two CFG branches itself; a guidance term would have to enter after that combine
-        return _fallback("classifier guidance together with two-branch classifier-free guidance")
-
-    table, n_slots, t_cpu, sched_key, order, table_given = _step_table(
-        agent, solver=solver, sample_steps=sample_steps, order=order, step_values=step_values, alphas=alphas, sigmas=sigmas,
-        hs=hs, stds=stds, table=table, sched_id=sched_id)
-    keep_history = (not table_given) and S.solver_keeps_history(solver)
+    keep_history = aux_history or (table is None and S.solver_keeps_history(solver))     # multistep SDE solvers, EDM Heun
+    tab = _schedule(agent, device, solver=solver, sample_steps=sample_steps, order=order, step_values=step_values, alphas=alphas,
+                    sigmas=sigmas, hs=hs, stds=stds, table=table, sched_id=sched_id)
+    n_iters = tab.rows.shape[0]
     has_mask = isinstance(agent.fix_mask, torch.Tensor)
-    has_min, has_max = (agent.x_min is not None and clip_in_loop), (agent.x_max is not None and clip_in_loop)
+    has_min = clip_in_loop and getattr(agent, "x_min", None) is not None
+    has_max = clip_in_loop and getattr(agent, "x_max", None) is not None
     pn = bool(agent.predict_noise) if predict_noise is None else bool(predict_noise)
     math = _math_mode()
     row_elems = 1
@@ -422,32 +538,21 @@ def try_sample(agent, *, model, xt, prior, solver, sample_steps, order, step_val
         if cg_reason is None and _n_branches(batch, row_elems, False) != 1:
             cg_reason = "more than one sub-batch chain (CDS_BRANCHES)"
     lowered_cg = guide is not None and cg_reason is None
-    # noise tape: all draws of the loop up front when they fit the budget, else as many slots as fit (the loop then runs in
-    # chunks with the tape refilled in between -- O(budget) memory instead of O(sample_steps x batch x row))
-    tape_slots = min(n_slots, max(1, _tape_budget_bytes() // (4 * batch * row_elems))) if n_slots > 0 else 0
-    key = ("sde", id(net), batch, x_shape, len(order), tape_slots, cfg_mode, pn, has_mask,
-           has_min, has_max, keep_history, math, float(w_cfg) if cfg_mode == 2 else 0.0,
-           id(classifier.model_ema) if lowered_cg else None)
+    tape_slots = _tape_slots(tab.n_slots, batch, row_elems)
+    key = (id(net), batch, x_shape, n_iters, tape_slots, cfg_mode, pn, has_mask, has_min, has_max, keep_history, aux_history,
+           consistency, math, float(w_cfg) if cfg_mode == 2 else 0.0, id(classifier.model_ema) if lowered_cg else None)
 
     def factory():
-        plan = SamplerPlan(device, net, batch, x_shape, len(order), tape_slots, cfg_mode=cfg_mode,
-                           predict_noise=pn, has_mask=has_mask, has_min=has_min, has_max=has_max,
-                           keep_history=keep_history, math=math, classifier=classifier if lowered_cg else None)
+        plan = SamplerPlan(device, net, batch, x_shape, n_iters, tape_slots, cfg_mode=cfg_mode, predict_noise=pn,
+                           has_mask=has_mask, has_min=has_min, has_max=has_max, keep_history=keep_history, math=math,
+                           consistency=consistency, aux_history=aux_history, classifier=classifier if lowered_cg else None)
         plan.build(w_cfg)
         return plan
 
-    try:
-        plan = _get_plan(agent, key, factory)
-    except Unsupported as e:
-        return _fallback(str(e))
-    except cabi.CdsError as e:
-        if e.code == -3:
-            return _fallback(str(e))
-        raise
-
-    t_all = _load_resident(agent, plan, xt, prior, table, sched_key, tape_slots, n_slots, x_shape, order, t_cpu, device)
-    # the loop's draws: same calls, same order, same shapes as the reference loop's (diffusionsde.py:548,571,...)
-    t_key = (t_cpu.numpy().tobytes(), tuple(order))
+    plan = _get_plan(agent, key, factory)
+    if plan is None:
+        return None
+    _load_resident(agent, plan, xt, prior, tab, tape_slots)
     STATS["guidance_path"], STATS["guidance_reason"] = None, cg_reason
     if lowered_cg:
         # the guidance scale of every iteration, the reference's own expression (classifier_guidance), evaluated on the device
@@ -462,252 +567,10 @@ def try_sample(agent, *, model, xt, prior, solver, sample_steps, order, step_val
         if plan.n_branches != 1 or getattr(plan, "pred", None) is None:
             return _fallback("guided sampling needs a single-branch program with a dense prediction buffer")
         slots = plan.coef[:, S.R_NOISE].cpu().tolist()              # tape slot per iteration as the update kernel sees it
-        plan.run_guided(t_all, cond_emb, xt, slots, lambda n, x, p: guide(n, order[n], x, p), t_key=t_key)
+        plan.run_guided(tab.t, cond_emb, xt, slots, lambda n, x, p: guide(n, order[n], x, p), t_key=tab.t_key)
     else:
-        plan.run_chunked(t_all, cond_emb, xt, (table[:, S.R_NOISE] > 0).tolist(),
-                         use_graph=os.environ.get("CDS_GRAPH", "1") != "0", t_key=t_key)
-    STATS["engine_calls"] += 1
-    return plan.x.clone()
-
-
-def _step_table(agent, *, solver, sample_steps, order, step_values, alphas, sigmas, hs, stds, table, sched_id):
-    """The coefficient table of one ``sample()`` call -> ``(table [n_iters, ROW], number of noise slots, time per step (CPU),
-    schedule key, iteration order, table_given)``."""
-    # ---- per-iteration scalars (host, reference op order); identical requests reuse the table (building it costs ~10 ms
-    # of Python scalar arithmetic for 100 steps -- more than a tenth of a whole cfg2 sample() on the engine) ---------------
-    table_given = table is not None
-    if table_given:
-        rows_given, slots_given, t_given = table
-        t_cpu = t_given.detach().cpu()
-        order = list(range(rows_given.shape[0]))
-        sched_key = (solver, rows_given.numpy().tobytes(), t_cpu.numpy().tobytes())
-        cached = (rows_given, int(slots_given))
-    else:
-        # ``sched_id``: a hashable the caller vouches for -- everything alphas / sigmas / hs / stds / step_values are functions of.
-        # A hit skips the five device->host reads below: each of them is a stream synchronisation, which would keep the host from
-        # preparing call n + 1 while call n still runs (1-step samplers: a quarter of the wall time).
-        fast_key = None if sched_id is None else (sched_id, solver, sample_steps, tuple(order))
-        fast = agent.__dict__.setdefault("_engine_sched_ids", {}).get(fast_key) if fast_key is not None else None
-        if fast is not None:
-            sched_key, t_cpu = fast
-            cached = agent._engine_tables.get(sched_key) if hasattr(agent, "_engine_tables") else None
-        else:
-            cached = None
-        if cached is None:
-            alphas_c, sigmas_c, hs_c, stds_c = (z.detach().float().cpu() for z in (alphas, sigmas, hs, stds))
-            t_cpu = step_values.detach().cpu()
-            sched_key = (solver, sample_steps, tuple(order), alphas_c.numpy().tobytes(), sigmas_c.numpy().tobytes(),
-                         hs_c.numpy().tobytes(), stds_c.numpy().tobytes(), t_cpu.numpy().tobytes())
-            cached = agent._engine_tables.get(sched_key) if hasattr(agent, "_engine_tables") else None
-            if fast_key is not None:
-                if len(agent._engine_sched_ids) > 16:
-                    agent._engine_sched_ids.clear()
-                agent._engine_sched_ids[fast_key] = (sched_key, t_cpu)
-    if cached is None:
-        table = S.coeff_table(solver, order, sample_steps, alphas_c, sigmas_c, hs_c, stds_c, t_cpu.double())
-        n_slots = 0
-        for n in range(len(order)):
-            if table[n, S.R_NOISE] > 0:
-                n_slots += 1
-                table[n, S.R_NOISE] = float(n_slots)       # 1 + slot index
-        if not hasattr(agent, "_engine_tables"):
-            agent._engine_tables = {}
-        if len(agent._engine_tables) > 16:
-            agent._engine_tables.clear()
-        agent._engine_tables[sched_key] = (table, n_slots)
-    else:
-        table, n_slots = cached
-    return table, n_slots, t_cpu, sched_key, order, table_given
-
-
-def _load_resident(agent, plan, xt, prior, table, sched_key, tape_slots, n_slots, x_shape, order, t_cpu, device):
-    """Fill the plan's resident buffers (x_t, coefficient rows, mask, clip bounds) -> the time value of every iteration."""
-    with torch.no_grad():
-        plan.x.copy_(xt)
-        if getattr(plan, "_coef_key", None) != sched_key:
-            if tape_slots and tape_slots < n_slots:          # slots are reused chunk by chunk: k-th draw -> slot k mod tape_slots
-                local = table.clone()
-                draws = local[:, S.R_NOISE] > 0
-                local[draws, S.R_NOISE] = (local[draws, S.R_NOISE] - 1) % tape_slots + 1
-                plan.coef.copy_(local)
-            else:
-                plan.coef.copy_(table)
-            plan._coef_key = sched_key
-        if plan.mask is not None:
-            plan.prior.copy_(prior)
-            plan.mask.copy_(_row(agent.fix_mask, x_shape, device))
-        if plan.x_min is not None:
-            plan.x_min.copy_(_row(agent.x_min, x_shape, device))
-        if plan.x_max is not None:
-            plan.x_max.copy_(_row(agent.x_max, x_shape, device))
-        idx = torch.as_tensor(order, dtype=torch.long)
-        return t_cpu[idx].to(device)      # int64 (discrete) or float32 (continuous), one entry per iteration
-
-
-def try_sample_consistency(agent, *, model, xt, prior, sigmas, order, cond_emb, n_samples, sched_id=None):
-    """ContinuousConsistencyModel.sample on the engine: iteration 0 evaluates f at sigma_max, the following
-    iterations re-noise to sigma_i and evaluate f again (consistency_model.py:401-426)."""
-    if _backend() == "torch":
-        return None
-    device = _device_of(agent)
-    if not _device_ok(device) or xt.dtype != torch.float32:
-        return None
-    net = model["diffusion"]
-    batch, x_shape = xt.shape[0], tuple(xt.shape[1:])
-    if n_samples != batch:
-        return _fallback("n_samples != prior.shape[0]")
-    cfg_mode = 0 if cond_emb is None else 1
-    # ``sched_id`` (see try_sample): a hit reuses the coefficient table and its device copy of the time column -- no device->host
-    # read, so the host can prepare the next call while this one runs (the 1-step sampler is 8 ms of GPU work per call)
-    cm_key = None if sched_id is None else (sched_id, tuple(order), str(device))
-    hit = agent.__dict__.setdefault("_engine_cm_tables", {}).get(cm_key) if cm_key is not None else None
-    sig = None if hit is not None else sigmas.detach().float().cpu()
-    levels = [] if hit is not None else [sig[-1]] + [sig[i] for i in order]
-    n_iters = hit[0].shape[0] if hit is not None else len(levels)
-    sd, smin = agent.sigma_data, agent.sigma_min
-    table = hit[0] if hit is not None else torch.zeros((n_iters, S.ROW), dtype=torch.float32)
-    for n, s in enumerate(levels):                     # 0-d fp32 tensors, reference op order (:241-251, :423)
-        table[n, S.R_K0] = float(sd ** 2 / (sd ** 2 + (s - smin) ** 2))                      # c_skip
-        table[n, S.R_K1] = float((s - smin) * sd / (sd ** 2 + s ** 2).sqrt())               # c_out
-        table[n, S.R_K3] = float(1 / (sd ** 2 + s ** 2).sqrt())                              # c_in
-        table[n, S.R_KIND] = float(S.UPD_CM)
-        if n > 0:
-            table[n, S.R_K2] = float((s ** 2 - smin ** 2).sqrt())                            # re-noise scale
-            table[n, S.R_NOISE] = float(n)
-        table[n, S.R_T] = float(0.25 * s.log())                                               # c_noise
-    n_slots = n_iters - 1
-    has_mask = isinstance(agent.fix_mask, torch.Tensor)
-    has_min, has_max = agent.x_min is not None, agent.x_max is not None
-    math = _math_mode()
-    key = ("cm", id(net), batch, x_shape, n_iters, cfg_mode, has_mask, has_min, has_max, math)
-
-    def factory():
-        plan = SamplerPlan(device, net, batch, x_shape, n_iters, n_slots, cfg_mode=cfg_mode, predict_noise=False,
-                           has_mask=has_mask, has_min=has_min, has_max=has_max, keep_history=False, math=math,
-                           consistency=True)
-        plan.build(1.0)
-        return plan
-
-    try:
-        plan = _get_plan(agent, key, factory)
-    except Unsupported as e:
-        return _fallback(str(e))
-    except cabi.CdsError as e:
-        if e.code == -3:
-            return _fallback(str(e))
-        raise
-    with torch.no_grad():
-        plan.x.copy_(xt)
-        plan.coef.copy_(table, non_blocking=True)
-        if has_mask:
-            plan.prior.copy_(prior)
-            plan.mask.copy_(_row(agent.fix_mask, x_shape, device))
-        if has_min:
-            plan.x_min.copy_(_row(agent.x_min, x_shape, device))
-        if has_max:
-            plan.x_max.copy_(_row(agent.x_max, x_shape, device))
-        for k in range(n_slots):
-            _draw_noise(plan.noise[k], xt)
-        if hit is not None:
-            t_all = hit[1]
-        else:
-            t_all = table[:, S.R_T].to(device)         # the network sees c_noise = ln(sigma)/4 as its "time"
-            if cm_key is not None:
-                if len(agent._engine_cm_tables) > 16:
-                    agent._engine_cm_tables.clear()
-                agent._engine_cm_tables[cm_key] = (table, t_all)
-    plan.run(t_all, cond_emb, use_graph=os.environ.get("CDS_GRAPH", "1") != "0")
-    STATS["engine_calls"] += 1
-    return plan.x.clone()
-
-
-def try_sample_edm(agent, *, model, xt, prior, solver, sigmas, order, cond_emb, w_cfg, n_samples, evals=None, clip=True,
-                   sched_id=None):
-    """ContinuousEDM.sample on the engine (newedm.py:395-431).  Every network evaluation is one engine iteration:
-    ``euler``: one per reverse step; ``heun``: predictor + corrector (two evaluations) for every step but the last.
-    ``sigmas``: the Karras grid (sample_steps + 1 entries, fp32), ``order``: the reverse steps i in loop order."""
-    if _backend() == "torch":
-        return None
-    device = _device_of(agent)
-    if not _device_ok(device) or xt.dtype != torch.float32:
-        return None
-    net = model["diffusion"]
-    cfg_mode = _cfg_mode(w_cfg, cond_emb)
-    if cfg_mode is None:
-        return _fallback("two-branch CFG without condition")
-    batch, x_shape = xt.shape[0], tuple(xt.shape[1:])
-    if n_samples != batch:
-        return _fallback("n_samples != prior.shape[0]")
-    sd = agent.sigma_data
-    given = evals is not None                    # legacy EDM: the caller lists the evaluations (sigma, kind, dt, flag, xw, dw)
-    # ``sched_id`` (see try_sample): a hit reuses the table without reading the Karras grid back from the device
-    edm_key = None if (sched_id is None or given) else (sched_id, solver, tuple(order), str(device))
-    hit = agent.__dict__.setdefault("_engine_edm_tables", {}).get(edm_key) if edm_key is not None else None
-    sig = sigmas.detach().float().cpu() if (not given and hit is None) else None
-    evals = list(evals) if given else []         # (sigma of the evaluation, kind, dt, predictor flag[, x_weight, D_weight])
-    for i in ([] if (given or hit is not None) else order):
-        dt = sig[i] - sig[i - 1]
-        heun = solver == "heun" and i > 1
-        evals.append((sig[i], S.UPD_EDM, dt, 1.0 if heun else 0.0))
-        if heun:
-            # the corrector evaluates at t = t_i / sigma_i * sigma_{i-1} (newedm.py:421) = sigma_{i-1} exactly (x / x == 1)
-            evals.append((sig[i - 1], S.UPD_EDM_HEUN, dt, 0.0))
-    n_iters = hit[0].shape[0] if hit is not None else len(evals)
-    table = hit[0] if hit is not None else torch.zeros((n_iters, S.ROW), dtype=torch.float32)
-    for n, ev in enumerate(evals):                         # 0-d fp32 tensors, reference op order (newedm.py:128-148)
-        s, kind, dt, pred_flag = ev[:4]
-        if len(ev) > 4:
-            table[n, S.R_XW], table[n, S.R_DW] = float(ev[4]), float(ev[5])
-        table[n, S.R_K0] = float(sd ** 2 / (sd ** 2 + s ** 2))                  # c_skip
-        table[n, S.R_K1] = float(s * sd / (sd ** 2 + s ** 2).sqrt())            # c_out
-        table[n, S.R_K3] = float(1 / (sd ** 2 + s ** 2).sqrt())                 # c_in
-        table[n, S.R_K2] = float(dt)
-        table[n, S.R_K4] = pred_flag
-        table[n, S.R_SIGMA] = float(s)                                          # the slope divides by it
-        table[n, S.R_KIND] = float(kind)
-        table[n, S.R_T] = float(0.25 * s.log())                                 # c_noise
-    has_mask = isinstance(agent.fix_mask, torch.Tensor)
-    has_min = clip and getattr(agent, "x_min", None) is not None
-    has_max = clip and getattr(agent, "x_max", None) is not None
-    math = _math_mode()
-    heun = solver == "heun"
-    key = ("edm", id(net), batch, x_shape, n_iters, cfg_mode, has_mask, has_min, has_max, heun, math,
-           float(w_cfg) if cfg_mode == 2 else 0.0)
-
-    def factory():
-        plan = SamplerPlan(device, net, batch, x_shape, n_iters, 0, cfg_mode=cfg_mode, predict_noise=False,
-                           has_mask=has_mask, has_min=has_min, has_max=has_max, keep_history=heun, math=math,
-                           consistency=True, aux_history=heun)
-        plan.build(w_cfg)
-        return plan
-
-    try:
-        plan = _get_plan(agent, key, factory)
-    except Unsupported as e:
-        return _fallback(str(e))
-    except cabi.CdsError as e:
-        if e.code == -3:
-            return _fallback(str(e))
-        raise
-    with torch.no_grad():
-        plan.x.copy_(xt)
-        plan.coef.copy_(table, non_blocking=True)
-        if has_mask:
-            plan.prior.copy_(prior)
-            plan.mask.copy_(_row(agent.fix_mask, x_shape, device))
-        if has_min:
-            plan.x_min.copy_(_row(agent.x_min, x_shape, device))
-        if has_max:
-            plan.x_max.copy_(_row(agent.x_max, x_shape, device))
-        if hit is not None:
-            t_all = hit[1]
-        else:
-            t_all = table[:, S.R_T].to(device)         # the network sees c_noise = ln(sigma)/4 as its "time"
-            if edm_key is not None:
-                if len(agent._engine_edm_tables) > 16:
-                    agent._engine_edm_tables.clear()
-                agent._engine_edm_tables[edm_key] = (table, t_all)
-    plan.run(t_all, cond_emb, use_graph=os.environ.get("CDS_GRAPH", "1") != "0")
+        # the loop's draws: same calls, same order, same shapes as the reference loop's (diffusionsde.py:548,571,...)
+        plan.run_chunked(tab.t, cond_emb, xt, (tab.rows[:, S.R_NOISE] > 0).tolist(), t_key=tab.t_key)
     STATS["engine_calls"] += 1
     return plan.x.clone()
 
@@ -720,36 +583,13 @@ class GradSamplerPlan(SamplerPlan):
     no CFG combine, no solver history."""
 
     def __init__(self, device, net, batch, x_shape, n_iters, n_slots, *, predict_noise, has_mask, has_min, has_max, math):
-        self.device, self.net, self.batch, self.x_shape = device, net, batch, tuple(x_shape)
-        row = x_shape[0]
-        self.row, self.n_iters, self.cfg_mode, self.n_branches = row, n_iters, 1, 1
-        root = Program(device, batch, n_iters, math)
-        back = Program(device, batch, n_iters, math)
-        self.program, self.back = root, back
-        self.x = root.buf(batch, row)
-        self.prior = root.buf(batch, row) if has_mask else None
-        self.mask = root.buf(row) if has_mask else None
-        self.x_min = root.buf(row) if has_min else None
-        self.x_max = root.buf(row) if has_max else None
-        self.coef = root.buf(n_iters, cabi.ROW_FLOATS)
-        self.noise = root.buf(max(n_slots, 1), batch, row) if n_slots > 0 else None
-        self.grad = g = DQLGrad(root, back, net, View(self.x, 1, row))
+        self._resident(device, net, batch, x_shape, n_iters, n_slots, cfg_mode=1, has_mask=has_mask, has_min=has_min,
+                       has_max=has_max, keep_history=False, aux_history=False, math=math)
+        self.n_branches, row = 1, self.row
+        self.back = back = Program(device, batch, n_iters, math)
+        self.grad = g = DQLGrad(self.program, back, net, View(self.x, 1, row))
         self.pred = g.pred.t
-
-        op = cabi.Op()
-        op.kind = cabi.OP_UPDATE
-        u = op.u.update
-        u.batch, u.row, u.x, u.pred = batch, row, self.x.data_ptr(), g.pred.ptr
-        if self.noise is not None:
-            u.noise, u.noise_slot_stride = self.noise.data_ptr(), batch * row
-        u.prior = self.prior.data_ptr() if has_mask else None
-        u.mask = self.mask.data_ptr() if has_mask else None
-        u.x_min = self.x_min.data_ptr() if has_min else None
-        u.x_max = self.x_max.data_ptr() if has_max else None
-        u.coef = self.coef.data_ptr()
-        u.predict_noise = 1 if predict_noise else 0
-        root.ops.append(op)
-        self._update_ops = [op]
+        u = self._update_op(self.program, g.pred.ptr, batch, 0, predict_noise)
 
         bop = cabi.Op()                                      # the update's backward opens every backward iteration
         bop.kind = cabi.OP_UPDATE_BWD
@@ -762,31 +602,7 @@ class GradSamplerPlan(SamplerPlan):
         b.coef, b.coef_iter_stride = _rev(self.coef)
         b.predict_noise = u.predict_noise
         back.ops.insert(0, bop)
-
-        self._fillers = []                 # the tables are autograd inputs, copied in by _GradSampleFn
-        self.handle: Optional[cabi.Plan] = None
-        self.back_handle: Optional[cabi.Plan] = None
-        self.version = None
         self.generation = 0                # forward runs so far: a backward must belong to the latest one
-
-    def build(self, w_cfg: float):
-        super().build(w_cfg)
-        self.back_handle = _make_handle(self.device, self.back.ops, self.n_iters)
-
-    def refresh_weights(self, epoch: int = 0):
-        v = _weights_version(self.net, epoch)
-        if self.version is None:
-            self.version = v
-        elif v != self.version:
-            for fn in self.program.packers + self.back.packers:
-                fn()
-            self.version = v
-
-    def close(self):
-        super().close()
-        if self.back_handle is not None:
-            self.back_handle.close()
-            self.back_handle = None
 
     def backward(self, grad_x0, generation):
         """d x0 -> the gradients of the Function's inputs (step_tab, samp_tab, W_x, W2, b2, W3, b3, W_f, b_f)."""
@@ -835,38 +651,35 @@ def try_sample_grad(agent, *, model, xt, prior, solver, sample_steps, order, ste
     """``sample(requires_grad=True)`` on the engine: x0 connected to autograd through ``_GradSampleFn``.  Covers DQLMlp with
     the DDPM / DDIM / first-order DPM-Solver updates, one CFG branch and CDS_MATH = fp32 | tf32; everything else takes the
     PyTorch loop (which autograd differentiates) through ``_fallback``."""
-    if _backend() == "torch":
-        return None
-    device = _device_of(agent)
-    if not _device_ok(device) or xt.dtype != torch.float32:
-        return None
     net = model["diffusion"]
-    name = type(net).__name__
-    if name != "DQLMlp" or xt.dim() != 2:
-        return _fallback(f"requires_grad=True: backbone {name} has no differentiable engine program (DQLMlp only)")
-    if S.solver_keeps_history(solver):
-        return _fallback(f"requires_grad=True with the multistep solver {solver} (history)")
-    cfg_mode = _cfg_mode(w_cfg, cond_emb)
-    if cfg_mode is None or cfg_mode == 2:
-        return _fallback("requires_grad=True with two-branch classifier-free guidance")
-    if guided:
-        return _fallback("requires_grad=True with classifier guidance")
-    math = _math_mode()
-    if math == cabi.MATH_BF16_TC:
-        return _fallback("requires_grad=True with CDS_MATH=bf16 (fp32 and tf32 only)")
-    batch, x_shape = xt.shape[0], tuple(xt.shape[1:])
-    if n_samples != batch:
-        return _fallback("n_samples != prior.shape[0]")
 
-    table, n_slots, t_cpu, sched_key, order, _ = _step_table(
-        agent, solver=solver, sample_steps=sample_steps, order=order, step_values=step_values, alphas=alphas, sigmas=sigmas,
-        hs=hs, stds=stds, table=None, sched_id=sched_id)
+    def decline(cfg_mode):
+        name = type(net).__name__
+        if name != "DQLMlp" or xt.dim() != 2:
+            return f"requires_grad=True: backbone {name} has no differentiable engine program (DQLMlp only)"
+        if S.solver_keeps_history(solver):
+            return f"requires_grad=True with the multistep solver {solver} (history)"
+        if cfg_mode is None or cfg_mode == 2:
+            return "requires_grad=True with two-branch classifier-free guidance"
+        if guided:
+            return "requires_grad=True with classifier guidance"
+        if _math_mode() == cabi.MATH_BF16_TC:
+            return "requires_grad=True with CDS_MATH=bf16 (fp32 and tf32 only)"
+        return None
+    screened = _screen(agent, xt, w_cfg, cond_emb, n_samples, decline)
+    if screened is None:
+        return None
+    device, cfg_mode = screened
+    batch, x_shape = xt.shape[0], tuple(xt.shape[1:])
+    tab = _schedule(agent, device, solver=solver, sample_steps=sample_steps, order=order, step_values=step_values, alphas=alphas,
+                    sigmas=sigmas, hs=hs, stds=stds, table=None, sched_id=sched_id)
     has_mask = isinstance(agent.fix_mask, torch.Tensor)
     has_min, has_max = agent.x_min is not None, agent.x_max is not None
     pn = bool(agent.predict_noise)
-    tape_slots = min(n_slots, max(1, _tape_budget_bytes() // (4 * batch * x_shape[0]))) if n_slots > 0 else 0
-    key = ("sde", id(net), batch, x_shape, len(order), tape_slots, cfg_mode, pn, has_mask, has_min, has_max, False, math, 0.0,
-           "grad")
+    math = _math_mode()
+    tape_slots = _tape_slots(tab.n_slots, batch, x_shape[0])
+    key = (id(net), batch, x_shape, len(order), tape_slots, cfg_mode, pn, has_mask, has_min, has_max, False, False, False, math,
+           0.0, None, "grad")
 
     def factory():
         plan = GradSamplerPlan(device, net, batch, x_shape, len(order), tape_slots, predict_noise=pn, has_mask=has_mask,
@@ -874,27 +687,21 @@ def try_sample_grad(agent, *, model, xt, prior, solver, sample_steps, order, ste
         plan.build(1.0)
         return plan
 
-    try:
-        plan = _get_plan(agent, key, factory)
-    except Unsupported as e:
-        return _fallback(str(e))
-    except cabi.CdsError as e:
-        if e.code == -3:
-            return _fallback(str(e))
-        raise
-
-    t_all = _load_resident(agent, plan, xt, prior, table, sched_key, tape_slots, n_slots, x_shape, order, t_cpu, device)
+    plan = _get_plan(agent, key, factory)
+    if plan is None:
+        return None
+    _load_resident(agent, plan, xt, prior, tab, tape_slots)
     lin1, fl = net.mid_layer[0], net.final_layer
     a, e = x_shape[0], net.time_mlp[2].out_features
     with torch.enable_grad():
         # the per-call tables with autograd: Linear over cat[x, time_mlp(map_noise(t)), obs] = W_x x + (W_t temb + b) + W_o obs
-        step_tab = F.linear(net.time_mlp(net.map_noise(t_all)), lin1.weight[:, a:a + e], lin1.bias)
+        step_tab = F.linear(net.time_mlp(net.map_noise(tab.t)), lin1.weight[:, a:a + e], lin1.bias)
         if cfg_mode == 1:
             samp_tab = F.linear(_cond_rows(cfg_mode, cond_emb), lin1.weight[:, a + e:])
         else:
             samp_tab = torch.zeros((batch, lin1.out_features), device=device)
-        noise_rows = (table[:, S.R_NOISE] > 0).tolist()
-        run = lambda: plan.run_chunked(t_all, None, xt, noise_rows, use_graph=os.environ.get("CDS_GRAPH", "1") != "0")  # noqa: E731
+        noise_rows = (tab.rows[:, S.R_NOISE] > 0).tolist()
+        run = lambda: plan.run_chunked(tab.t, None, xt, noise_rows)  # noqa: E731
         x0 = _GradSampleFn.apply(plan, run, step_tab, samp_tab, lin1.weight[:, :a], net.mid_layer[2].weight,
                                  net.mid_layer[2].bias, net.mid_layer[4].weight, net.mid_layer[4].bias, fl.weight, fl.bias)
     STATS["engine_calls"] += 1

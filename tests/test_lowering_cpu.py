@@ -203,9 +203,27 @@ def test_table_caches_follow_the_request(golden):
 
 
 def test_schedule_identity_fast_path_is_keyed_on_what_the_schedule_depends_on(golden):
-    """The discrete sampler hands the engine a ``sched_id`` (named step schedule, grid length, identity + version of the alpha /
-    sigma buffers); a repeated request must not read the schedule back from the device (on a GPU each read is a stream
-    synchronisation), a changed schedule must miss."""
+    """The samplers hand the engine a ``sched_id``: the discrete SDE sampler its named step schedule, grid length and the identity +
+    version of the alpha / sigma buffers; the consistency and EDM samplers their step count and sigma grid parameters.  A repeated
+    request must not read the schedule back from the device (on a GPU each read is a stream synchronisation), a changed schedule
+    must miss.  All of them share the agent's one table cache."""
+    from test_edm import build_edm
+
+    def ids(agent):                                        # the cache entries keyed on a schedule identity
+        return [k for k in agent._engine_tables if k[0] == "id"]
+
+    def hit(agent, run, steps):
+        reads = []
+        real_cpu = torch.Tensor.cpu
+        try:
+            torch.Tensor.cpu = lambda self, *a, **k: (reads.append(tuple(self.shape)), real_cpu(self, *a, **k))[1]
+            out = run()
+        finally:
+            torch.Tensor.cpu = real_cpu
+        assert not [r for r in reads if r == (steps,) or r == (steps + 1,)], reads     # no schedule read-back
+        assert len(ids(agent)) == 1
+        return out
+
     name = "disc_dup_ddpm_x0"
     spec = cases.sampler_cases()[name]
     agent, inp, kw = build_agent(spec)
@@ -216,24 +234,45 @@ def test_schedule_identity_fast_path_is_keyed_on_what_the_schedule_depends_on(go
             return agent.sample(inp["prior"], **{**kw, **over})[0].numpy()
 
     a0 = run()
-    assert len(agent._engine_sched_ids) == 1
-    (key0, (sched_key0, _)), = agent._engine_sched_ids.items()
-    reads = []
-    real_cpu = torch.Tensor.cpu
-    try:
-        torch.Tensor.cpu = lambda self, *a, **k: (reads.append(tuple(self.shape)), real_cpu(self, *a, **k))[1]
-        a1 = run()
-    finally:
-        torch.Tensor.cpu = real_cpu
-    np.testing.assert_array_equal(a1, a0)
-    assert not [r for r in reads if r == (kw["sample_steps"],) or r == (kw["sample_steps"] + 1,)], reads   # no schedule read-back
-    assert len(agent._engine_sched_ids) == 1
+    assert len(ids(agent)) == 1
+    np.testing.assert_array_equal(hit(agent, run, kw["sample_steps"]), a0)
     with torch.no_grad():
         agent.alpha.mul_(0.999)                            # the schedule changes in place -> version bump -> new identity
     a2 = run()
-    assert len(agent._engine_sched_ids) == 2 and np.abs(a2 - a0).max() > 1e-6
+    assert len(ids(agent)) == 2 and np.abs(a2 - a0).max() > 1e-6
     run(sample_step_schedule=lambda T, S: torch.arange(S + 1) * (T - 1) // S)       # callables carry no identity: no entry
-    assert len(agent._engine_sched_ids) == 2
+    assert len(ids(agent)) == 2
+
+    g = golden["consistency"]
+    net, _ = product_net(cases.NETS["chi_cm_fourier"])
+    cm = ContinuousConsistencyModel(net, IdentityCondition(dropout=0.0), x_max=torch.ones(1, 8, 3),
+                                    x_min=-torch.ones(1, 8, 3), device="cpu")
+
+    def run_cm():
+        with NoiseTape(tape_of(g, "cm3")).active(), torch.no_grad():
+            return cm.sample(torch.zeros(4, 8, 3), n_samples=4, sample_steps=3, condition_cfg=torch.as_tensor(g["cm3/cond"]),
+                             w_cfg=1.0)[0].numpy()
+
+    c0 = run_cm()
+    assert len(ids(cm)) == 1
+    np.testing.assert_array_equal(hit(cm, run_cm, 3), c0)
+    cm.sigma_min *= 2                                      # another sigma grid -> another identity
+    c2 = run_cm()
+    assert len(ids(cm)) == 2 and np.abs(c2 - c0).max() > 1e-6
+
+    name = "edm_heun_mask_clip_dx"
+    edm, inp, kw, _ = build_edm(cases.edm_cases()[name])
+
+    def run_edm():
+        with NoiseTape(tape_of(golden["edm"], name)).active(), torch.no_grad():
+            return edm.sample(inp["prior"], **kw)[0].numpy()
+
+    e0 = run_edm()
+    assert len(ids(edm)) == 1
+    np.testing.assert_array_equal(hit(edm, run_edm, kw["sample_steps"]), e0)
+    edm.sigma_max *= 0.5
+    e2 = run_edm()
+    assert len(ids(edm)) == 2 and np.abs(e2 - e0).max() > 1e-6
 
 
 @pytest.mark.parametrize("name,math", [("disc_dup_ddpm_x0", "fp32"), ("cont_cfg2branch_2M", "fp32"), ("cont_ddim_eps", "bf16")])
