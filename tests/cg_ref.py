@@ -47,6 +47,102 @@ def gn_bwd(h, gamma, beta, dout, groups, eps, act=cabi.ACT_MISH):
     return (rstd * (dg - m1 - xg * m2)).reshape(B, L, C)
 
 
+# ---------------------------------------------------------------- error bounds of csrc/classifier.cuh (u = 2^-24)
+U32 = grad_ref.U32
+# A TF32 store rounds to nearest: at most half a TF32 unit, 2^-11 |ref|.  The bound allows a whole unit, R_TF32 |ref|, as it
+# does for the audit's other TF32 outputs (conv, LNMOD), so that a correctly rounded value of the exact result takes at most
+# half of it.  That leaves room for a store that truncates instead of rounding; the rounding mode itself is pinned elsewhere:
+# GN / GN_BWD store through f32_for_store (csrc/common.cuh), whose TF32 rounding every audited `update + x_cast -> tf32`
+# compares bit for bit with opref.tf32_round, and the TF32 outputs here must have their low 13 bits clear.
+R_TF32 = 2.0 ** -10
+MISH_LIP, MISH_GRAD_LIP = 1.1, 1.0          # max Mish' = 1.089, max |Mish''| = 0.644
+
+
+def _gmean(t, groups):
+    """per-element (B, L, C) view of the (trajectory, group) mean of t"""
+    B, L, C = t.shape
+    return t.reshape(B, L, groups, C // groups).mean(dim=(1, 3), keepdim=True).expand(B, L, groups, C // groups).reshape(B, L, C)
+
+
+def _xhat_error(h, groups, eps):
+    """(xhat, rstd, k, e_x) in fp64.  One warp owns the n = L C / groups elements of a (trajectory, group): each lane sums
+    about ceil(n/32) of them in order, then a 5-level butterfly, so k = ceil(n/32) + 5 is the summation depth.
+      mean m:  |m - mean| <= (k + 1) u mean|h|  (k adds and the division by n)
+      rstd:    the centred squares are positive, so their sum has relative error <= k u; each d = h - m rounds once (2 u on
+               d^2); m enters the variance only to second order (sum (h - mean) = 0); with / n, + eps, sqrtf and 1 / x the
+               relative error of rstd is at most (k/2 + 4) u
+      xhat = (h - m) rstd:  e_x = rstd (k + 1) u mean|h| + (k/2 + 6) u |xhat|  (the subtraction and the product add 2 u)"""
+    B, L, C = h.shape
+    g, mean, rstd = _stats(h, groups, eps)
+    k = -(-(L * C // groups) // 32) + 5
+    xhat = ((g - mean) * rstd).reshape(B, L, C)
+    rstd = rstd.expand(B, L, groups, C // groups).reshape(B, L, C)
+    e_x = rstd * (k + 1) * U32 * _gmean(h.to(F64).abs(), groups) + (k / 2 + 6) * U32 * xhat.abs()
+    return xhat, rstd, k, e_x
+
+
+def _store_term(ref, dtype):
+    return R_TF32 * ref.abs() if dtype == cabi.TF32 else 0.0
+
+
+def gn_bound(h, gamma, beta, groups, eps, ref, act=cabi.ACT_MISH, vec=None, res=None, out_dtype=cabi.F32):
+    """Per-element bound on |CDS_OP_GN - gn(...)| (gn_kernel; ``ref`` = gn(...) in fp64).  From the xhat error e_x of
+    ``_xhat_error``:
+      z = fmaf(xhat, gamma, beta):  e_z = |gamma| e_x + u |z|
+      y = Mish(z):  MISH_LIP e_z (Mish is 1.1-Lipschitz) + grad_ref.mish_bound(z) (the fp32 evaluation)
+      + vec, + res:  one rounding per add, 2 u (|y| + |vec|) and 2 u (|y| + |vec| + |res|): twice the rounding, so that
+                     a store's rounding of the exact result is at most half of its term, as for R_TF32
+      TF32 store:  R_TF32 |ref|"""
+    xhat, _, _, e_x = _xhat_error(h, groups, eps)
+    ga = gamma.to(F64)
+    z = xhat * ga + beta.to(F64)
+    e = ga.abs() * e_x + U32 * z.abs()
+    if act == cabi.ACT_MISH:
+        e = MISH_LIP * e + grad_ref.mish_bound(z)
+    mag = opref.act(act, z).abs()
+    if vec is not None:
+        v = vec.to(F64).abs()
+        mag = mag + (v[None, None] if v.dim() == 1 else v[:, None])
+        e = e + 2 * U32 * mag
+    if res is not None:
+        mag = mag + res.to(F64).abs()
+        e = e + 2 * U32 * mag
+    return e + _store_term(ref, out_dtype)
+
+
+def gn_bwd_bound(h, gamma, beta, dout, groups, eps, ref, act=cabi.ACT_MISH, dh_dtype=cabi.F32):
+    """Per-element bound on |CDS_OP_GN_BWD - gn_bwd(...)| (gn_bwd_kernel; ``ref`` = gn_bwd(...) in fp64).  dh = rstd (d - m1 -
+    xhat m2) cancels, so the bound is relative to rstd (|d| + mean|d| + |xhat| mean|d xhat|), not to dh.  From e_x of
+    ``_xhat_error`` and e_z = |gamma| e_x + u |z|:
+      d = gamma dout Mish'(z):  e_d = |gamma dout| (grad_ref.mish_grad_bound(z) + MISH_GRAD_LIP e_z) + 2 u |d|
+      m1 = mean d:              e_m1 = (k + 1) u mean|d| + mean e_d
+      m2 = mean d xhat (fmaf):  e_m2 = (k + 1) u mean|d xhat| + mean(e_d |xhat| + |d| e_x)
+      dh:  rstd (e_d + e_m1 + |xhat| e_m2 + |m2| e_x + 3 u (|d| + |m1| + |xhat m2|)) + (k/2 + 5) u |dh| (rstd's relative
+           error and the final product), + R_TF32 |ref| for a TF32 store"""
+    xhat, rstd, k, e_x = _xhat_error(h, groups, eps)
+    ga = gamma.to(F64)
+    z = xhat * ga + beta.to(F64)
+    d = gd = ga * dout.to(F64)
+    e_d = 0.0
+    if act == cabi.ACT_MISH:
+        d = gd * torch.from_numpy(grad_ref.mish_grad(z.cpu().numpy())).to(gd.device)
+        e_d = gd.abs() * (grad_ref.mish_grad_bound(z) + MISH_GRAD_LIP * (ga.abs() * e_x + U32 * z.abs()))
+    e_d = e_d + 2 * U32 * d.abs()
+    m1, m2 = _gmean(d, groups), _gmean(d * xhat, groups)
+    e_m1 = (k + 1) * U32 * _gmean(d.abs(), groups) + _gmean(e_d, groups)
+    e_m2 = (k + 1) * U32 * _gmean((d * xhat).abs(), groups) + _gmean(e_d * xhat.abs() + d.abs() * e_x, groups)
+    e = rstd * (e_d + e_m1 + xhat.abs() * e_m2 + m2.abs() * e_x + 3 * U32 * (d.abs() + m1.abs() + (xhat * m2).abs()))
+    return e + (k / 2 + 5) * U32 * ref.abs() + _store_term(ref, dh_dtype)
+
+
+# the classifiers of the reference's guided pipelines (diffuser / adaptdiffuser / veteran on D4RL): HalfJannerUNet1d keyword
+# arguments, and the observation part of x (the rest is the action)
+PIPELINES = {"hopper": dict(horizon=32, in_dim=14), "walker": dict(horizon=32, in_dim=23),
+             "halfcheetah": dict(horizon=4, in_dim=23, dim_mult=(1, 4, 2)), "antmaze": dict(horizon=64, in_dim=37),
+             "kitchen": dict(horizon=32, in_dim=69)}
+OBS_DIM = {"hopper": 11, "walker": 17, "halfcheetah": 17, "antmaze": 29, "kitchen": 60}
+
+
 # ---------------------------------------------------------------- descriptor interpreters (memory backends of tests/emulator.py)
 def run_gn(g, it, mem):
     v = emulator.view

@@ -89,6 +89,68 @@ def wgrad(dz, h, act_kind=cabi.ACT_NONE):
     return dz.T @ act(act_kind, h), dz.sum(0)
 
 
+# ---------------------------------------------------------------- error bounds of the fp32 kernels (csrc/grad.cuh), u = 2^-24
+# Each takes fp64 numpy arrays (or torch tensors where it only uses abs and arithmetic) and returns the per-element bound on
+# |kernel - fp64 reference|.  The operator tests (tests/test_grad_sampling_gpu.py) and the program audit
+# (tests/program_audit.py) both apply them.
+U32 = 2.0 ** -24
+
+
+def mish_bound(z):
+    """fp32 Mish(z) = z tanh(log1pf(expf(z))): expf, log1pf and tanhf are within 2 ulp (4 u relative) each; the relative error
+    of e^z passes at most once through log1p (log1p(y) >= y / (1 + y)) and through tanh ((1 - t^2) s / t <= 1), so with the
+    product Mish's relative error is at most 11 u, and |Mish(z)| <= |z|: 12 u (1 + |z|) also covers the softplus threshold at
+    z = 20 and values near 0."""
+    return 12 * U32 * (1 + abs(z))
+
+
+def mish_grad_bound(z):
+    """fp32 Mish'(z): tanh(softplus(z)) and 1 - tanh^2 carry absolute errors of a few u, scaled by |z| through z sigmoid(z)"""
+    return (8 + 8 * abs(z)) * U32
+
+
+def update_bwd_bound(g, alpha, sigma, k0, k1):
+    """CDS_OP_UPDATE_BWD: a handful of fp32 operations per element, each within u of its exact result, on terms of size at
+    most |g| (|k0| + |k1|) (1 + 1/alpha + 1/sigma)^2; 16 u of that (the clip decisions are exact: grad_ref.update_bwd takes
+    them in fp32 like the kernel)"""
+    return 16 * U32 * np.abs(np.asarray(g, np.float64)) * (abs(k0) + abs(k1)) * (1 + 1 / alpha + 1 / sigma) ** 2
+
+
+def dgrad_bound(dz, w, z=None, act_kind=cabi.ACT_NONE, before=None):
+    """CDS_OP_DGRAD, out [+]= (dz W) Mish'(z): each output is one thread's fma chain over N, so the dot-product bound
+    (N + 4) u |dz||W|, times |Mish'(z)| when the derivative is fused; the fp32 Mish' adds |dz W| mish_grad_bound(z).  An
+    accumulating store (``before``: the output before the launch, for accumulate = 1 and for out_sum) adds 2 u (|before| + |y|)."""
+    dz, w = np.asarray(dz, np.float64), np.asarray(w, np.float64)
+    dzw = dz @ w
+    mag, y = np.abs(dz) @ np.abs(w), dzw
+    bound = 0.0
+    if act_kind == cabi.ACT_MISH:
+        z = np.asarray(z, np.float64)
+        mg = mish_grad(z)
+        mag, y = mag * np.abs(mg), dzw * mg
+        bound = np.abs(dzw) * mish_grad_bound(z)
+    bound = bound + (dz.shape[1] + 4) * U32 * mag
+    if before is not None:
+        bound = bound + 2 * U32 * (np.abs(np.asarray(before, np.float64)) + np.abs(y))
+    return bound
+
+
+def wgrad_bound(dz, h, act_kind=cabi.ACT_NONE, dw_before=None, db_before=None):
+    """CDS_OP_WGRAD -> (bound of dw (N, K), bound of db (N,)): each output sums the rows in order in one thread, so
+    (rows + 8) u |dz|^T |act(h)| (the fp32 activation's relative error included) and (rows + 2) u sum_rows |dz| for the bias
+    column; an accumulating store adds 2 u (|before| + |contribution|)."""
+    dz = np.asarray(dz, np.float64)
+    rows, adz = dz.shape[0], np.abs(dz)
+    gw, gb = wgrad(dz, h, act_kind)
+    bw = (rows + 8) * U32 * (adz.T @ np.abs(act(act_kind, h)))
+    bb = (rows + 2) * U32 * adz.sum(0)
+    if dw_before is not None:
+        bw = bw + 2 * U32 * (np.abs(np.asarray(dw_before, np.float64)) + np.abs(gw))
+    if db_before is not None:
+        bb = bb + 2 * U32 * (np.abs(np.asarray(db_before, np.float64)) + np.abs(gb))
+    return bw, bb
+
+
 # ---------------------------------------------------------------- descriptor interpreters (memory backends of tests/emulator.py)
 def _f32(v):
     return np.asarray(v, np.float64).astype(np.float32)
@@ -135,6 +197,37 @@ def run_wgrad(g, it, arr):
     if g.db:
         b = arr(g.db + 4 * it * g.db_iter_stride, (g.N,), (1,))
         b[...] = _f32(b.astype(np.float64) + db) if g.accumulate else _f32(db)
+
+
+# ---------------------------------------------------------------- differentiable calls audited operator by operator
+# (tests/test_program_audit_cpu.py, tests/test_program_audit_gpu.py), 5 steps each
+GRAD_CASES = {
+    # Diffusion-QL's call: discrete eps-prediction clipped to [-1, 1]
+    "dql-eps": dict(net=dict(obs_dim=17, act_dim=6, emb_dim=16), kind="discrete", predict_noise=True, solver="ddpm"),
+    # continuous x0-prediction with a fix_mask
+    "dql-x0": dict(net=dict(obs_dim=11, act_dim=3), kind="continuous", predict_noise=False, solver="sde_dpmsolver++_1"),
+}
+
+
+def grad_agent(case, device):
+    """(agent, sample() keyword arguments without the prior and the condition) of a GRAD_CASES case"""
+    from cleandiffuser_b200.diffusion import ContinuousDiffusionSDE, DiscreteDiffusionSDE
+    from cleandiffuser_b200.nn_condition import IdentityCondition
+    from cleandiffuser_b200.nn_diffusion import DQLMlp
+    from cleandiffuser_b200.testing import load_synth
+    import torch
+    spec = GRAD_CASES[case]
+    net = load_synth(DQLMlp(**spec["net"]), seed=1)
+    a = spec["net"]["act_dim"]
+    kw = dict(predict_noise=spec["predict_noise"], device=device)
+    if spec["kind"] == "discrete":
+        kw.update(x_max=torch.full((1, a), 1.0), x_min=torch.full((1, a), -1.0))
+        agent = DiscreteDiffusionSDE(net, IdentityCondition(dropout=0.0), diffusion_steps=5, **kw)
+    else:
+        mask = torch.zeros(a)
+        mask[0] = 1.
+        agent = ContinuousDiffusionSDE(net, IdentityCondition(dropout=0.0), fix_mask=mask, **kw)
+    return agent, dict(solver=spec["solver"], sample_steps=5, use_ema=False, w_cfg=1.0, requires_grad=True)
 
 
 # ---------------------------------------------------------------- programs with backward operators

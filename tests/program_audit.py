@@ -8,8 +8,10 @@ every operand's extent checked against its owner), on the device for a real plan
 checks:
   - its output against tests/opref.py in fp64, computed from the same state before the launch, under the derived bound of
     the operator's kernel family: conv_cases.check (+ gn_offset_atol for GroupNorm on tensor cores), attn_cases.bound,
-    mha_cases.bound, the LNMOD bound of tests/test_elementwise_gpu.py; UPDATE / PREP / CAST bit for bit against the
-    interpreter run on host copies of their operands;
+    mha_cases.bound, the LNMOD bound of tests/test_elementwise_gpu.py; UPDATE / PREP / CAST / GUIDE and STASH's slot
+    copy bit for bit against the interpreter run on host copies of their operands; GN / GN_BWD under cg_ref.gn_bound /
+    gn_bwd_bound, STASH's Mish under grad_ref.mish_bound, UPDATE_BWD / DGRAD / WGRAD under grad_ref.update_bwd_bound /
+    dgrad_bound / wgrad_bound (accumulating outputs as before + contribution), the bounds the operator tests apply;
   - that nothing outside its declared outputs changed: every other owner keeps its fingerprint, and inside the owner of an
     output view the elements outside the view keep theirs.
 The largest error as a fraction of the bound is recorded per (program, kernel instantiation).
@@ -17,11 +19,14 @@ Never imported by the product.
 """
 import math
 
+import numpy as np
 import torch
 
 import attn_cases
+import cg_ref
 import conv_cases
 import emulator
+import grad_ref
 import mha_cases
 import mha_ref
 import opref
@@ -34,19 +39,49 @@ CHUNK = 1 << 24                                 # output elements per fp64 refer
 PARK = 1 << 30                                  # fp64 references kept across a launch wait in host memory above this size
 DT_NAME = {cabi.F32: "f32", cabi.TF32: "tf32", cabi.BF16: "bf16"}
 KIND_NAME = {cabi.OP_CONV: "conv", cabi.OP_UPDATE: "update", cabi.OP_LNMOD: "lnmod", cabi.OP_ATTN: "attn",
-             cabi.OP_PREP: "prep", cabi.OP_CAST: "cast", cabi.OP_MHA: "mha"}
+             cabi.OP_PREP: "prep", cabi.OP_CAST: "cast", cabi.OP_MHA: "mha", cabi.OP_STASH: "stash",
+             cabi.OP_UPDATE_BWD: "update_bwd", cabi.OP_DGRAD: "dgrad", cabi.OP_WGRAD: "wgrad", cabi.OP_GN: "gn",
+             cabi.OP_GN_BWD: "gn_bwd", cabi.OP_GUIDE: "guide"}
 
 
 def plan_owners(plan):
     """the tensors a SamplerPlan's descriptors may point into: every kept buffer and packed weight copy of the root program
-    (which holds the branch programs' as well), and the network's parameters and buffers"""
-    keep = [t for t in plan.program.keep if isinstance(t, torch.Tensor)]
-    return keep + list(plan.net.parameters()) + list(plan.net.buffers())
+    (which holds the branch programs' as well) and of a GradSamplerPlan's backward program, and the parameters and buffers
+    of the network and of a lowered classifier"""
+    progs = [plan.program] + ([plan.back] if getattr(plan, "back", None) is not None else [])
+    keep = [t for p in progs for t in p.keep if isinstance(t, torch.Tensor)]
+    nets = [plan.net] + ([plan.classifier.model_ema] if getattr(plan, "classifier", None) is not None else [])
+    return keep + [t for n in nets for t in (*n.parameters(), *n.buffers())]
 
 
-def declared_outputs(op):
-    """(ptr, shape, strides, dtype) of every view operator ``op`` may write"""
+def declared_outputs(op, it):
+    """(ptr, shape, strides, dtype) of every view operator ``op`` may write at iteration ``it`` (a stash slot and WGRAD's
+    bias row move with the iteration)"""
     k = op.kind
+    if k == cabi.OP_STASH:
+        s = op.u.stash
+        outs = [(s.dst + 4 * it * s.dst_iter_stride, (s.n,), (1,), cabi.F32)]
+        return outs + ([(s.act_out, (s.n,), (1,), cabi.F32)] if s.act_out else [])
+    if k == cabi.OP_UPDATE_BWD:
+        u = op.u.update_bwd
+        return [(p, (u.batch, u.row), (u.row, 1), cabi.F32) for p in (u.gx, u.gpred)]
+    if k == cabi.OP_DGRAD:
+        d = op.u.dgrad
+        outs = [(d.out, (d.rows, d.K), (d.ldo, 1), cabi.F32)]
+        return outs + ([(d.out_sum, (d.rows, d.K), (d.K, 1), cabi.F32)] if d.out_sum else [])
+    if k == cabi.OP_WGRAD:
+        g = op.u.wgrad
+        outs = [(g.dw, (g.N, g.K), (g.lddw, 1), cabi.F32)]
+        return outs + ([(g.db + 4 * it * g.db_iter_stride, (g.N,), (1,), cabi.F32)] if g.db else [])
+    if k == cabi.OP_GN:
+        g = op.u.gn
+        return [(g.out, (g.batch, g.L, g.C), (g.out_bstride, g.out_lstride, 1), g.out_dtype)]
+    if k == cabi.OP_GN_BWD:
+        g = op.u.gn_bwd
+        return [(g.dh, (g.batch, g.L, g.C), (g.dh_bstride, g.dh_lstride, 1), g.dh_dtype)]
+    if k == cabi.OP_GUIDE:
+        q = op.u.guide
+        return [(q.pred, (q.batch, q.L, q.C), (q.L * q.C, q.C, 1), cabi.F32)]
     if k == cabi.OP_CONV:
         c = op.u.conv
         return [(c.out, (c.batch, c.L_out * c.phases, c.C_out), (c.out_bstride, c.out_lstride, 1), c.out_dtype)]
@@ -93,6 +128,24 @@ def instantiation(op):
         return f"cast {'once ' if op.flags & cabi.OPF_ONCE else ''}-> {DT_NAME[op.u.cast.out_dtype]}"
     if op.kind == cabi.OP_UPDATE and op.u.update.x_cast:
         return f"update + x_cast -> {DT_NAME[op.u.update.x_cast_dtype]}"
+    if op.kind == cabi.OP_GN:
+        g = op.u.gn
+        return f"gn{' +vec' if g.vec.step or g.vec.sample else ''}{' +res' if g.res else ''} -> {DT_NAME[g.out_dtype]}"
+    if op.kind == cabi.OP_GN_BWD:
+        return f"gn_bwd -> {DT_NAME[op.u.gn_bwd.dh_dtype]}"
+    if op.kind == cabi.OP_STASH:
+        return "stash +act" if op.u.stash.act_out else "stash"
+    if op.kind == cabi.OP_UPDATE_BWD:
+        u = op.u.update_bwd
+        return f"update_bwd {'eps' if u.predict_noise else 'x0'}{' clip' if u.x_min or u.x_max else ''}" \
+            f"{' mask' if u.mask else ''}"
+    if op.kind == cabi.OP_DGRAD:
+        d = op.u.dgrad
+        return f"dgrad{' mish' if d.act == cabi.ACT_MISH else ''}{' +=' if d.accumulate else ''}" \
+            f"{' +out_sum' if d.out_sum else ''}"
+    if op.kind == cabi.OP_WGRAD:
+        g = op.u.wgrad
+        return f"wgrad{' mish' if g.act == cabi.ACT_MISH else ''}{' +bias' if g.db else ''}"
     return KIND_NAME[op.kind]
 
 
@@ -144,26 +197,26 @@ class Auditor:
         if not frac <= 1.0:
             self.failures.append(f"{self.name} {where} [{inst}]: {frac:.3g} of the bound")
 
-    def _views(self, op):
-        return [emulator.view(self.mem, *o) for o in declared_outputs(op)]
+    def _views(self, op, it):
+        return [emulator.view(self.mem, *o) for o in declared_outputs(op, it)]
 
     def _fingerprints(self):
         """per owner, the sum of its bit patterns: any single changed element changes it"""
         return torch.stack([_bits(t).sum(dtype=torch.int64) for t in self.mem.owners]).tolist()
 
-    def _sums(self, ops):
-        """(owner index, sum of the bit patterns) of every declared output view of ``ops``"""
-        outs = [o for op in ops for o in declared_outputs(op)]
+    def _sums(self, ops, it):
+        """(owner index, sum of the bit patterns) of every declared output view of ``ops`` at iteration ``it``"""
+        outs = [o for op in ops for o in declared_outputs(op, it)]
         if not outs:
             return []
         owners = [self.mem.owner(o[0], (2 if o[3] == cabi.BF16 else 4) * emulator._span(o[1], o[2])) for o in outs]
         sums = torch.stack([_bits(emulator.view(self.mem, *o)).sum(dtype=torch.int64) for o in outs]).tolist()
         return list(zip(owners, sums))
 
-    def _stray_writes(self, before, ops, sums_before, where):
+    def _stray_writes(self, before, ops, it, sums_before, where):
         """every owner but the outputs' keeps its fingerprint; inside an output's owner, only the view changed: the owner's
         fingerprint minus its views' sums is the same before and after (the sums are exact int64 arithmetic)"""
-        after, sums_after = self._fingerprints(), self._sums(ops)
+        after, sums_after = self._fingerprints(), self._sums(ops, it)
         outside_before, outside_after = list(before), list(after)
         for (k, sb), (_, sa) in zip(sums_before, sums_after):
             outside_before[k] -= sb
@@ -283,15 +336,18 @@ class Auditor:
         return check
 
     def _exact(self, op, it):
-        """UPDATE / PREP / CAST: the interpreter on host copies of the operands; the kernel must give the same bits"""
+        """UPDATE / PREP / CAST / GUIDE: the interpreter on host copies of the operands; the kernel must give the same bits
+        (GUIDE: cg_ref.run_guide is the kernel's fp32 multiply, then fp32 add)"""
         host = emulator.Owned(self.mem.owners, host=True)
         if op.kind == cabi.OP_UPDATE:
             emulator.run_update(op.u.update, it, host)
         elif op.kind == cabi.OP_PREP:
             emulator.run_prep(op.u.prep, it, host)
+        elif op.kind == cabi.OP_GUIDE:
+            cg_ref.run_guide(op.u.guide, it, host)
         else:
             emulator.run_cast(op.u.cast, host)
-        outs = declared_outputs(op)
+        outs = declared_outputs(op, it)
         want = [emulator.view(host, *o) for o in outs]
 
         def check():
@@ -299,6 +355,107 @@ class Auditor:
             return [(0.0 if same_bits(g.cpu(), w) else math.inf, f"output {j} bit for bit")
                     for j, (g, w) in enumerate(zip(got, want))]
         return check
+
+    # ---- classifier guidance (cg_ref) and the backward operators of a differentiable loop (grad_ref) -------------------
+    def _bounded(self, outs, refs):
+        """check() of the declared outputs ``outs`` against [(fp64 reference, bound)] (torch on any device, or numpy); a TF32
+        output must also have the low 13 bits of every element clear"""
+        def check():
+            res = []
+            for j, (o, (ref, bound)) in enumerate(zip(outs, refs)):
+                ref = torch.as_tensor(ref, dtype=F64)
+                y = emulator.view(self.mem, *o).float().to(ref.device)
+                err = (y.to(F64) - ref).abs()
+                frac = _frac(err, torch.as_tensor(bound, dtype=F64, device=ref.device).expand_as(err),
+                             bool(torch.isfinite(y).all()))
+                if o[3] == cabi.TF32 and int((y.contiguous().view(torch.int32) & 0x1FFF).abs().max()) != 0:
+                    frac = math.inf
+                res.append((frac, f"output {j}"))
+            return res
+        return check
+
+    def _host_arr(self):
+        """numpy float32 views (ptr, shape, strides) of host copies of the owners, for grad_ref's numpy references"""
+        host = emulator.Owned(self.mem.owners, host=True)
+        return lambda ptr, shape, strides: emulator._arr(ptr, shape, strides, host)
+
+    def _gn(self, op, it):
+        g = op.u.gn
+        v = emulator.view
+        h = v(self.mem, g.h, (g.batch, g.L, g.C), (g.h_bstride, g.h_lstride, 1), cabi.F32)
+        gamma, beta = v(self.mem, g.gamma, (g.C,), (1,), cabi.F32), v(self.mem, g.beta, (g.C,), (1,), cabi.F32)
+        vec = emulator.vec(g.vec, it, g.batch, g.C, 1, self.mem)
+        res = v(self.mem, g.res, (g.batch, g.L, g.C), (g.res_bstride, g.res_lstride, 1), cabi.F32) if g.res else None
+        ref = cg_ref.gn(h, gamma, beta, g.groups, g.eps, g.act, vec, res)
+        bound = cg_ref.gn_bound(h, gamma, beta, g.groups, g.eps, ref, g.act, vec, res, g.out_dtype)
+        return self._bounded(declared_outputs(op, it), [(ref, bound)])
+
+    def _gn_bwd(self, op, it):
+        g = op.u.gn_bwd
+        v = emulator.view
+        h = v(self.mem, g.h, (g.batch, g.L, g.C), (g.h_bstride, g.h_lstride, 1), cabi.F32)
+        gamma, beta = v(self.mem, g.gamma, (g.C,), (1,), cabi.F32), v(self.mem, g.beta, (g.C,), (1,), cabi.F32)
+        dout = v(self.mem, g.dout, (g.batch, g.L, g.C), (g.dout_bstride, g.dout_lstride, 1), cabi.F32)
+        ref = cg_ref.gn_bwd(h, gamma, beta, dout, g.groups, g.eps, g.act)
+        bound = cg_ref.gn_bwd_bound(h, gamma, beta, dout, g.groups, g.eps, ref, g.act, g.dh_dtype)
+        return self._bounded(declared_outputs(op, it), [(ref, bound)])
+
+    def _stash(self, op, it):
+        """the slot copy bit for bit; the Mish of the pre-activation under grad_ref.mish_bound"""
+        s = op.u.stash
+        arr = self._host_arr()
+        src = arr(s.src, (s.n,), (1,)).copy()
+        outs = declared_outputs(op, it)
+        refs = []
+        if s.act_out:
+            assert s.act == cabi.ACT_MISH, s.act
+            refs = [(grad_ref.mish(src), grad_ref.mish_bound(src.astype(np.float64)))]
+        bounded = self._bounded(outs[1:], refs)
+
+        def check():
+            got = emulator.view(self.mem, *outs[0]).cpu()
+            return [(0.0 if same_bits(got, torch.from_numpy(src)) else math.inf, "slot bit for bit")] + bounded()
+        return check
+
+    def _update_bwd(self, op, it):
+        u = op.u.update_bwd
+        arr = self._host_arr()
+        row = arr(u.coef + 4 * it * u.coef_iter_stride, (cabi.ROW_FLOATS,), (1,)).astype(np.float64)
+        shape, st = (u.batch, u.row), (u.row, 1)
+        gx = arr(u.gx, shape, st).copy()
+        x, pr = arr(u.x + 4 * it * u.x_iter_stride, shape, st), arr(u.pred + 4 * it * u.pred_iter_stride, shape, st)
+        vec = lambda p: None if not p else arr(p, (u.row,), (1,))          # noqa: E731
+        alpha, sigma, k0, k1 = row[0], row[1], row[2], row[3]
+        gp, dx = grad_ref.update_bwd(gx, x, pr, alpha=alpha, sigma=sigma, k0=k0, k1=k1, kind=int(row[7]),
+                                     predict_noise=bool(u.predict_noise), mask=vec(u.mask), x_min=vec(u.x_min),
+                                     x_max=vec(u.x_max))
+        bound = grad_ref.update_bwd_bound(gx, alpha, sigma, k0, k1)
+        return self._bounded(declared_outputs(op, it), [(dx, bound), (gp, bound)])
+
+    def _dgrad(self, op, it):
+        d = op.u.dgrad
+        arr = self._host_arr()
+        dz, w = arr(d.dz, (d.rows, d.N), (d.ldz, 1)), arr(d.w, (d.N, d.K), (d.ldw, 1))
+        z = arr(d.z + 4 * it * d.z_iter_stride, (d.rows, d.K), (d.K, 1)) if d.z else None
+        y = grad_ref.dgrad(dz, w, z, d.act)
+        before = arr(d.out, (d.rows, d.K), (d.ldo, 1)).astype(np.float64) if d.accumulate else None
+        refs = [(y if before is None else before + y, grad_ref.dgrad_bound(dz, w, z, d.act, before))]
+        if d.out_sum:
+            s0 = arr(d.out_sum, (d.rows, d.K), (d.K, 1)).astype(np.float64)
+            refs.append((s0 + y, grad_ref.dgrad_bound(dz, w, z, d.act, s0)))
+        return self._bounded(declared_outputs(op, it), refs)
+
+    def _wgrad(self, op, it):
+        g = op.u.wgrad
+        arr = self._host_arr()
+        dz = arr(g.dz, (g.rows, g.N), (g.ldz, 1))
+        h = arr(g.h + 4 * it * g.h_iter_stride, (g.rows, g.K), (g.ldh, 1))
+        gw, gb = grad_ref.wgrad(dz, h, g.act)
+        w0 = arr(g.dw, (g.N, g.K), (g.lddw, 1)).astype(np.float64) if g.accumulate else None
+        b0 = arr(g.db + 4 * it * g.db_iter_stride, (g.N,), (1,)).astype(np.float64) if g.db and g.accumulate else None
+        bw, bb = grad_ref.wgrad_bound(dz, h, g.act, w0, b0)
+        refs = [(gw if w0 is None else w0 + gw, bw)] + ([(gb if b0 is None else b0 + gb, bb)] if g.db else [])
+        return self._bounded(declared_outputs(op, it), refs)
 
     def reference(self, op, it):
         if op.kind == cabi.OP_CONV:
@@ -309,6 +466,10 @@ class Auditor:
             return self._attn(op.u.attn)
         if op.kind == cabi.OP_MHA:
             return self._mha(op.u.mha, it)
+        special = {cabi.OP_GN: self._gn, cabi.OP_GN_BWD: self._gn_bwd, cabi.OP_STASH: self._stash,
+                   cabi.OP_UPDATE_BWD: self._update_bwd, cabi.OP_DGRAD: self._dgrad, cabi.OP_WGRAD: self._wgrad}
+        if op.kind in special:
+            return special[op.kind](op, it)
         return self._exact(op, it)
 
     # ---- the audit -------------------------------------------------------------------------------------------------------
@@ -322,13 +483,13 @@ class Auditor:
         if not once:
             return
         checks = [self.reference(op, first) for op in once]
-        before, sums = self._fingerprints(), self._sums(once)
+        before, sums = self._fingerprints(), self._sums(once, first)
         self.handle.run(first, 0, self.stream, False)
         self.sync()
         for op, chk in zip(once, checks):
             for frac, label in chk():
                 self._record(instantiation(op), frac, f"once op: {label}")
-        self._stray_writes(before, once, sums, "once ops")
+        self._stray_writes(before, once, first, sums, "once ops")
 
     def audit_iteration(self, it):
         """every operator of iteration ``it`` alone; leaves the state of the iteration's end"""
@@ -338,20 +499,21 @@ class Auditor:
                 continue
             where = f"it {it} op {i} ({KIND_NAME[op.kind]})"
             check = self.reference(op, it)
-            sums = self._sums([op])
+            sums = self._sums([op], it)
             self._launch(it, i, 1)
             for frac, label in check():
                 self._record(instantiation(op), frac, f"{where} {label}")
-            fp = self._stray_writes(fp, [op], sums, where)
+            fp = self._stray_writes(fp, [op], it, sums, where)
 
 
 # ---- whole iterations -------------------------------------------------------------------------------------------------
-def written_owners(mem, ops):
-    """indices of the owners some operator of ``ops`` writes"""
+def written_owners(mem, ops, its):
+    """indices of the owners some operator of ``ops`` writes in an iteration of ``its``"""
     idx = set()
-    for op in ops:
-        for ptr, shape, strides, dt in declared_outputs(op):
-            idx.add(mem.owner(ptr, (2 if dt == cabi.BF16 else 4) * emulator._span(shape, strides)))
+    for it in its:
+        for op in ops:
+            for ptr, shape, strides, dt in declared_outputs(op, it):
+                idx.add(mem.owner(ptr, (2 if dt == cabi.BF16 else 4) * emulator._span(shape, strides)))
     return sorted(idx)
 
 
@@ -384,3 +546,32 @@ def report_lines(worst):
     for (prog, inst), (frac, where) in sorted(worst.items()):
         lines.append(f"{prog:<14} {inst:<48} {frac:>7.3f}  {where}")
     return lines
+
+
+# ---- differentiable plans ---------------------------------------------------------------------------------------------
+def seed_backward(plan, seed):
+    """the state GradSamplerPlan.backward starts from: a seeded d x0 in ``gx`` and the accumulators zeroed"""
+    g = plan.grad
+    with torch.no_grad():
+        for t in g.accumulators:
+            t.zero_()
+        gen = torch.Generator().manual_seed(seed)
+        g.gx.copy_(torch.randn(g.gx.shape, generator=gen))
+
+
+def audit_grad_plan(name, plan, fwd, back, stream=0, sync=lambda: None, seed=3):
+    """(forward auditor, backward auditor) of a GradSamplerPlan: every operator of every iteration of the forward program
+    from the current x_t (run by ``fwd``), then of every iteration of the backward program (run by ``back``) from
+    seed_backward.  Every iteration: backward iteration m reads the stash slots of forward iteration n_iters - 1 - m, and
+    only the middle one of an odd count reads its own."""
+    owners = plan_owners(plan)
+    fa = Auditor(f"{name} fwd", plan.program.ops, fwd, owners, stream, sync)
+    fa.audit_once(0)
+    for it in range(plan.n_iters):
+        fa.audit_iteration(it)
+    seed_backward(plan, seed)
+    sync()
+    ba = Auditor(f"{name} bwd", plan.back.ops, back, owners, stream, sync)
+    for it in range(plan.n_iters):
+        ba.audit_iteration(it)
+    return fa, ba

@@ -74,12 +74,7 @@ def test_dgrad_wgrad_operators(rows, dims, layer):
     _run(op)
     zz = z[1].double().numpy()
     y = grad_ref.dgrad(dz.numpy(), w.numpy(), zz, act)
-    mg = np.abs(grad_ref.mish_grad(zz)) if mish else 1.0
-    mag = (np.abs(dz.double().numpy()) @ np.abs(w.double().numpy())) * mg
-    # fp32 Mish derivative: tanh(softplus(z)) and 1 - tanh^2 carry absolute errors of a few u, scaled by |z| through z sigmoid(z)
-    mg_err = (8 + 8 * np.abs(zz)) * U32 if mish else 0.0
-    bound = (N + 4) * U32 * mag + np.abs(dz.double().numpy() @ w.double().numpy()) * mg_err + \
-        2 * U32 * (np.abs(prev.double().numpy()) + np.abs(y)) + 1e-30
+    bound = grad_ref.dgrad_bound(dz.numpy(), w.numpy(), zz, act, before=prev.double().numpy()) + 1e-30
     for got in (d_out, d_sum):
         err = np.abs(got.cpu().double().numpy() - (prev.double().numpy() + y))
         _record(f"dgrad {layer}", (err / bound).max())
@@ -95,10 +90,8 @@ def test_dgrad_wgrad_operators(rows, dims, layer):
     q.dw, q.lddw, q.db, q.db_iter_stride, q.accumulate = d_dw.data_ptr(), K, d_db.data_ptr() + 4 * N, -N, 1
     _run(op)
     gw, gb = grad_ref.wgrad(dz.numpy(), zz, act)
-    hmag = np.abs(grad_ref.act(act, zz))
-    adz = np.abs(dz.double().numpy())
-    bw = (rows + 8) * U32 * (adz.T @ hmag) + 2 * U32 * (np.abs(dw0.double().numpy()) + np.abs(gw)) + 1e-30
-    bb = (rows + 2) * U32 * adz.sum(0) + 2 * U32 * (np.abs(db0[1].double().numpy()) + np.abs(gb)) + 1e-30
+    bw, bb = grad_ref.wgrad_bound(dz.numpy(), zz, act, dw0.double().numpy(), db0[1].double().numpy())
+    bw, bb = bw + 1e-30, bb + 1e-30
     _record(f"wgrad {layer}", (np.abs(d_dw.cpu().double().numpy() - (dw0.double().numpy() + gw)) / bw).max())
     _record(f"wgrad {layer} bias", (np.abs(d_db[1].cpu().double().numpy() - (db0[1].double().numpy() + gb)) / bb).max())
     assert torch.equal(d_db[0].cpu(), db0[0]), "wgrad wrote outside its iteration's bias row"
@@ -156,10 +149,7 @@ def test_update_bwd_operator(kind, predict_noise, bounds, act_dim):
     gp, dx = grad_ref.update_bwd(gx.numpy(), x.numpy(), pred.numpy(), alpha=r[0], sigma=r[1], k0=r[2], k1=r[3], kind=kind,
                                  predict_noise=predict_noise, mask=mask.numpy(),
                                  x_min=None if x_min is None else x_min.numpy(), x_max=None if x_max is None else x_max.numpy())
-    # a handful of fp32 operations per element, each within u of its exact result; the terms are at most |g| (|k0| + |k1|)
-    # (1 + 1/alpha + 1/sigma)^2 in size
-    scale = np.abs(gx.double().numpy()) * (abs(r[2]) + abs(r[3])) * (1 + 1 / r[0] + 1 / r[1]) ** 2
-    bound = 16 * U32 * scale + 1e-30
+    bound = grad_ref.update_bwd_bound(gx.numpy(), r[0], r[1], r[2], r[3]) + 1e-30
     _record("update_bwd d pred", (np.abs(dev["gp"].cpu().double().numpy() - gp) / bound).max())
     _record("update_bwd d x", (np.abs(dev["gx"].cpu().double().numpy() - dx) / bound).max())
 

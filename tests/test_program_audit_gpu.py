@@ -5,8 +5,10 @@ ChiTransformer kitchen shape (tests/golden/chi_cases.py) at batch 2048 as script
 bf16).  "dit256" adds cfg4 with a DiT1d of d_model 256 over x_t of 96 channels: the only audited program with 256-wide
 gated Linears (attention out-projection, second MLP Linear) and a 256-wide x_proj that reads x_t shared by the two CFG
 halves (in_batch_mod), i.e. conv_tc's gated and table epilogue lanes, each followed by a LayerNorm, at a width other than
-cfg4's 320.  Each is built by one ``sample()``, so that the plan, its tables and its per-call fills are what production builds; its
-handle is then driven directly.
+cfg4's 320.  "cg_<shape>" is scripts/cg_bench.py's classifier-guided call with the classifier of a reference pipeline
+(cg_ref.PIPELINES).  Each is built by one ``sample()``, so that the plan, its tables and its per-call fills are what
+production builds; its handle is then driven directly.  The differentiable programs of sample(requires_grad=True) over
+DQLMlp (grad_ref.GRAD_CASES) have their own test: all 5 forward and all 5 backward iterations.
 
 - Every operator of iterations 0, 1, the middle one (loops of 50 steps or more) and the last, reached by graph replay, is
   run alone and checked on every trajectory against fp64 under its kernel family's bound, and for writes outside its
@@ -24,19 +26,23 @@ import time
 import pytest
 import torch
 
+import cg_ref
 import chi_cases as cc
 import emulator
+import grad_ref
 import program_audit as pa
 from cleandiffuser_b200 import workloads
 from cleandiffuser_b200.diffusion import DDPM
+from cleandiffuser_b200.engine import cabi, runtime
 from cleandiffuser_b200.nn_condition import IdentityCondition
 from cleandiffuser_b200.nn_diffusion import ChiTransformer
-from cleandiffuser_b200.testing import synth_state_dict
+from cleandiffuser_b200.testing import load_synth, synth_state_dict
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
 PROGRAMS = ["cfg2-fp32", "cfg2-tf32", "cfg2-bf16", "cfg3-tf32", "cfg3-bf16", "cfg4-tf32", "cfg4-bf16", "cfg5-tf32",
-            "cfg5-bf16", "chi-tf32", "chi-bf16", "dit256-tf32"]
+            "cfg5-bf16", "chi-tf32", "chi-bf16", "dit256-tf32"] + \
+    [f"cg_{n}-tf32" for n in cg_ref.PIPELINES] + ["cg_hopper-fp32", "cg_halfcheetah-fp32"]
 CHI_BATCH, CHI_STEPS = 2048, 50
 WORST, COST = {}, {}
 
@@ -80,6 +86,8 @@ def _sample(name):
         return agent
     if name == "dit256":
         return _dit256()
+    if name.startswith("cg_"):
+        return _guided(name[3:])
     w = workloads.BUILDERS[name](DEV)
     with torch.no_grad():
         w.sample(DEV)
@@ -108,6 +116,34 @@ def _dit256(batch=2048, steps=20, w_cfg=6.0):
         agent.sample(prior.to(DEV), n_samples=batch, solver="ode_dpmsolver++_2M", sample_steps=steps,
                      sample_step_schedule="uniform_continuous", temperature=0.5, w_cfg=w_cfg, condition_cfg=cond.to(DEV))
     return agent
+
+
+def _guided(shape, batch=3200, steps=20, w_cg=0.3):
+    """scripts/cg_bench.py's guided call (DiscreteDiffusionSDE, JannerUNet1d denoiser, 20 DDPM steps, w_cg = 0.3) with the
+    classifier of a reference pipeline (cg_ref.PIPELINES); the horizon-4 halfcheetah denoiser halves twice, not three times"""
+    from cleandiffuser_b200.diffusion import DiscreteDiffusionSDE
+    from cleandiffuser_b200.nn_diffusion import JannerUNet1d
+    kw = cg_ref.PIPELINES[shape]
+    H, D, obs = kw["horizon"], kw["in_dim"], cg_ref.OBS_DIM[shape]
+    net = load_synth(JannerUNet1d(D, model_dim=32, emb_dim=32, kernel_size=5, dim_mult=[1, 4, 2] if H == 4 else [1, 2, 2, 2]),
+                     seed=0)
+    mask = torch.zeros(H, D)
+    mask[0, :obs] = 1.
+    agent = DiscreteDiffusionSDE(net, None, fix_mask=mask, predict_noise=True, diffusion_steps=steps, device=DEV,
+                                 classifier=cg_ref.make_classifier(kw, 31, DEV))
+    g = torch.Generator().manual_seed(1)
+    prior = torch.zeros(batch, H, D)
+    prior[:, 0, :obs] = torch.randn(batch, obs, generator=g)
+    agent.sample(prior.to(DEV), solver="ddpm", n_samples=batch, sample_steps=steps, use_ema=True, temperature=0.5, w_cg=w_cg)
+    assert runtime.STATS["guidance_path"] == "graph", runtime.STATS.get("guidance_reason")
+    return agent
+
+
+def _centre_tap_dgrad(op):
+    """the data gradient of a Downsample1d over a length-1 map: one 1x1 conv of its centre tap, no bias"""
+    c = op.u.conv
+    return op.kind == cabi.OP_CONV and c.taps == 1 and c.L_in == c.L_out == 1 and c.C_in == c.C_out and \
+        not (c.bias.step or c.bias.sample)
 
 
 def _build(prog, monkeypatch):
@@ -166,6 +202,8 @@ def test_every_operator_matches_fp64(prog, monkeypatch):
     assert not aud.failures, "\n".join(aud.failures[:20])
     # every launch of an iteration is one of the operators checked above, or the counter advance
     assert plan.handle.launches_per_iter() == pa.launches_per_iter(ops)
+    if prog.startswith("cg_halfcheetah"):       # horizon 4: the last Downsample's input has length 1
+        assert any(_centre_tap_dgrad(op) for op in ops)
 
 
 @pytest.mark.parametrize("prog", PROGRAMS)
@@ -176,7 +214,7 @@ def test_replay_gives_the_bits_of_operator_by_operator_runs(prog, monkeypatch):
     K = min(12, n - f)
     with _Cost(f"{prog} whole iterations {f}..{f + K - 1}"):
         mem = emulator.Owned(pa.plan_owners(plan))
-        written = [mem.owners[i] for i in pa.written_owners(mem, ops)]
+        written = [mem.owners[i] for i in pa.written_owners(mem, ops, range(f, f + K))]
         _start(plan)
         plan.handle.run(0, f, st, True)
         torch.cuda.synchronize()
@@ -233,3 +271,66 @@ def test_parallel_branches_give_the_operator_by_operator_bits(prog, branches, mo
             if k != "noise":
                 assert pa.same_bits(getattr(planb, k), want[k]), (k, "graph" if graph else "direct")
     assert math.isfinite(float(planb.x.abs().max()))
+
+
+GRAD_BATCH = {"dql-eps": 4096, "dql-x0": 256}
+
+
+def _grad_plan(case, math_mode, monkeypatch):
+    """a GradSamplerPlan after one sample(requires_grad=True) of grad_ref.GRAD_CASES[case] at its batch"""
+    monkeypatch.setenv("CDS_MATH", math_mode)
+    agent, kw = grad_ref.grad_agent(case, DEV)
+    B, spec = GRAD_BATCH[case], grad_ref.GRAD_CASES[case]
+    g = torch.Generator().manual_seed(B)
+    prior = torch.randn(B, spec["net"]["act_dim"], generator=g).to(DEV)
+    cond = torch.randn(B, spec["net"]["obs_dim"], generator=g).to(DEV)
+    agent.sample(prior, n_samples=B, condition_cfg=cond, **kw)
+    (plan,) = agent._engine_plans.values()
+    torch.cuda.synchronize()
+    assert isinstance(plan, runtime.GradSamplerPlan) and plan.n_iters == 5
+    return plan
+
+
+@pytest.mark.parametrize("case", list(grad_ref.GRAD_CASES))
+@pytest.mark.parametrize("math_mode", ["fp32", "tf32"])
+def test_differentiable_programs_match_fp64_and_replay_bits(case, math_mode, monkeypatch):
+    """Every operator of the 5 forward iterations and of the 5 backward iterations (from a seeded d x0, accumulators zeroed
+    as GradSamplerPlan.backward does) against fp64; then both programs' whole iterations give the same bits operator by
+    operator, by graph replay and by direct launches."""
+    plan = _grad_plan(case, math_mode, monkeypatch)
+    prog, st = f"{case}-{math_mode}", _stream()
+    with _Cost(f"{prog} per-operator audit (5 + 5 iterations)"):
+        _start(plan)
+        fa, ba = pa.audit_grad_plan(prog, plan, plan.handle, plan.back_handle, st, torch.cuda.synchronize)
+    for aud in (fa, ba):
+        for inst, (frac, where) in aud.worst.items():
+            WORST[(aud.name, inst)] = (frac, where)
+    assert not fa.failures and not ba.failures, "\n".join((fa.failures + ba.failures)[:20])
+    assert plan.handle.launches_per_iter() == pa.launches_per_iter(plan.program.ops)
+    assert plan.back_handle.launches_per_iter() == pa.launches_per_iter(plan.back.ops)
+
+    n = plan.n_iters
+    with _Cost(f"{prog} whole iterations, both programs"):
+        mem = emulator.Owned(pa.plan_owners(plan))
+        for ops, handle, first in ((plan.program.ops, plan.handle, None), (plan.back.ops, plan.back_handle, 0)):
+            written = [mem.owners[i] for i in pa.written_owners(mem, ops, range(n))]
+            if first is None:
+                _start(plan)
+            else:
+                pa.seed_backward(plan, 3)
+            torch.cuda.synchronize()
+            snap = [t.cpu() for t in written]
+            outs = None
+            for mode in ("op by op", "graph", "direct"):
+                for t, s in zip(written, snap):
+                    t.copy_(s)
+                if mode == "op by op":
+                    pa.run_op_by_op(handle, ops, 0, n, st, torch.cuda.synchronize)
+                else:
+                    handle.run(0, n, st, mode == "graph")
+                torch.cuda.synchronize()
+                if outs is None:
+                    outs = [t.cpu() for t in written]
+                    continue
+                diff = [f"{tuple(t.shape)}" for t, o in zip(written, outs) if not pa.same_bits(t.cpu(), o)]
+                assert not diff, f"{prog} {mode}: {len(diff)} buffers differ from the operator-by-operator run: {diff[:8]}"
