@@ -2,12 +2,14 @@
 
 Same surface as the reference's (cleandiffuser/classifier/base.py, rew_classifiers.py): ``model`` is trained, ``model_ema`` (an
 eval-mode copy updated by ``ema_update``) is what ``logp`` evaluates.  When a ``CumRewClassifier`` over ``HalfJannerUNet1d``
-guides ``sample()``, the engine evaluates the input gradient inside the replayed loop and ``gradients`` is not called.
+or a ``QGPOClassifier`` over ``QGPONNClassifier`` guides ``sample()``, the engine evaluates the input gradient inside the
+replayed loop and ``gradients`` is not called.
 """
 from copy import deepcopy
-from typing import Optional
+from typing import Dict, Optional
 
 import torch
+import torch.nn.functional as F
 
 
 class BaseClassifier:
@@ -20,6 +22,9 @@ class BaseClassifier:
         self.model = nn_classifier.to(device)
         self.model_ema = deepcopy(self.model).eval()
         self.optim = torch.optim.Adam(self.model.parameters(), **optim_params)
+        # bumped by every write to model_ema that moves no autograd version counter (ema_update writes through .data, load
+        # replaces the values): the engine folds it into the fingerprint of the weights it has packed copies of
+        self.weights_epoch = 0
 
     def eval(self):
         self.model.eval()
@@ -33,6 +38,7 @@ class BaseClassifier:
         with torch.no_grad():
             for p, p_ema in zip(self.model.parameters(), self.model_ema.parameters()):
                 p_ema.data.mul_(self.ema_rate).add_(p.data, alpha=1. - self.ema_rate)
+        self.weights_epoch += 1
 
     def loss(self, x: torch.Tensor, noise: torch.Tensor, y: torch.Tensor):
         raise NotImplementedError
@@ -68,6 +74,7 @@ class BaseClassifier:
         ckpt = torch.load(path, map_location=self.device)
         self.model.load_state_dict(ckpt["model"])
         self.model_ema.load_state_dict(ckpt["model_ema"])
+        self.weights_epoch += 1
 
 
 class CumRewClassifier(BaseClassifier):
@@ -89,3 +96,36 @@ class CumRewClassifier(BaseClassifier):
 
     def logp(self, x, noise, c=None):
         return self.model_ema(x, noise)
+
+
+class QGPOClassifier(BaseClassifier):
+    """QGPO's energy guidance f_phi (qgpo_classifier.py; https://arxiv.org/abs/2304.12824): ``logp = model_ema(x, t, obs)``,
+    trained with the in-support contrastive energy prediction loss over K support actions per observation."""
+
+    def loss(self, x: torch.Tensor, t: torch.Tensor, y: Dict[str, torch.Tensor]):
+        """x (batch, K, act_dim) noisy support actions, t (batch,), y = {"soft_label": (batch, K, 1) softmax of Q values,
+        "obs": (batch, obs_dim)} -> (loss, {f_max, f_mean, f_min})"""
+        b, k = x.shape[:2]
+        soft_label, obs = y["soft_label"], y["obs"]
+        f = self.model(x, t.unsqueeze(1).repeat(1, k), obs.unsqueeze(1).repeat(1, k, 1))
+        loss = -(soft_label * F.log_softmax(f, 1)).sum(1).mean()
+        with torch.no_grad():
+            f_max, f_mean, f_min = f.max(1)[0].mean().item(), f.mean().item(), f.min(1)[0].mean().item()
+        return loss, {"f_max": f_max, "f_mean": f_mean, "f_min": f_min}
+
+    def update(self, x: torch.Tensor, noise: torch.Tensor, y: Dict[str, torch.Tensor], update_ema: bool = True):
+        loss, log = self.loss(x, noise, y)
+        self.optim.zero_grad()
+        loss.backward()
+        grad_norm = None
+        if isinstance(self.grad_clip_norm, float):
+            grad_norm = torch.nn.utils.clip_grad_norm_(self.model.parameters(), self.grad_clip_norm).item()
+        self.optim.step()
+        if update_ema:
+            self.ema_update()
+        log.update({"loss": loss.item(), "grad_norm": grad_norm})
+        return log
+
+    def logp(self, x: torch.Tensor, t: torch.Tensor, c: torch.Tensor):
+        """x (batch, act_dim), t (batch,), c (batch, obs_dim) observations -> energy (batch, 1)"""
+        return self.model_ema(x, t, c)

@@ -211,8 +211,9 @@ int validate(const cds_op& op, Step* out) {
     }
     case CDS_OP_STASH: {
       const cds_stash_op& t = op.u.stash;
-      if (t.n <= 0 || !t.src || !t.dst) return fail(CDS_ERR_INVALID, "stash: bad arguments");
-      if (t.act_out && t.act != CDS_ACT_NONE && t.act != CDS_ACT_MISH) return fail(CDS_ERR_UNSUPPORTED, "stash: act %d", t.act);
+      if (t.n <= 0 || !t.src || (!t.dst && !t.act_out)) return fail(CDS_ERR_INVALID, "stash: bad arguments");
+      if (t.act_out && t.act != CDS_ACT_NONE && t.act != CDS_ACT_MISH && t.act != CDS_ACT_SILU)
+        return fail(CDS_ERR_UNSUPPORTED, "stash: act %d", t.act);
       return CDS_OK;
     }
     case CDS_OP_UPDATE_BWD: {
@@ -225,8 +226,9 @@ int validate(const cds_op& op, Step* out) {
       const cds_dgrad_op& d = op.u.dgrad;
       if (d.rows <= 0 || d.N <= 0 || d.K <= 0 || !d.dz || !d.w || !d.out || d.ldz < d.N || d.ldw < d.K || d.ldo < d.K)
         return fail(CDS_ERR_INVALID, "dgrad: bad arguments");
-      if (d.act != CDS_ACT_NONE && d.act != CDS_ACT_MISH) return fail(CDS_ERR_UNSUPPORTED, "dgrad: act %d", d.act);
-      if (d.act == CDS_ACT_MISH && !d.z) return fail(CDS_ERR_INVALID, "dgrad: Mish derivative without a pre-activation");
+      if (d.act != CDS_ACT_NONE && d.act != CDS_ACT_MISH && d.act != CDS_ACT_SILU)
+        return fail(CDS_ERR_UNSUPPORTED, "dgrad: act %d", d.act);
+      if (d.act != CDS_ACT_NONE && !d.z) return fail(CDS_ERR_INVALID, "dgrad: activation derivative without a pre-activation");
       return CDS_OK;
     }
     case CDS_OP_WGRAD: {
@@ -257,6 +259,13 @@ int validate(const cds_op& op, Step* out) {
       const cds_guide_op& g = op.u.guide;
       if (g.batch <= 0 || g.L <= 0 || g.C <= 0 || !g.pred || !g.g || !g.s || g.g_lstride < g.C)
         return fail(CDS_ERR_INVALID, "guide: bad arguments");
+      return CDS_OK;
+    }
+    case CDS_OP_HEAD_GRAD: {
+      const cds_head_grad_op& q = op.u.head_grad;
+      if (q.rows <= 0 || q.K <= 0 || q.ldh < q.K || !q.h || !q.w || !q.b || !q.seed || !(q.scale != 0.f))
+        return fail(CDS_ERR_INVALID, "head_grad: bad arguments");
+      if (q.act != CDS_ACT_NONE && q.act != CDS_ACT_SILU) return fail(CDS_ERR_UNSUPPORTED, "head_grad: act %d", q.act);
       return CDS_OK;
     }
     default:
@@ -339,6 +348,10 @@ int launch(const Step& s, const int* iter_ptr, int sm_count, cudaStream_t st, in
       CDS_CUDA(cudaGetLastError());
       return CDS_OK;
     }
+    case CDS_OP_HEAD_GRAD:
+      cds::head_grad_kernel<<<cds::head_grad_grid(s.op.u.head_grad.rows), 256, 0, st>>>(s.op.u.head_grad);
+      CDS_CUDA(cudaGetLastError());
+      return CDS_OK;
   }
   return fail(CDS_ERR_INVALID, "unknown operator kind");
 }
@@ -368,6 +381,7 @@ int preload_kernels() {
   CDS_CUDA(cudaFuncGetAttributes(&a, cds::gn_kernel));
   CDS_CUDA(cudaFuncGetAttributes(&a, cds::gn_bwd_kernel));
   CDS_CUDA(cudaFuncGetAttributes(&a, cds::guide_kernel));
+  CDS_CUDA(cudaFuncGetAttributes(&a, cds::head_grad_kernel));
   CDS_CUDA(cudaFuncGetAttributes(&a, cds::set_iter_kernel));
   CDS_CUDA(cudaFuncGetAttributes(&a, cds::advance_iter_kernel));
   return CDS_OK;
@@ -397,7 +411,8 @@ static_assert(sizeof(cds_stash_op) <= sizeof(cds_conv_op) && sizeof(cds_update_b
               "backward operators must not grow the cds_op union");
 // ... nor do the classifier-guidance operators
 static_assert(sizeof(cds_gn_op) <= sizeof(cds_conv_op) && sizeof(cds_gn_bwd_op) <= sizeof(cds_conv_op) &&
-              sizeof(cds_guide_op) <= sizeof(cds_conv_op), "classifier-guidance operators must not grow the cds_op union");
+              sizeof(cds_guide_op) <= sizeof(cds_conv_op) && sizeof(cds_head_grad_op) <= sizeof(cds_conv_op),
+              "classifier-guidance operators must not grow the cds_op union");
 
 struct cds_plan {
   int device = 0;

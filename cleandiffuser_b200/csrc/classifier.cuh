@@ -2,6 +2,8 @@
 //   CDS_OP_GN      act(GroupNorm(h) gamma + beta) [+ vec] [+ res] over a kept pre-norm input h, 8..16 B / element
 //   CDS_OP_GN_BWD  its backward with respect to h (statistics recomputed from h), 12 B / element
 //   CDS_OP_GUIDE   pred += s[iter] * g, 12 B / element
+// and, for QGPOClassifier (an Mlp of Linear + SiLU under an energy head 10 tanh(z / 10)):
+//   CDS_OP_HEAD_GRAD  z = act(h) . w + b per row and the seed d logp / d z of the backward, 4 B / element of h
 // One warp owns one (trajectory, group): a group holds at most a few hundred elements at the classifier's shapes (L x C/groups
 // <= 64 x 32), too few to split, and a warp-local reduction keeps every sum in one fixed order with no atomics -- two runs are
 // bitwise equal and CDS_OP_GN_BWD recomputes exactly the mean and rstd CDS_OP_GN used.
@@ -97,6 +99,23 @@ static __global__ void __launch_bounds__(256) guide_kernel(const cds_guide_op p,
   }
 }
 
+// One warp per row: the out_dim-1 Linear is a K-long dot product (K = 256 at QGPO's shapes), too short for a GEMM tile and
+// one launch instead of a conv plus an elementwise tanh.  Lane l sums elements l, l + 32, ... in order, then warp_sum's fixed
+// xor butterfly: the same bits on every run.  The seed follows autograd's order for logp = scale * tanh(z / scale):
+// mul's backward (1 * scale), tanh_backward (g * (1 - y * y)), then div's backward (/ scale).
+static __global__ void __launch_bounds__(256) head_grad_kernel(const cds_head_grad_op p) {
+  const int r = (int)((blockIdx.x * blockDim.x + threadIdx.x) >> 5), lane = threadIdx.x & 31;
+  if (r >= p.rows) return;
+  const float* h = p.h + (int64_t)r * p.ldh;
+  float s = 0.f;
+  for (int k = lane; k < p.K; k += 32) s = fmaf(apply_act(p.act, h[k]), p.w[k], s);
+  const float z = add_(warp_sum(s), p.b[0]);
+  const float y = tanhf(div_(z, p.scale));
+  if (lane == 0) p.seed[r] = div_(mul_(mul_(1.f, p.scale), sub_(1.f, mul_(y, y))), p.scale);
+}
+
 inline int gn_grid(int batch, int groups) { return (int)(((int64_t)batch * groups + 7) / 8); }
+
+inline int head_grad_grid(int rows) { return (rows + 7) / 8; }
 
 }  // namespace cds

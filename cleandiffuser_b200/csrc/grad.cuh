@@ -1,7 +1,7 @@
 // Backward operators of a differentiable reverse loop (sample(requires_grad=True) over DQLMlp):
 //   CDS_OP_STASH       per-iteration copy of a forward operand (+ the Mish of a pre-activation), 8..12 B / element
 //   CDS_OP_UPDATE_BWD  backward of the solver update + clip_prediction + fix_mask (kinds DDPM, DDIM, EPS, X), 24..36 B / element
-//   CDS_OP_DGRAD       dH = dZ W with the Mish derivative of the stashed pre-activation fused into the epilogue
+//   CDS_OP_DGRAD       dH = dZ W with the Mish or SiLU derivative of the stashed pre-activation fused into the epilogue
 //   CDS_OP_WGRAD       dW += Z^T H, db += sum_rows dZ, accumulated over the iterations
 // The two GEMM-shaped operators run on fp32 CUDA cores with 32 x 32 output tiles staged through shared memory: every output
 // element is one thread's sum in a fixed order (no split-K, no atomics), so a backward run is bitwise reproducible.
@@ -18,12 +18,20 @@ __device__ __forceinline__ float mish_grad(float x) {
   return tsp + x * sig * (1.f - tsp * tsp);
 }
 
+// d/dx silu(x), ATen's formula (aten/src/ATen/native/cuda/ActivationSiluKernel.cu, silu_backward): sig (1 + x (1 - sig))
+__device__ __forceinline__ float silu_grad(float x) {
+  const float sig = 1.f / (1.f + expf(-x));
+  return sig * (1.f + x * (1.f - sig));
+}
+
+__device__ __forceinline__ float act_grad(int act, float x) { return act == CDS_ACT_SILU ? silu_grad(x) : mish_grad(x); }
+
 static __global__ void __launch_bounds__(256) stash_kernel(const cds_stash_op p, const int* __restrict__ iter_ptr) {
   const int iter = *iter_ptr;
-  float* dst = p.dst + (int64_t)iter * p.dst_iter_stride;
+  float* dst = p.dst ? p.dst + (int64_t)iter * p.dst_iter_stride : nullptr;
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < p.n; i += (int64_t)gridDim.x * blockDim.x) {
     const float v = p.src[i];
-    dst[i] = v;
+    if (dst) dst[i] = v;
     if (p.act_out) p.act_out[i] = apply_act(p.act, v);
   }
 }
@@ -138,7 +146,7 @@ static __global__ void __launch_bounds__(256) dgrad_kernel(const cds_dgrad_op p,
     const int k = c0 + lc + j;
     if (k >= p.K) continue;
     float v = acc[j];
-    if (p.act == CDS_ACT_MISH) v = mul_(v, mish_grad(z[(int64_t)r * p.K + k]));
+    if (p.act != CDS_ACT_NONE) v = mul_(v, act_grad(p.act, z[(int64_t)r * p.K + k]));
     float* o = p.out + (int64_t)r * p.ldo + k;
     *o = p.accumulate ? add_(*o, v) : v;
     if (p.out_sum) { float* s = p.out_sum + (int64_t)r * p.K + k; *s = add_(*s, v); }

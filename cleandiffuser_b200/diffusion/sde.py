@@ -180,8 +180,8 @@ class BaseDiffusionSDE(DiffusionModel):
             from ..engine import runtime
             guide = None
             if self.classifier is not None and w_cg != 0.0:
-                # classifier guidance on the engine.  A CumRewClassifier over HalfJannerUNet1d is lowered into the replayed
-                # program (runtime.try_sample); any other classifier runs step by step: the engine evaluates the denoiser, this
+                # classifier guidance on the engine.  A CumRewClassifier over HalfJannerUNet1d or a QGPOClassifier over
+                # QGPONNClassifier is lowered into the replayed program (runtime.try_sample); any other classifier runs step by step: the engine evaluates the denoiser, this
                 # callback adds the guidance term to the prediction in place (same tensor expression as classifier_guidance
                 # above), the engine applies the update.
                 def guide(n, i, x_t, pred):
@@ -197,7 +197,7 @@ class BaseDiffusionSDE(DiffusionModel):
                                      sample_steps=sample_steps, order=order, step_values=step_values,
                                      alphas=alphas, sigmas=sigmas, hs=hs, stds=stds,
                                      cond_emb=condition_vec_cfg, w_cfg=w_cfg, n_samples=n_samples, guide=guide, sched_id=sched_id,
-                                     classifier=self.classifier, w_cg=w_cg)
+                                     classifier=self.classifier, w_cg=w_cg, cond_cg=condition_vec_cg)
             if out is not None:
                 return out
 

@@ -10,12 +10,13 @@ import os
 
 _LIB_PATH = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "csrc", "libcds.so")
 
-ABI_VERSION = 7
+ABI_VERSION = 8
 OPF_BRANCH_SHIFT = 8   # cds_op.flags bits 8..15: branch index (independent chains run on parallel streams)
 OPF_ONCE = 1          # cds_op.flags: run once per plan run (before its first iteration), not in every iteration
 OP_CONV, OP_UPDATE, OP_LNMOD, OP_ATTN, OP_PREP, OP_CAST, OP_MHA = range(7)
 OP_STASH, OP_UPDATE_BWD, OP_DGRAD, OP_WGRAD = 7, 8, 9, 10      # backward operators of a differentiable loop (csrc/grad.cuh)
 OP_GN, OP_GN_BWD, OP_GUIDE = 11, 12, 13       # classifier guidance inside the loop (csrc/classifier.cuh)
+OP_HEAD_GRAD = 14                             # QGPOClassifier's energy head and the seed of its backward (csrc/classifier.cuh)
 ACT_NONE, ACT_MISH, ACT_SILU, ACT_GELU_TANH, ACT_MISH_SILU, ACT_LEAKY_RELU, ACT_GELU_ERF = range(7)
 MATH_FP32, MATH_BF16_TC, MATH_TF32_TC = 0, 1, 2
 TC_MODES = (MATH_BF16_TC, MATH_TF32_TC)
@@ -137,10 +138,15 @@ class GuideOp(C.Structure):
                 ("g", _f32p), ("g_bstride", C.c_int64), ("g_lstride", C.c_int32), ("s", _f32p)]
 
 
+class HeadGradOp(C.Structure):
+    _fields_ = [("rows", C.c_int32), ("K", C.c_int32), ("h", _f32p), ("ldh", C.c_int32), ("act", C.c_int32),
+                ("w", _f32p), ("b", _f32p), ("scale", C.c_float), ("seed", _f32p)]
+
+
 class _OpUnion(C.Union):
     _fields_ = [("conv", ConvOp), ("update", UpdateOp), ("lnmod", LnModOp), ("attn", AttnOp), ("prep", PrepOp),
                 ("cast", CastOp), ("mha", MhaOp), ("stash", StashOp), ("update_bwd", UpdateBwdOp), ("dgrad", DgradOp),
-                ("wgrad", WgradOp), ("gn", GnOp), ("gn_bwd", GnBwdOp), ("guide", GuideOp)]
+                ("wgrad", WgradOp), ("gn", GnOp), ("gn_bwd", GnBwdOp), ("guide", GuideOp), ("head_grad", HeadGradOp)]
 
 
 class Op(C.Structure):

@@ -1037,12 +1037,29 @@ def lower_denoiser(p: Program, net: nn.Module, x: View, x_shape, has_cond: bool,
     raise Unsupported(f"backbone {name} with x_shape {tuple(x_shape)}")
 
 
-# =============================================================================== classifier guidance: HalfJannerUNet1d's input gradient
-def half_janner_guidable(clf, x_shape) -> Optional[str]:
-    """None when ``clf`` is a CumRewClassifier over a HalfJannerUNet1d whose input gradient ``lower_half_janner_grad`` can put
-    into the loop (recognised structurally, so that the reference's own instances qualify), else the reason it cannot."""
-    if type(clf).__name__ != "CumRewClassifier":
-        return f"classifier {type(clf).__name__} (CumRewClassifier only)"
+# =============================================================================== classifier guidance: the classifier's input gradient
+def guidable(clf, x_shape, cond_cg=None) -> Optional[str]:
+    """None when ``lower_classifier_grad`` can put the input gradient of ``clf`` at x_t into the loop, else the reason it cannot.
+    The classifiers are recognised structurally (class names and the attributes the lowering reads), so that the reference's own
+    instances qualify: a CumRewClassifier over a HalfJannerUNet1d, or a QGPOClassifier over a QGPONNClassifier guided with a
+    per-trajectory condition ``cond_cg`` (the observations)."""
+    name = type(clf).__name__
+    if name == "CumRewClassifier":
+        return _half_janner_reason(clf, x_shape)
+    if name == "QGPOClassifier":
+        return _qgpo_reason(clf, x_shape, cond_cg)
+    return f"classifier {name} (CumRewClassifier or QGPOClassifier only)"
+
+
+def lower_classifier_grad(p: Program, clf, x: View) -> View:
+    """Append the input gradient d sum(logp) / d x of a classifier ``guidable`` accepted to the iteration program -> the gradient
+    as a view shaped like ``x`` (its channels may include x's zero padding)"""
+    if type(clf).__name__ == "QGPOClassifier":
+        return lower_qgpo_grad(p, clf, x)
+    return lower_half_janner_grad(p, clf, x)
+
+
+def _half_janner_reason(clf, x_shape) -> Optional[str]:
     net = getattr(clf, "model_ema", None)
     if type(net).__name__ != "HalfJannerUNet1d":
         return f"classifier network {type(net).__name__} (HalfJannerUNet1d only)"
@@ -1058,6 +1075,44 @@ def half_janner_guidable(clf, x_shape) -> Optional[str]:
     L = max(x_shape[0] >> (len(net.downs) + 1), 1)
     if net.final_block[0].in_features != L * blocks[-1].conv1[0].out_channels + net.map_emb[2].out_features:
         return "classifier final_block does not match its feature map"
+    return None
+
+
+def _qgpo_layers(net):
+    """(hidden Linears, output Linear) of QGPONNClassifier.mlp when it is Linear + SiLU stages under an out_dim-1 Linear and an
+    identity, else None"""
+    seq = getattr(getattr(net, "mlp", None), "mlp", None)
+    if not isinstance(seq, nn.Sequential) or len(seq) < 3 or type(seq[-1]).__name__ != "Identity":
+        return None
+    stages, out = list(seq)[:-2], seq[-2]
+    if not isinstance(out, nn.Linear) or out.out_features != 1:
+        return None
+    if not all(isinstance(s, nn.Sequential) and len(s) == 2 and isinstance(s[0], nn.Linear) and type(s[1]).__name__ == "SiLU"
+               for s in stages):
+        return None
+    return [s[0] for s in stages], out
+
+
+def _qgpo_reason(clf, x_shape, cond_cg) -> Optional[str]:
+    net = getattr(clf, "model_ema", None)
+    if type(net).__name__ != "QGPONNClassifier":
+        return f"classifier network {type(net).__name__} (QGPONNClassifier only)"
+    if net.training:
+        return "classifier model_ema in train mode"
+    obs, act = getattr(net, "obs_proj", None), getattr(net, "act_proj", None)
+    if not isinstance(obs, nn.Linear) or not isinstance(act, nn.Linear) or obs.out_features != act.out_features:
+        return "classifier obs_proj / act_proj are not Linears of one width"
+    layers = _qgpo_layers(net)
+    if layers is None:
+        return "classifier mlp is not Linear + SiLU layers under an out_dim-1 Linear"
+    if layers[0][0].in_features <= 2 * act.out_features:
+        return "classifier mlp input has no time-embedding columns"
+    if len(x_shape) != 1 or x_shape[0] != act.in_features:
+        return "classifier act_proj does not match x"
+    if cond_cg is None:
+        return "no classifier condition (condition_cg=None)"
+    if cond_cg.dim() != 2 or cond_cg.shape[1] != obs.in_features:
+        return "classifier condition does not match obs_proj"
     return None
 
 
@@ -1118,7 +1173,7 @@ def w_down_dgrad(conv: nn.Conv1d) -> WSpec:
 
 
 def lower_half_janner_grad(p: Program, clf, x: View) -> View:
-    """Append the input gradient d sum(logp) / d x of ``clf.model_ema`` (a HalfJannerUNet1d; ``half_janner_guidable``) at x_t
+    """Append the input gradient d sum(logp) / d x of ``clf.model_ema`` (a HalfJannerUNet1d; ``guidable``) at x_t
     to the iteration program -> the gradient as a (rows, horizon, x.C) fp32 view (x.C may include zero padding channels).
 
     Forward, per ResidualBlock: conv1 -> h1;  m = CDS_OP_GN(h1) + time row;  conv2 -> h2;  [1x1 shortcut conv -> s];
@@ -1221,6 +1276,91 @@ def lower_half_janner_grad(p: Program, clf, x: View) -> View:
         p.conv(d1, w_conv_dgrad(blk.conv1[0], xin.C), dx, taps=k, pad=k // 2, **short)
         g = dx
     return g
+
+
+def _act_stash(p: Program, z: View, out: View, act: int):
+    """CDS_OP_STASH without a slot: out = act(z) (dense (rows, C) fp32 views)"""
+    op = cabi.Op()
+    op.kind = cabi.OP_STASH
+    s = op.u.stash
+    s.n, s.act, s.src, s.act_out = p.rows * z.C, act, z.ptr, out.ptr
+    p.ops.append(op)
+
+
+def _dgrad(p: Program, dz: torch.Tensor, w: torch.Tensor, out: torch.Tensor, z: Optional[View] = None, act: int = cabi.ACT_NONE):
+    """CDS_OP_DGRAD: out = (dz W) act'(z), dz (rows, N), W (N, K) dense, out (rows, K) dense"""
+    op = cabi.Op()
+    op.kind = cabi.OP_DGRAD
+    d = op.u.dgrad
+    n, k = w.shape
+    d.rows, d.N, d.K, d.dz, d.ldz, d.w, d.ldw = p.rows, n, k, dz.data_ptr(), n, w.data_ptr(), k
+    if z is not None:
+        d.z, d.z_iter_stride, d.act = z.ptr, 0, act
+    d.out, d.ldo = out.data_ptr(), k
+    p.ops.append(op)
+
+
+def lower_qgpo_grad(p: Program, clf, x: View) -> View:
+    """Append the input gradient d sum(logp) / d x of ``clf.model_ema`` (a QGPONNClassifier; ``guidable``) at x_t (rows, act_dim)
+    to the iteration program -> the gradient as a dense (rows, 1, act_dim) fp32 view.
+
+    logp = 10 tanh(z / 10),  z = W_o h_n + b_o,  h_k = silu(z_k),  z_k = W_k h_{k-1} + b_k,
+    z_1 = W_1 [obs_proj(c) | act_proj(x) | map_noise(t)] + b_1 = W_1a act_proj(x) + (W_1e map_noise(t) + b_1) + W_1y obs_proj(c)
+    Forward: a = act_proj(x) (CDS_OP_CONV);  z_1 (CDS_OP_CONV, its bias the per-iteration row W_1e e(t) + b_1 plus the
+    per-trajectory row W_1y obs_proj(c), both filled once per call);  per hidden layer h_k = silu(z_k) (CDS_OP_STASH without a
+    slot) and z_{k+1} (CDS_OP_CONV): the pre-activations stay for the backward.
+    Backward: the seed d logp / d z (CDS_OP_HEAD_GRAD over silu(z_n)), dz_n = (seed W_o) silu'(z_n), ..., dz_1 (CDS_OP_DGRAD
+    with SiLU), da = dz_1 W_1a, dx = da W_act (CDS_OP_DGRAD): the reference's factorisation through act_proj, kept so that the
+    gradient's summation error stays that of the two products autograd forms."""
+    net = clf.model_ema
+    R = p.rows
+    hidden, lin_o = _qgpo_layers(net)
+    lin1 = hidden[0]
+    E = net.act_proj.out_features
+    step_tab, samp_tab = p.buf(p.n_iters, lin1.out_features), p.buf(R, lin1.out_features)
+
+    def fill_time(ctx):
+        step_tab.copy_(F.linear(net.map_noise(ctx.t_all), lin1.weight[:, 2 * E:], lin1.bias))
+    fill_time.time_only = True
+
+    def fill_cond(ctx):
+        samp_tab.copy_(F.linear(net.obs_proj(ctx.cond_cg.to(torch.float32)), lin1.weight[:, :E]))
+    p.per_call += [fill_time, fill_cond]
+
+    dense = lambda w: View(p.buf(R, 1, w), 1, w)                 # noqa: E731   exact fp32 activations
+    a = p.conv(x, w_linear(net.act_proj.weight), dense(E), bias=_const_vec(p.packed(lambda: net.act_proj.bias)))
+    zs = []
+    h = a
+    for k, lin in enumerate(hidden):
+        z = dense(lin.out_features)
+        if k == 0:
+            p.conv(h, w_linear(lin.weight, slice(E, 2 * E)), z, bias=_vec(step_tab, samp_tab))
+        else:
+            p.conv(h, w_linear(lin.weight), z, bias=_const_vec(p.packed(lambda m=lin: m.bias)))
+        zs.append(z)
+        if k + 1 < len(hidden):
+            h = dense(lin.out_features)
+            _act_stash(p, z, h, cabi.ACT_SILU)
+
+    seed = p.buf(R, 1)
+    op = cabi.Op()
+    op.kind = cabi.OP_HEAD_GRAD
+    q = op.u.head_grad
+    q.rows, q.K, q.h, q.ldh, q.act = R, zs[-1].C, zs[-1].ptr, zs[-1].C, cabi.ACT_SILU
+    q.w, q.b = p.packed(lambda: lin_o.weight.reshape(-1)).data_ptr(), p.packed(lambda: lin_o.bias).data_ptr()
+    q.scale, q.seed = 10.0, seed.data_ptr()
+    p.ops.append(op)
+
+    up, w_up = seed, p.packed(lambda: lin_o.weight)
+    for k in range(len(hidden) - 1, -1, -1):
+        dz = p.buf(R, hidden[k].out_features)
+        _dgrad(p, up, w_up, dz, zs[k], cabi.ACT_SILU)
+        up, w_up = dz, p.packed(lambda m=hidden[k]: m.weight)
+    da = p.buf(R, E)
+    _dgrad(p, up, p.packed(lambda: lin1.weight[:, E:2 * E]), da)
+    dx = View(p.buf(R, 1, x.C), 1, x.C)
+    _dgrad(p, da, p.packed(lambda: net.act_proj.weight), dx.t)
+    return dx
 
 
 def guide(p: Program, pred: View, g: View, scale: torch.Tensor):

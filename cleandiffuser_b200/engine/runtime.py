@@ -31,8 +31,8 @@ import torch
 import torch.nn.functional as F
 
 from . import cabi
-from .lower import (DQLGrad, Program, Unsupported, View, _rev, guide as emit_guide, half_janner_guidable, lower_denoiser,
-                    lower_half_janner_grad)
+from .lower import (DQLGrad, Program, Unsupported, View, _rev, guidable, guide as emit_guide, lower_classifier_grad,
+                    lower_denoiser)
 from ..diffusion import solvers as S
 
 # guidance_path: how the latest engine call with classifier guidance was served -- "graph" (the classifier's input gradient is
@@ -59,7 +59,10 @@ def _math_mode():
 def _weights_version(module: torch.nn.Module, epoch: int = 0):
     """Fingerprint of the parameters a plan has packed copies of: tensor identities + autograd version counters (bumped by
     every in-place op on the parameter) + the owner's ``_weights_epoch`` (bumped by optimiser steps, EMA updates and
-    checkpoint loads of DiffusionModel -- writes through ``.data`` do not touch the version counters)."""
+    checkpoint loads of DiffusionModel -- writes through ``.data`` do not touch the version counters) or, for a classifier, its
+    ``weights_epoch`` (bumped by ``ema_update`` and ``load``).  A classifier object without that counter (the reference's own
+    classes) is fingerprinted by its version counters alone: after its ``update()`` / ``load()`` outside
+    ``agent.update_classifier`` the packed copies are stale until the plan is rebuilt."""
     acc = int(epoch) & 0xFFFFFFFFFFFF
     for p in module.parameters():
         acc = (acc * 1000003 + p._version * 31 + p.data_ptr()) & 0xFFFFFFFFFFFF
@@ -109,8 +112,9 @@ def _make_handle(device: torch.device, ops, n_iters: int):
 class _Ctx:
     """What the per-call table fillers see."""
 
-    def __init__(self, t_all, cond_rows):
-        self.t_all, self.cond_rows = t_all, cond_rows
+    def __init__(self, t_all, cond_rows, cond_cg=None):
+        # cond_cg: the classifier's per-trajectory condition (condition_cg), rows of this program's sub-batch
+        self.t_all, self.cond_rows, self.cond_cg = t_all, cond_rows, cond_cg
 
 
 def _n_branches(batch, row, consistency):
@@ -131,8 +135,8 @@ class SamplerPlan:
 
     def __init__(self, device, net, batch, x_shape, n_iters, n_slots, *, cfg_mode, predict_noise, has_mask,
                  has_min, has_max, keep_history, math, consistency=False, aux_history=False, classifier=None):
-        """classifier: a CumRewClassifier over HalfJannerUNet1d (``half_janner_guidable``) whose input gradient at x_t enters the
-        prediction between the denoiser and the update of every iteration (``pred += cg_scale[iter] * grad``).
+        """classifier: a classifier ``lower.guidable`` accepts, whose input gradient at x_t enters the prediction between the
+        denoiser and the update of every iteration (``pred += cg_scale[iter] * grad``).
         consistency: the EDM-preconditioned family (ContinuousConsistencyModel, ContinuousEDM): a CDS_OP_PREP in front of the
         denoiser (re-noise + c_in scaling) and the c_skip / c_out combine in the update; aux_history: second history buffer (the
         EDM Heun corrector needs the predictor's x_t and slope)."""
@@ -169,7 +173,7 @@ class SamplerPlan:
                 self.pred = pred.t if (pred.offset == 0 and pred.lstride == pred.C and pred.bstride == pred.L * pred.C) else None
             if classifier is not None:
                 assert K == 1 and cfg_mode != 2
-                grad = lower_half_janner_grad(p, classifier, _input_view(p, n_before, xview))
+                grad = lower_classifier_grad(p, classifier, _input_view(p, n_before, xview))
                 self.cg_scale = root.buf(n_iters)           # per-iteration guidance scale, filled by every guided call
                 emit_guide(p, pred, grad, self.cg_scale)
 
@@ -252,7 +256,7 @@ class SamplerPlan:
     def refresh_weights(self, epoch: int = 0):
         v = _weights_version(self.net, epoch)
         if self.classifier is not None:
-            v = _weights_version(self.classifier.model_ema, v)
+            v = _weights_version(self.classifier.model_ema, v * 1000003 + getattr(self.classifier, "weights_epoch", 0))
         if self.version is None:         # packed at construction
             self.version = v
         elif v != self.version:
@@ -268,14 +272,16 @@ class SamplerPlan:
                 h.close()
         self.handle = self.back_handle = None
 
-    def fill_tables(self, t_all, cond_emb, t_key=None):
-        """Per-call tables (time-conditioning rows, per-trajectory condition terms), once per ``sample()``."""
+    def fill_tables(self, t_all, cond_emb, t_key=None, cond_cg=None):
+        """Per-call tables (time-conditioning rows, per-trajectory condition terms of the denoiser and of a lowered
+        classifier), once per ``sample()``."""
         # table fillers that depend on (weights, timesteps) only are skipped when neither changed since the last call
         fresh = t_key is None or (t_key, self.version) != getattr(self, "_time_tables_key", None)
         with torch.no_grad():
             for fn, sl in self._fillers:             # every branch fills its own tables from its slice of the condition
                 if fresh or not getattr(fn, "time_only", False):
-                    fn(_Ctx(t_all, _cond_rows(self.cfg_mode, None if cond_emb is None else cond_emb[sl])))
+                    fn(_Ctx(t_all, _cond_rows(self.cfg_mode, None if cond_emb is None else cond_emb[sl]),
+                            None if cond_cg is None else cond_cg[sl]))
         self._time_tables_key = (t_key, self.version) if t_key is not None else None
 
     def run_guided(self, t_all, cond_emb, xt, noise_slots, guide, t_key=None):
@@ -302,12 +308,12 @@ class SamplerPlan:
             self.handle.run_range(n, upd, 1, stream)
         STATS["launches"] = (self.handle.launches_per_iter() + 2) * self.n_iters + 1
 
-    def run_chunked(self, t_all, cond_emb, xt, noise_rows, t_key=None):
+    def run_chunked(self, t_all, cond_emb, xt, noise_rows, t_key=None, cond_cg=None):
         """The whole loop, with the noise tape refilled between chunks when it is shorter than the number of draws
         (``noise_rows[n]`` = does iteration n draw?).  The draws are taken in loop order, so a seeded run consumes the
         generator like the reference loop; everything is enqueued on one stream, so a refill cannot overtake its readers."""
         cap = self.noise.shape[0] if self.noise is not None else 0
-        self.fill_tables(t_all, cond_emb, t_key)
+        self.fill_tables(t_all, cond_emb, t_key, cond_cg)
         stream = torch.cuda.current_stream(self.device).cuda_stream if self.device.type == "cuda" else 0
         use_graph = os.environ.get("CDS_GRAPH", "1") != "0"
         timed = STATS.get("time_loop") and self.device.type == "cuda"
@@ -492,7 +498,7 @@ def _load_resident(agent, plan, xt, prior, tab: _Table, tape_slots):
 
 def try_sample(agent, *, model, xt, prior, solver, sample_steps, order, step_values, alphas, sigmas, hs, stds,
                cond_emb, w_cfg, n_samples, guide=None, table=None, clip_in_loop=True, predict_noise=None, sched_id=None,
-               classifier=None, w_cg=0.0, consistency=False, aux_history=False):
+               classifier=None, w_cg=0.0, cond_cg=None, consistency=False, aux_history=False):
     """One ``sample()`` call of any sampler family on the engine -> x0, or None when the caller's PyTorch loop must run.
 
     ``table``: the coefficient rows for samplers that are "the same update kernel with another coefficient table" (the legacy
@@ -504,7 +510,8 @@ def try_sample(agent, *, model, xt, prior, solver, sample_steps, order, step_val
     history buffers.
     ``guide``: optional host callback ``guide(n, i, x_t, pred)`` (n = iteration, i = its loop index) run between the denoiser
     and the update of every iteration (classifier guidance); the loop then runs step by step instead of as a replayed graph --
-    unless ``classifier`` (the one ``guide`` evaluates, with weight ``w_cg``) is a CumRewClassifier over HalfJannerUNet1d under
+    unless ``classifier`` (the one ``guide`` evaluates, with weight ``w_cg`` and condition ``cond_cg``) is one ``lower.guidable``
+    accepts (a CumRewClassifier over HalfJannerUNet1d, a QGPOClassifier over QGPONNClassifier with a condition) under
     CDS_MATH = fp32 | tf32 with one sub-batch chain: its input gradient and the guidance term are then operators of the replayed
     program, and ``guide`` is not called."""
     def decline(cfg_mode):
@@ -532,7 +539,9 @@ def try_sample(agent, *, model, xt, prior, solver, sample_steps, order, step_val
         row_elems *= s_
     cg_reason = None                       # why a guided call keeps the host callback (None: the graph serves it)
     if guide is not None:
-        cg_reason = "no classifier" if classifier is None else half_janner_guidable(classifier, x_shape)
+        cg_reason = "no classifier" if classifier is None else guidable(classifier, x_shape, cond_cg)
+        if cg_reason is None and cond_cg is not None and cond_cg.shape[0] != batch:
+            cg_reason = "classifier condition rows != batch"
         if cg_reason is None and math == cabi.MATH_BF16_TC:
             cg_reason = "CDS_MATH=bf16"
         if cg_reason is None and _n_branches(batch, row_elems, False) != 1:
@@ -570,7 +579,8 @@ def try_sample(agent, *, model, xt, prior, solver, sample_steps, order, step_val
         plan.run_guided(tab.t, cond_emb, xt, slots, lambda n, x, p: guide(n, order[n], x, p), t_key=tab.t_key)
     else:
         # the loop's draws: same calls, same order, same shapes as the reference loop's (diffusionsde.py:548,571,...)
-        plan.run_chunked(tab.t, cond_emb, xt, (tab.rows[:, S.R_NOISE] > 0).tolist(), t_key=tab.t_key)
+        plan.run_chunked(tab.t, cond_emb, xt, (tab.rows[:, S.R_NOISE] > 0).tolist(), t_key=tab.t_key,
+                         cond_cg=cond_cg if lowered_cg else None)
     STATS["engine_calls"] += 1
     return plan.x.clone()
 

@@ -3,9 +3,10 @@
 ``HalfJannerUNet1d`` is the down half of JannerUNet1d followed by a small MLP head, with the reference's constructor signature,
 parameter names and shapes (cleandiffuser/nn_classifier/half_jannerunet.py), so its checkpoints load.  Under classifier guidance
 (``CumRewClassifier``) the engine lowers its forward and input gradient into the replayed loop (``engine/lower.py``,
-``lower_half_janner_grad``); everything else about it runs in PyTorch.
+``lower_half_janner_grad``); everything else about it runs in PyTorch.  ``QGPONNClassifier`` (nn_classifier/mlp.py) is QGPO's
+energy network; under ``QGPOClassifier`` guidance its input gradient is lowered the same way (``lower_qgpo_grad``).
 """
-from typing import Optional, Tuple
+from typing import List, Optional, Tuple
 
 import numpy as np
 import torch
@@ -13,6 +14,7 @@ import torch.nn as nn
 
 from ..nn_diffusion.base import BaseNNDiffusion
 from ..nn_diffusion.unets import Downsample1d, ResidualBlock
+from ..utils import Mlp
 
 
 class HalfJannerUNet1d(BaseNNDiffusion):
@@ -61,3 +63,21 @@ class HalfJannerUNet1d(BaseNNDiffusion):
         for block, down in (self.mid_block1, self.mid_block2):
             h = down(block(h, emb))
         return self.final_block(torch.cat([h.flatten(1), emb], dim=-1))
+
+
+class QGPONNClassifier(BaseNNDiffusion):
+    """x (b, act_dim) noisy actions, t (b,), y (b, obs_dim) observations -> energy (b, 1) in (-10, 10):
+    ``10 tanh(mlp([obs_proj(y), act_proj(x), map_noise(t)]) / 10)`` with an Mlp of Linear + SiLU hidden layers."""
+
+    def __init__(self, obs_dim: int, act_dim: int, emb_dim: int, hidden_dims: List[int],
+                 timestep_emb_type: str = "positional"):
+        super().__init__(emb_dim, timestep_emb_type)
+        self.obs_proj = nn.Linear(obs_dim, emb_dim)
+        self.act_proj = nn.Linear(act_dim, emb_dim)
+        self.mlp = Mlp(in_dim=3 * emb_dim, hidden_dims=hidden_dims, out_dim=1, activation=nn.SiLU())
+
+    def forward(self, x: torch.Tensor, t: torch.Tensor, y: torch.Tensor):
+        y = self.obs_proj(y)
+        x = self.act_proj(x)
+        out = self.mlp(torch.cat([y, x, self.map_noise(t)], dim=-1))
+        return torch.tanh(out / 10) * 10

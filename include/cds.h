@@ -25,6 +25,8 @@
  *   CDS_OP_WGRAD        iteration stashes, the update's backward, Linear data / weight gradients (declared further down)
  *   CDS_OP_GN ..        classifier guidance inside the loop (diffusionsde.py:153-173 with CumRewClassifier over HalfJannerUNet1d):
  *   CDS_OP_GUIDE        GroupNorm + Mish over a kept pre-norm input, its backward, and pred += s[iter] * grad (further down)
+ *   CDS_OP_HEAD_GRAD    the energy head of QGPO's classifier (qgpo_classifier.py / nn_classifier/mlp.py: 10 tanh(z / 10) over
+ *                       an Mlp of Linear + SiLU): z = h . w + b per row and the seed of its backward (further down)
  *
  * Conventions
  *  - every function returns 0 on success, a negative cds_status otherwise; cds_last_error() gives the
@@ -51,7 +53,7 @@
 extern "C" {
 #endif
 
-#define CDS_ABI_VERSION 7
+#define CDS_ABI_VERSION 8
 
 typedef enum cds_status {
   CDS_OK = 0,
@@ -66,7 +68,9 @@ typedef enum cds_op_kind { CDS_OP_CONV = 0, CDS_OP_UPDATE = 1, CDS_OP_LNMOD = 2,
                            /* differentiable sampling (sample(requires_grad=True) over DQLMlp, csrc/grad.cuh) */
                            CDS_OP_STASH = 7, CDS_OP_UPDATE_BWD = 8, CDS_OP_DGRAD = 9, CDS_OP_WGRAD = 10,
                            /* classifier guidance (the input gradient of HalfJannerUNet1d, csrc/classifier.cuh) */
-                           CDS_OP_GN = 11, CDS_OP_GN_BWD = 12, CDS_OP_GUIDE = 13 } cds_op_kind;
+                           CDS_OP_GN = 11, CDS_OP_GN_BWD = 12, CDS_OP_GUIDE = 13,
+                           /* classifier guidance (the energy head of QGPOClassifier, csrc/classifier.cuh) */
+                           CDS_OP_HEAD_GRAD = 14 } cds_op_kind;
 typedef enum cds_act { CDS_ACT_NONE = 0, CDS_ACT_MISH = 1, CDS_ACT_SILU = 2, CDS_ACT_GELU_TANH = 3,
                        CDS_ACT_MISH_SILU = 4 /* silu(mish(x)): DiT's map_emb tail feeding every adaLN (dit.py:26,43,71) */,
                        CDS_ACT_LEAKY_RELU = 5 /* negative slope 0.01 (nn.LeakyReLU default; pearcemlp.py:44) */,
@@ -219,7 +223,8 @@ typedef struct cds_update_op {
  * the backward program walks the forward iterations in reverse by pointing at the last slot with a negative stride, so that
  * one captured graph serves every backward iteration like it does every forward one. */
 
-/* dst[iter*dst_iter_stride + i] = src[i];  act_out[i] = act(src[i]) when act_out != NULL (i < n).  act: CDS_ACT_NONE / MISH */
+/* dst[iter*dst_iter_stride + i] = src[i] when dst != NULL;  act_out[i] = act(src[i]) when act_out != NULL (i < n); at least one
+ * of the two.  act: CDS_ACT_NONE / MISH / SILU */
 typedef struct cds_stash_op {
   int64_t n;
   int32_t act;
@@ -248,7 +253,8 @@ typedef struct cds_update_bwd_op {
 
 /* Data gradient of a Linear layer:  out(r, k) [+]= (sum_n dz(r, n) W(n, k)) * act'(z(r, k))
  * dz (rows, N) row stride ldz; W (N, K) row stride ldw (a PyTorch [out, in] weight or a column block of one);
- * z = the stashed pre-activation of the layer's input (z + iter*z_iter_stride, dense (rows, K)), required when act = MISH;
+ * z = the stashed pre-activation of the layer's input (z + iter*z_iter_stride, dense (rows, K)), required when act = MISH or SILU
+ *     (act' follows ATen: mish_backward, and silu_backward's sig * (1 + z * (1 - sig)));
  * out (rows, K) row stride ldo, overwritten (accumulate = 0) or added to (1); out_sum (dense (rows, K), optional) += result.
  * fp32 CUDA cores; deterministic (every output is one thread's fixed-order sum). */
 typedef struct cds_dgrad_op {
@@ -314,6 +320,20 @@ typedef struct cds_guide_op {
   const float* s;
 } cds_guide_op;
 
+/* The energy head of QGPO's classifier, logp = scale * tanh(z / scale), z = act(h(r, :)) . w + b, and the seed of its backward:
+ *   seed(r) = ((1 * scale) * (1 - tanh(z / scale)^2)) / scale        (d sum(logp) / d z in autograd's order: the product's
+ *                                                                        backward, tanh_backward, then the division's)
+ * h (rows, K) row stride ldh, read through act (CDS_ACT_NONE or SILU: the head's input recomputed from the last hidden layer's
+ * pre-activation); w: K floats (the [1, K] weight of an out_dim-1 Linear); b: 1 float; seed: rows floats.  One warp per row,
+ * lane-strided partial sums reduced by a fixed xor butterfly: two runs are bitwise equal. */
+typedef struct cds_head_grad_op {
+  int32_t rows, K;
+  const float* h; int32_t ldh; int32_t act;
+  const float* w; const float* b;
+  float scale;
+  float* seed;
+} cds_head_grad_op;
+
 /* cds_op.flags */
 enum { CDS_OPF_ONCE = 1 /* run once per cds_plan_run, before its first iteration, instead of in every iteration */,
        CDS_OPF_BRANCH_SHIFT = 8, CDS_OPF_BRANCH_MASK = 0xff00
@@ -326,7 +346,7 @@ typedef struct cds_op {
   int32_t flags;
   union { cds_conv_op conv; cds_update_op update; cds_lnmod_op lnmod; cds_attn_op attn; cds_prep_op prep; cds_cast_op cast;
           cds_mha_op mha; cds_stash_op stash; cds_update_bwd_op update_bwd; cds_dgrad_op dgrad; cds_wgrad_op wgrad;
-          cds_gn_op gn; cds_gn_bwd_op gn_bwd; cds_guide_op guide; } u;
+          cds_gn_op gn; cds_gn_bwd_op gn_bwd; cds_guide_op guide; cds_head_grad_op head_grad; } u;
 } cds_op;
 
 typedef struct cds_plan cds_plan;
