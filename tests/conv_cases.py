@@ -171,6 +171,27 @@ CASES = [
     case("simt_convT", "fp32", 41, 8, 64, 64, simt(128), taps=3, phases=2, act=M),
     case("simt_head", "fp32", 41, 32, 32, 14, simt(32), taps=5, act=cabi.ACT_GELU_ERF, in_dtype=cabi.BF16),
     case("simt_wide_nogn", "fp32", 82, 4, 64, 320, simt(128), act=cabi.ACT_SILU, film="traj", in_mod=41),
+    # conv_simt storing TF32 / bf16: on tensor-core programs a Linear over the raw x_t (3..9 fp32 channels) is not
+    # tensor-core material, runs here, and stores the program's activation type (SfBCUNet's first block, PearceMlp's act_emb)
+    case("simt_c6_c512_tf32out", "fp32", 300, 1, 6, 512, simt(128), act=cabi.ACT_SILU, film="shift", out_dtype=cabi.TF32),
+    case("simt_c6_c512_bf16out", "fp32", 300, 1, 6, 512, simt(128), act=cabi.ACT_SILU, film="shift", out_dtype=cabi.BF16),
+    case("simt_c9_c128_bf16out", "fp32", 1000, 1, 9, 128, simt(128), act=cabi.ACT_LEAKY_RELU, out_dtype=cabi.BF16),
+    case("simt_c9_c256_tf32out", "fp32", 1000, 1, 9, 256, simt(128), bias="both", out_dtype=cabi.TF32),
+    case("simt_c6_c128_shortcut_tf32out", "fp32", 300, 1, 6, 128, simt(128), act=cabi.ACT_SILU, res="conv",
+         out_dtype=cabi.TF32),
+    # SfBCUNet's first block, second operator: h (the program's activation type) -> C_out, plus the 1x1 shortcut of x_t
+    case("simt_c512_shortcut_c6_bf16", "fp32", 300, 1, 512, 512, simt(128), act=cabi.ACT_SILU, res="conv", res_C=6,
+         in_dtype=cabi.BF16, out_dtype=cabi.BF16),
+    case("simt_c512_shortcut_c6_tf32", "fp32", 300, 1, 512, 256, simt(128), act=cabi.ACT_SILU, res="conv", res_C=6,
+         in_dtype=cabi.TF32, out_dtype=cabi.TF32),
+    # the CFG form: both halves share x_t (in_batch_mod) and the shortcut's input (res_batch_mod)
+    case("simt_cfg_c6_c256_bf16", "fp32", 600, 1, 6, 256, simt(128), act=cabi.ACT_SILU, film="shift", in_mod=300,
+         res="conv", res_mod=300, out_dtype=cabi.BF16),
+    case("simt_cfg_c6_c256_tf32", "fp32", 600, 1, 6, 256, simt(128), act=cabi.ACT_SILU, film="shift", in_mod=300,
+         res="conv", res_mod=300, out_dtype=cabi.TF32),
+    # PearceMlp's FCBlock on fp32 programs: Linear + GroupNorm(8) + exact GELU, a constant scale, an identity residual
+    case("simt_gn_gelu_c512", "fp32", 300, 1, 512, 512, simt(64), groups=8, act=cabi.ACT_GELU_ERF, bias="both",
+         film="const_scale", res="id"),
 ]
 
 # ---- the persistent tile loop: a large-batch twin of one case per conv_tc instantiation, so that every CTA of the launch runs
@@ -266,6 +287,8 @@ def make(c, device, it=1):
             v = torch.randn(rows, Lv, C, generator=g)
             if not (name == "in" and c["in_dtype"] == cabi.F32 and math == "tf32"):
                 v = _rnd(v, math if name in ("in", "res_in") or math == "bf16" else "fp32")
+            if dt == cabi.TF32:             # a CDS_TF32 tensor holds TF32 values, whichever kernel family reads it
+                v = _rnd(v, "tf32")
             view.copy_(v.to(buf.dtype))
         d["buf/" + name] = buf.to(device)
         d["off/" + name] = off
@@ -307,6 +330,9 @@ def make(c, device, it=1):
         d["bias"] = d["bias"] + c["offset"]
     film = c["film"]
     d["scale_vec"], d["scale"] = vec(False, film in ("traj", "gate"), 0.3, 1.0) if film in ("traj", "gate") else (cabi.Vec(), None)
+    if film == "const_scale":               # one (C_out,) vector for every row and iteration (step_stride 0)
+        d["scale"] = (1.414 + 0.3 * torch.randn(C_out, generator=g)).to(device)
+        d["scale_vec"] = cabi.Vec(d["scale"].data_ptr(), 0, 0, 0)
     d["shift_vec"], d["shift"] = vec(film == "shift", film == "traj") if film in ("shift", "traj") else (cabi.Vec(), None)
     if c["groups"]:
         d["gamma"] = (1 + 0.2 * torch.randn(C_out, generator=g)).to(device)
@@ -359,7 +385,7 @@ def descriptor(c, d=None, ptr=None):
     else:                                   # presence (and shape) of the vectors is all that eligibility looks at
         fake_vec = lambda step, sample: cabi.Vec(10 << 28 if step else 0, 16, 11 << 28 if sample else 0, 16)
         o.bias = fake_vec(c["bias"] in ("step", "both"), c["bias"] in ("sample", "both"))
-        o.scale = fake_vec(False, c["film"] in ("traj", "gate"))
+        o.scale = fake_vec(c["film"] == "const_scale", c["film"] in ("traj", "gate"))
         o.shift = fake_vec(c["film"] == "shift", c["film"] == "traj")
     return op
 

@@ -70,7 +70,8 @@ def test_conv_choice_reports_refusals():
 
 
 # ---- the checker itself, with the fp64 reference standing in for the kernel (small batches, CPU)
-SELF_CHECK = ["bf16_c128_k64", "tf32_c32_gn_k64", "tf32_convT_c64", "ps_tf32_c128_k5", "simt_bn64_cpg8"]
+SELF_CHECK = ["bf16_c128_k64", "tf32_c32_gn_k64", "tf32_convT_c64", "ps_tf32_c128_k5", "simt_bn64_cpg8",
+              "simt_c6_c128_shortcut_tf32out", "simt_gn_gelu_c512"]
 
 
 def _small(name):

@@ -1,8 +1,8 @@
 """Operator-level parity of CDS_OP_CONV: every case of tests/conv_cases.py runs through ``cds_run_op`` and is checked
 against tests/opref.py's fp64 reference on the same GPU, with the bound of conv_cases.check.  Each case also checks
 that the gaps of every buffer (NaN) are neither read nor written, that the result is deterministic and does not depend
-on the TMA store / residual-prefetch path, on the position of the batch in its tiles, or (CDS_TF32 outputs) on
-anything but the round-to-nearest of the kernel's fp32 value."""
+on the TMA store / residual-prefetch path, on the position of the batch in its tiles, or (CDS_TF32 outputs, and every
+TF32 / bf16 output of conv_simt) on anything but the round-to-nearest of the kernel's fp32 value."""
 import pytest
 import torch
 
@@ -160,6 +160,9 @@ def test_conv_case_matches_fp64(name, monkeypatch):
         assert torch.equal(opref.tf32_round(d32["view/out"]).view(torch.int32), y.view(torch.int32)), \
             "CDS_TF32 store is not the round-to-nearest (ties away) of the kernel's fp32 value"
 
+    if fam == "simt" and c["out_dtype"] != cabi.F32:
+        _simt_store_is_the_rounding_of_fp32(c, d, y)
+
     if fam == "ps":
         monkeypatch.setenv("CDS_PS", "0")
         op_tc = cc.descriptor(c, d)
@@ -170,3 +173,20 @@ def test_conv_case_matches_fp64(name, monkeypatch):
         _record("tc", frac, name + " (CDS_PS=0)")
         assert ok, "CDS_PS=0 (conv_tc): " + msg
         assert _gaps_untouched(c, d)
+
+
+def _simt_store_is_the_rounding_of_fp32(c, d, y):
+    """conv_gemm_f32_kernel reads out_dtype only in st_act, at the store: everything before it is the same arithmetic for
+    every output type.  So the same op with an fp32 output, into a separate buffer, gives the kernel's fp32 value, and a
+    TF32 / bf16 output must be exactly its round-to-nearest -- a check no bound can make, since one TF32 ulp is within
+    the 2^-10 |ref| of conv_cases.check."""
+    c32 = dict(c, out_dtype=cabi.F32)
+    d32 = cc.make(c32, DEV)
+    for name in cc.geometry(c):                         # the same operands, bit for bit
+        if name != "out":
+            assert torch.equal(d32["buf/" + name].float().nan_to_num(7.0), d["buf/" + name].float().nan_to_num(7.0)), name
+    _run(c32, cc.descriptor(c32, d32))
+    y32 = d32["view/out"]
+    want = opref.tf32_round(y32) if c["out_dtype"] == cabi.TF32 else y32.to(torch.bfloat16).float()
+    assert torch.equal(want.view(torch.int32), y.view(torch.int32)), \
+        f"conv_simt's {'CDS_TF32' if c['out_dtype'] == cabi.TF32 else 'bf16'} store is not the round-to-nearest of its fp32 value"

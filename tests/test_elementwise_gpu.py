@@ -358,17 +358,32 @@ LN_CASES = [(C, 0, p) for p, Cs in (("<16,3>", (32, 64, 192)), ("<16,6>", (256, 
                                      ("scalar", (30, 322)), ("streaming", (768, 1024))) for C in Cs] + [(320, 1, "scalar")]
 
 
+# mod_bstride = 0: one modulation row for every row (IDQLMlp's LayerNorm affine, L = 1), at IDQLMlp's hidden widths
+BROADCAST_C = (256, 512)
+
+
+def _mod_rows(B, C, bstride, g):
+    """a (B, C) modulation operand with rows bstride floats apart; bstride = 0: one row, followed by B - 1 rows of NaN, so
+    that a kernel reading row b at b * C stores NaN"""
+    if bstride:
+        return (0.3 * torch.randn(B, bstride, generator=g)).to(DEV)[:, :C]
+    buf = torch.full((B, C), float("nan"))
+    buf[0] = 0.3 * torch.randn(C, generator=g)
+    return buf.to(DEV)[:1].expand(B, C)
+
+
 @pytest.mark.gpu
 @pytest.mark.parametrize("C,out_off,path", LN_CASES)
 def test_lnmod_matches_fp64(C, out_off, path):
-    B, L = 37, 7                                            # 259 rows: the 16-lane paths leave a half-warp idle
     st = torch.cuda.current_stream().cuda_stream
-    for bstride in (C, 2 * C + 4):
+    for bstride in (C, 2 * C + 4) + ((0,) if C in BROADCAST_C and out_off == 0 else ()):
+        # 259 rows: the 16-lane paths leave a half-warp idle
+        B, L = (37, 7) if bstride else (259, 1)
         assert ln_path(C, out_off, bstride) == path
         g = torch.Generator().manual_seed(C + bstride)
         x = (2 * torch.randn(B, L, C, generator=g) + 0.5).to(DEV)
-        shift = (0.3 * torch.randn(B, bstride, generator=g)).to(DEV)[:, :C]
-        scale = (0.3 * torch.randn(B, bstride, generator=g)).to(DEV)[:, :C]
+        shift = _mod_rows(B, C, bstride, g)
+        scale = _mod_rows(B, C, bstride, g)
         ref = opref.lnmod(x, shift, scale, 1e-6)
         y32 = None
         for od in (cabi.F32, cabi.TF32, cabi.BF16):
