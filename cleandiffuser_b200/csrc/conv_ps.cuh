@@ -9,12 +9,15 @@
 //
 // * A_l = the activations of input position l: ONE TMA box {KC channels, 1 position, 128 trajectories} of the channels-last
 //   tensor; every activation byte enters the SM once, the conv's zero padding is simply the absence of the (l, l') pairs
-//   that fall outside [0, P) (14 MMAs instead of 20 for P = 4, taps = 5).
-// * W_j = TMA box {KC, N} of the [tap][C_out][C_in] weight, fetched once per channel chunk and used by up to P MMAs:
-//   4 x the trajectories per weight byte of conv_tc_kernel.
+//   that fall outside [0, P) (14 (l, l') products instead of 20 for P = 4, taps = 5).
+// * W_j = TMA box {KC, N} of the [tap][C_out][C_in] weight, fetched once per channel chunk and used by up to P positions:
+//   4 x the trajectories per weight byte of conv_tc_kernel.  The tap slots are stored in reverse order, so the W tiles that
+//   one input position needs for consecutive output positions are consecutive.
 // * two consumer warpgroups (warps 0-7): warpgroup g holds the P accumulators D_l' of trajectories [64 g, 64 g + 64) in
-//   registers (wgmma, N columns each; the shortcut conv's P accumulators next to them).  The CTA has one tile, so once the
-//   MMAs are done the operand ring is idle and the accumulators are written over it as a 128-row fp32 tile.
+//   registers (the shortcut conv's P accumulators next to them).  An input position's outputs take one wgmma of several x N
+//   columns per register block of the accumulators instead of one N-column wgmma each, so the A tile is read from shared
+//   memory fewer times (conv_ps_mma_position: 7 wgmmas per k step instead of 14 for taps = 5).  The CTA has one tile, so
+//   once the MMAs are done the operand ring is idle and the accumulators are written over it as a 128-row fp32 tile.
 // * epilogue (the same 8 warps): thread = one trajectory x NH = N/2 columns (ONE GroupNorm group) x all P positions, so the
 //   GroupNorm statistics over (P positions x C_out/8 channels) are plain in-thread sums: no shuffles.  Two passes over the
 //   tile (statistics, then normalise + Mish + store).
@@ -24,6 +27,7 @@
 //
 // Algorithmic HBM bytes per launch: 2*(batch*P*C_in + batch*P*C_out) (+ shortcut input), weights once through L2.
 #pragma once
+#include <utility>
 #include "conv_tc.cuh"
 
 namespace cds {
@@ -32,7 +36,7 @@ struct ConvPsParams {
   CUtensorMap tm_a, tm_b, tm_a2, tm_b2;
   CUtensorMap tm_out;             // output as a TMA-store target: box {16 channels, 1 position, 32 trajectories} (one epilogue warp's
   int out_tma;                    // lanes x 16 columns), staged in shared memory; valid when out_tma != 0
-  int batch, C_out, taps, pad;
+  int batch, C_out, taps;         // taps 1, 3 or 5 with pad = taps / 2 (conv_ps_eligible)
   int kchunks, kchunks2;          // channel chunks of the main conv / of the shortcut conv
   int n_tiles;                    // column tiles per trajectory tile (C_out / N)
   int in_batch_mod, res_batch_mod;
@@ -65,6 +69,99 @@ struct ConvPsCfg {
   static_assert(kStagingBytes + 128 * kAccPitch * 4 <= kStages * kStageBytes, "accumulator tile must fit over the ring");
   static_assert(kSmemBytes <= 227 * 1024, "stage ring does not fit");
 };
+
+// The main-conv MMAs of input position L for one channel chunk.  Input position L feeds output positions lo..hi through taps
+// j = L - l' + pad, and the producer stores tap j's W tile in slot taps-1-j, so output l' reads slot l' - L + taps-1-pad: the
+// W tiles of lo..hi are consecutive, and a run of outputs is ONE wgmma of (run length) x N columns that reads the A tile once
+// (columns [i N, (i + 1) N) of the run are the next accumulator, in the fragment layout of wgmma_sm90.cuh).
+// The run cannot always be all of lo..hi: a wgmma's accumulators are one register tuple, and ptxas can share registers
+// between tuples only when they start at the same register; runs that start at different outputs of one accumulator would
+// force copies and serialize every wgmma of the loop.  So the accumulators are register blocks that start at each
+// position's lo -- outputs 0 .. P-2-pad alone, then P-1-pad .. P-1 as one block -- and every run covers a prefix of a block:
+// 7 wgmmas per k step instead of 14 for taps 5 (runs of 1+2, 1+3, 1+3 and 3 outputs), 8 instead of 10 for taps 3.
+// Each output element sums the same products in the same order as with one N-column wgmma per (l, l') pair.  The
+// accumulators start at zero in registers and every wgmma accumulates, so no first chunk is special.
+template <int W, int KC, bool TF32>
+__device__ __forceinline__ void conv_ps_mma_run(float (&dv)[W / 2], uint64_t da, uint64_t db) {
+#pragma unroll
+  for (int k = 0; k < KC / 16; ++k) ptx::Wgmma<W, TF32>::mma(dv, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), 1u);
+}
+
+template <int TAPS, int L, int KC, int N, int P, bool TF32>
+__device__ __forceinline__ void conv_ps_mma_position(float (&d)[P][N / 2], uint64_t da, uint32_t sb) {
+  using Cfg = ConvPsCfg<KC, N, P, false>;
+  constexpr int pad = TAPS / 2;
+  constexpr int lo = L - pad > 0 ? L - pad : 0;
+  constexpr int hi = L + pad < P - 1 ? L + pad : P - 1;
+  constexpr int tail = P - 1 - pad;                   // first output of the last register block
+  constexpr int t0 = lo > tail ? lo : tail;           // first output of this position's run in that block
+  const uint32_t sb_lo = sb + (uint32_t)((lo - L + TAPS - 1 - pad) * Cfg::kBTile);     // W slot of output lo
+#pragma unroll
+  for (int lp = lo; lp < t0 && lp <= hi; ++lp)
+    conv_ps_mma_run<N, KC, TF32>(d[lp], da, ptx::make_kmajor_desc<Cfg::kRowBytes>(sb_lo + (lp - lo) * Cfg::kBTile));
+  if constexpr (t0 <= hi)
+    conv_ps_mma_run<(hi - t0 + 1) * N, KC, TF32>(*reinterpret_cast<float (*)[(hi - t0 + 1) * N / 2]>(&d[t0][0]), da,
+                                                 ptx::make_kmajor_desc<Cfg::kRowBytes>(sb_lo + (t0 - lo) * Cfg::kBTile));
+}
+
+template <int TAPS, int KC, int N, int P, bool TF32, int... Ls>
+__device__ __forceinline__ void conv_ps_mma_chunk(float (&d)[P][N / 2], uint32_t sa, uint32_t sb, std::integer_sequence<int, Ls...>) {
+  using Cfg = ConvPsCfg<KC, N, P, false>;
+  (conv_ps_mma_position<TAPS, Ls, KC, N, P, TF32>(d, ptx::make_kmajor_desc<Cfg::kRowBytes>(sa + Ls * Cfg::kATile), sb), ...);
+}
+
+// Consumer warps 0..7: the main loop over the channel chunks (warpgroup g accumulates trajectories [64 g, 64 g + 64): D[l'] in
+// registers, the shortcut's D2[l] next to them), then the accumulators as a 128-row fp32 tile over the idle ring.
+template <int TAPS, int KC, int N, int P, bool HAS_RES, bool TF32>
+__device__ __forceinline__ void conv_ps_mma(const ConvPsParams& p, uint64_t* full_bar, uint64_t* empty_bar, uint32_t smem_base,
+                                            float* acc) {
+  using Cfg = ConvPsCfg<KC, N, P, HAS_RES>;
+  constexpr int kStages = Cfg::kStages;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int g = warp >> 2;
+  const int n_main = p.kchunks;
+  const int n_chunks = n_main + (HAS_RES ? p.kchunks2 : 0);
+  float d[P][N / 2];
+  float d2[HAS_RES ? P : 1][N / 2];
+#pragma unroll
+  for (int l = 0; l < P; ++l)
+#pragma unroll
+    for (int i = 0; i < N / 2; ++i) { d[l][i] = 0.f; d2[HAS_RES ? l : 0][i] = 0.f; }
+#pragma unroll 1                                      // each chunk waits on its stage anyway: unrolling only grows the code
+  for (int c = 0; c < n_chunks; ++c) {
+    const int s = c % kStages;
+    ptx::mbar_wait(&full_bar[s], (c / kStages) & 1);
+    if (c == 0 && threadIdx.x == 0) CDS_TRACE(9, clock64());
+    const uint32_t sa = smem_base + s * Cfg::kStageBytes + (uint32_t)(g * 64 * Cfg::kRowBytes);
+    const uint32_t sb = smem_base + s * Cfg::kStageBytes + P * Cfg::kATile;
+    ptx::wgmma_fence();
+    if (!HAS_RES || c < n_main) {
+      conv_ps_mma_chunk<TAPS, KC, N, P, TF32>(d, sa, sb, std::make_integer_sequence<int, P>{});
+    } else if constexpr (HAS_RES) {
+      const uint64_t db = ptx::make_kmajor_desc<Cfg::kRowBytes>(sb);
+#pragma unroll
+      for (int l = 0; l < P; ++l) {
+        const uint64_t da = ptx::make_kmajor_desc<Cfg::kRowBytes>(sa + l * Cfg::kATile);
+#pragma unroll
+        for (int k = 0; k < KC / 16; ++k) ptx::Wgmma<N, TF32>::mma(d2[l], da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), 1u);
+      }
+    }
+    ptx::wgmma_commit();
+    ptx::wgmma_wait<1>();                             // the previous chunk's MMAs are complete: its stage is free
+    if (c > 0) { __syncwarp(); if (lane == 0) ptx::mbar_arrive(&empty_bar[(c - 1) % kStages]); }
+  }
+  ptx::wgmma_wait<0>();
+  __syncwarp();
+  if (lane == 0) ptx::mbar_arrive(&empty_bar[(n_chunks - 1) % kStages]);
+  ptx::named_bar_sync(1, kPsEpiThreads);              // every consumer is done with the ring (and s_col is staged)
+  float* const tile = acc + 64 * g * Cfg::kAccPitch;
+#pragma unroll
+  for (int l = 0; l < P; ++l) {
+    ptx::acc_store<N>(tile + l * N, Cfg::kAccPitch, d[l], threadIdx.x & 127);
+    if constexpr (HAS_RES) ptx::acc_store<N>(tile + P * N + l * N, Cfg::kAccPitch, d2[l], threadIdx.x & 127);
+  }
+  ptx::named_bar_sync(1, kPsEpiThreads);              // the accumulator tile is complete
+}
 
 // TF32: fp32 activations / weights read as TF32; KC stays the row width in bf16-equivalents (row bytes / 2), see conv_tc.cuh
 template <int KC, int N, int P, bool HAS_RES, bool TF32>
@@ -162,61 +259,10 @@ conv_ps_kernel(const __grid_constant__ ConvPsParams p, const int* __restrict__ i
         s_col[4][n] = (HAS_RES && p.res_bias) ? __ldg(p.res_bias + c) : 0.f;
       }
     }
-    // ---- MMA: warpgroup g accumulates trajectories [64 g, 64 g + 64); D[l'] in registers, shortcut D2[l] next to them
-    {
-      const int g = warp >> 2;
-      float d[P][N / 2];
-      float d2[HAS_RES ? P : 1][N / 2];
-#pragma unroll
-      for (int l = 0; l < P; ++l)
-#pragma unroll
-        for (int i = 0; i < N / 2; ++i) { d[l][i] = 0.f; d2[HAS_RES ? l : 0][i] = 0.f; }
-      for (int c = 0; c < n_chunks; ++c) {
-        const int s = c % kStages;
-        ptx::mbar_wait(&full_bar[s], (c / kStages) & 1);
-        if (c == 0 && threadIdx.x == 0) CDS_TRACE(9, clock64());
-        const uint32_t sa = smem_base + s * Cfg::kStageBytes + (uint32_t)(g * 64 * Cfg::kRowBytes);
-        const uint32_t sb = smem_base + s * Cfg::kStageBytes + P * Cfg::kATile;
-        ptx::wgmma_fence();
-        if (!HAS_RES || c < n_main) {
-          // input position l feeds output position l' through tap j = l - l' + pad, whose W tile sits in slot taps-1-j
-#pragma unroll
-          for (int l = 0; l < P; ++l) {
-            const uint64_t da = ptx::make_kmajor_desc<Cfg::kRowBytes>(sa + l * Cfg::kATile);
-#pragma unroll
-            for (int lp = 0; lp < P; ++lp) {
-              const int j = l - lp + p.pad;
-              if (j < 0 || j >= p.taps) continue;
-              const uint64_t db = ptx::make_kmajor_desc<Cfg::kRowBytes>(sb + (p.taps - 1 - j) * Cfg::kBTile);
-#pragma unroll
-              for (int k = 0; k < KC / 16; ++k) ptx::Wgmma<N, TF32>::mma(d[lp], da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), 1u);
-            }
-          }
-        } else if constexpr (HAS_RES) {
-          const uint64_t db = ptx::make_kmajor_desc<Cfg::kRowBytes>(sb);
-#pragma unroll
-          for (int l = 0; l < P; ++l) {
-            const uint64_t da = ptx::make_kmajor_desc<Cfg::kRowBytes>(sa + l * Cfg::kATile);
-#pragma unroll
-            for (int k = 0; k < KC / 16; ++k) ptx::Wgmma<N, TF32>::mma(d2[l], da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), 1u);
-          }
-        }
-        ptx::wgmma_commit();
-        ptx::wgmma_wait<1>();                         // the previous chunk's MMAs are complete: its stage is free
-        if (c > 0) { __syncwarp(); if (lane == 0) ptx::mbar_arrive(&empty_bar[(c - 1) % kStages]); }
-      }
-      ptx::wgmma_wait<0>();
-      __syncwarp();
-      if (lane == 0) ptx::mbar_arrive(&empty_bar[(n_chunks - 1) % kStages]);
-      ptx::named_bar_sync(1, kPsEpiThreads);          // every consumer is done with the ring (and s_col is staged)
-      float* const tile = acc + 64 * g * Cfg::kAccPitch;
-#pragma unroll
-      for (int l = 0; l < P; ++l) {
-        ptx::acc_store<N>(tile + l * N, Cfg::kAccPitch, d[l], threadIdx.x & 127);
-        if constexpr (HAS_RES) ptx::acc_store<N>(tile + P * N + l * N, Cfg::kAccPitch, d2[l], threadIdx.x & 127);
-      }
-      ptx::named_bar_sync(1, kPsEpiThreads);          // the accumulator tile is complete
-    }
+    // ---- MMA, with the span of every input position a compile-time constant (conv_ps_eligible: taps 1, 3 or 5)
+    if (p.taps == 5) conv_ps_mma<5, KC, N, P, HAS_RES, TF32>(p, full_bar, empty_bar, smem_base, acc);
+    else if (p.taps == 3) conv_ps_mma<3, KC, N, P, HAS_RES, TF32>(p, full_bar, empty_bar, smem_base, acc);
+    else conv_ps_mma<1, KC, N, P, HAS_RES, TF32>(p, full_bar, empty_bar, smem_base, acc);
     // ===================================== epilogue =====================================
     // thread = one trajectory (accumulator row) x NH = N/2 columns (ONE GroupNorm group) x all P positions
     constexpr int NH = N / 2;
@@ -406,7 +452,7 @@ inline bool conv_ps_prepare(const cds_conv_op& c, ConvPsLaunch* out) {
     uint32_t b2[2] = {(uint32_t)ke, (uint32_t)L.n};
     if (!encode_act_map(&p.tm_b2, c.res_w, 2, d2, s2, b2, kc, tf32)) return false;
   }
-  p.batch = c.batch; p.C_out = c.C_out; p.taps = c.taps; p.pad = c.pad;
+  p.batch = c.batch; p.C_out = c.C_out; p.taps = c.taps;
   p.kchunks = c.C_in / ke; p.kchunks2 = L.has_res ? c.res_C / ke : 0;
   p.n_tiles = c.C_out / L.n;
   p.in_batch_mod = c.in_batch_mod; p.res_batch_mod = c.res_batch_mod;
