@@ -1,9 +1,10 @@
-"""TEST INFRASTRUCTURE: torch fp64 semantics of the classifier-guidance operators (include/cds.h: CDS_OP_GN, CDS_OP_GN_BWD,
-CDS_OP_GUIDE), with the stores of their output dtypes.  ``run_program`` / ``Handle`` extend tests/grad_ref.py's interpreter
-(which extends tests/emulator.py's) with them; the GPU parity tests compare the kernels against the same functions."""
+"""TEST INFRASTRUCTURE: fp64 semantics of the classifier operators (include/cds.h: CDS_OP_GN, CDS_OP_GN_BWD, CDS_OP_GUIDE,
+CDS_OP_HEAD_GRAD, csrc/classifier.cuh) and the error bounds of their kernels.  tests/emulator.py runs them on a program's
+descriptors; the GPU parity tests and tests/program_audit.py compare the kernels against the same functions.  Plus the
+classifiers of tests/golden/classifier.npz and the lowered input gradient of either classifier."""
+import numpy as np
 import torch
 
-import emulator
 import grad_ref
 import opref
 from cleandiffuser_b200.engine import cabi
@@ -45,6 +46,13 @@ def gn_bwd(h, gamma, beta, dout, groups, eps, act=cabi.ACT_MISH):
     m1 = dg.mean(dim=(1, 3), keepdim=True)
     m2 = (dg * xg).mean(dim=(1, 3), keepdim=True)
     return (rstd * (dg - m1 - xg * m2)).reshape(B, L, C)
+
+
+def head_grad(h, w, b, scale, act_kind=cabi.ACT_SILU):
+    """CDS_OP_HEAD_GRAD in fp64 (numpy) -> (z (rows,), seed (rows,)): z = act(h) . w + b, seed = d scale tanh(z/scale) / dz"""
+    z = grad_ref.act(act_kind, h) @ np.asarray(w, np.float64).reshape(-1) + float(np.asarray(b).reshape(-1)[0])
+    y = np.tanh(z / scale)
+    return z, 1.0 - y * y
 
 
 # ---------------------------------------------------------------- error bounds of csrc/classifier.cuh (u = 2^-24)
@@ -135,6 +143,21 @@ def gn_bwd_bound(h, gamma, beta, dout, groups, eps, ref, act=cabi.ACT_MISH, dh_d
     return e + (k / 2 + 5) * U32 * ref.abs() + _store_term(ref, dh_dtype)
 
 
+def head_grad_bound(h, w, b, scale, act_kind=cabi.ACT_SILU):
+    """Per-row bound on |CDS_OP_HEAD_GRAD seed - head_grad(...)|.  z: each lane sums ceil(K/32) fma terms in order, then a
+    5-level butterfly and the bias add, so (ceil(K/32) + 6) u sum|act(h) w| + u |b|, plus the fp32 SiLU's silu_bound(h) |w|.
+    seed(z) = 1 - tanh(z/scale)^2 has |d seed / d z| <= 0.77 / scale (max of 2 y (1 - y^2)).  The evaluation: z / scale and
+    tanhf (2 ulp) put 4 u |y| on y, 1 - y*y then carries 2 |y| 4 u |y| + 2 u and the product and quotient with scale 2 u: 12 u
+    absolute covers it."""
+    h = np.asarray(h, np.float64)
+    w = np.abs(np.asarray(w, np.float64).reshape(-1))
+    K = h.shape[1]
+    e_z = (-(-K // 32) + 6) * U32 * (np.abs(grad_ref.act(act_kind, h)) @ w) + U32 * abs(float(np.asarray(b).reshape(-1)[0]))
+    if act_kind == cabi.ACT_SILU:
+        e_z = e_z + grad_ref.silu_bound(h) @ w
+    return 0.77 / abs(scale) * e_z + 12 * U32
+
+
 # the classifiers of the reference's guided pipelines (diffuser / adaptdiffuser / veteran on D4RL): HalfJannerUNet1d keyword
 # arguments, and the observation part of x (the rest is the action)
 PIPELINES = {"hopper": dict(horizon=32, in_dim=14), "walker": dict(horizon=32, in_dim=23),
@@ -143,70 +166,7 @@ PIPELINES = {"hopper": dict(horizon=32, in_dim=14), "walker": dict(horizon=32, i
 OBS_DIM = {"hopper": 11, "walker": 17, "halfcheetah": 17, "antmaze": 29, "kitchen": 60}
 
 
-# ---------------------------------------------------------------- descriptor interpreters (memory backends of tests/emulator.py)
-def run_gn(g, it, mem):
-    v = emulator.view
-    h = v(mem, g.h, (g.batch, g.L, g.C), (g.h_bstride, g.h_lstride, 1), cabi.F32)
-    vec = emulator.vec(g.vec, it, g.batch, g.C, 1, mem)
-    res = v(mem, g.res, (g.batch, g.L, g.C), (g.res_bstride, g.res_lstride, 1), cabi.F32) if g.res else None
-    y = gn(h, v(mem, g.gamma, (g.C,), (1,), cabi.F32), v(mem, g.beta, (g.C,), (1,), cabi.F32), g.groups, g.eps, g.act, vec, res)
-    out = v(mem, g.out, (g.batch, g.L, g.C), (g.out_bstride, g.out_lstride, 1), cabi.F32)
-    out.copy_(opref.store(y, g.out_dtype))
-
-
-def run_gn_bwd(g, it, mem):
-    v = emulator.view
-    h = v(mem, g.h, (g.batch, g.L, g.C), (g.h_bstride, g.h_lstride, 1), cabi.F32)
-    dout = v(mem, g.dout, (g.batch, g.L, g.C), (g.dout_bstride, g.dout_lstride, 1), cabi.F32)
-    y = gn_bwd(h, v(mem, g.gamma, (g.C,), (1,), cabi.F32), v(mem, g.beta, (g.C,), (1,), cabi.F32), dout, g.groups, g.eps, g.act)
-    out = v(mem, g.dh, (g.batch, g.L, g.C), (g.dh_bstride, g.dh_lstride, 1), cabi.F32)
-    out.copy_(opref.store(y, g.dh_dtype))
-
-
-def run_guide(q, it, mem):
-    """fp32 multiply, then fp32 add: the kernel's exact arithmetic"""
-    v = emulator.view
-    s = v(mem, q.s + 4 * it, (1,), (1,), cabi.F32)[0]
-    pred = v(mem, q.pred, (q.batch, q.L, q.C), (q.L * q.C, q.C, 1), cabi.F32)
-    g = v(mem, q.g, (q.batch, q.L, q.C), (q.g_bstride, q.g_lstride, 1), cabi.F32)
-    pred.copy_(pred + s * g)
-
-
-_CG_OPS = {cabi.OP_GN: (run_gn, "gn"), cabi.OP_GN_BWD: (run_gn_bwd, "gn_bwd"), cabi.OP_GUIDE: (run_guide, "guide")}
-
-
-def run_program(ops, n_iters, first=0, mem=emulator.HOST):
-    """tests/grad_ref.py's run_program for programs that also hold the classifier-guidance operators"""
-    emulator.run_program([op for op in ops if op.flags & cabi.OPF_ONCE], 0, first, mem)
-    for it in range(first, first + n_iters):
-        for op in ops:
-            if op.flags & cabi.OPF_ONCE:
-                continue
-            if op.kind in _CG_OPS:
-                fn, field = _CG_OPS[op.kind]
-                fn(getattr(op.u, field), it, mem)
-            else:
-                grad_ref.run_program([op], 1, it, mem)
-
-
-class Handle(emulator.Handle):
-    """emulator.Handle whose interpreter also runs the backward and classifier-guidance operators"""
-
-    def run(self, first, count, stream, use_graph=True):
-        run_program(self.ops, count, first, self.mem)
-
-    def run_range(self, it, op_first, op_count, stream):
-        keep = [op for op in self.ops[op_first:op_first + op_count] if not (op.flags & cabi.OPF_ONCE)]
-        run_program(keep, 1, it, self.mem)
-
-
 # ---------------------------------------------------------------- the objects of tests/golden/classifier.npz
-def golden():
-    import os
-    import numpy as np
-    return np.load(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "classifier.npz"), allow_pickle=False)
-
-
 def make_classifier(kw, seed, device="cpu"):
     """this package's CumRewClassifier over HalfJannerUNet1d with the golden generator's synthetic weights"""
     from cleandiffuser_b200.classifier import CumRewClassifier
@@ -235,10 +195,6 @@ def make_sample_agent(name, device="cpu", classifier=None):
     return agent, prior.to(device), kw
 
 
-def tape_of(g, name):
-    return [g[f"sample/{name}/z{j}"] for j in range(int(g[f"sample/{name}/n_draws"]))]
-
-
 class Fp64Time(torch.nn.Module):
     """the timestep embedding computes in fp32 whatever the weights: its output widened for an fp64 copy of a network"""
 
@@ -260,23 +216,22 @@ def input_gradient_fp64(clf, x, t):
     return torch.autograd.grad(lp.sum(), xx)[0]
 
 
-def lowered_gradient(clf, x, t_all, it, math, device, handle=None):
-    """the input gradient as the lowered program computes it at iteration ``it`` (time t_all[it] for every row): through
-    ``handle(ops, n_iters, owners)`` (default: this module's interpreter) -> (rows, H, in_dim) fp32"""
-    from cleandiffuser_b200.engine.lower import Program, View, lower_half_janner_grad
-    B, Hh, Dd = x.shape
+def lowered_gradient(clf, x, t_all, it, math, device, cond=None, handle=None):
+    """the input gradient of either lowered classifier (HalfJannerUNet1d: x (rows, H, in_dim); QGPO: x (rows, act_dim)) as
+    the program computes it at iteration ``it`` (time t_all[it] for every row, classifier condition ``cond``): through
+    ``handle(ops, n_iters, owners)`` (default: tests/emulator.py's Handle) -> (fp32 gradient shaped like x, program)"""
+    import emulator
+    from cleandiffuser_b200.engine.lower import Program, View, lower_classifier_grad
+    from cleandiffuser_b200.engine.runtime import _Ctx
+    B, H, D = x.shape if x.dim() == 3 else (x.shape[0], 1, x.shape[1])
     p = Program(torch.device(device), B, len(t_all), math)
-    xb = p.buf(B, Hh, Dd)
+    xb = p.buf(*x.shape)
     xb.copy_(x)
-    g = lower_half_janner_grad(p, clf, View(xb, Hh, Dd))
-
-    class Ctx:
-        pass
-    ctx = Ctx()
-    ctx.t_all, ctx.cond_rows = t_all.to(device), None
+    g = lower_classifier_grad(p, clf, View(xb, H, D))
+    ctx = _Ctx(t_all.to(device), None, None if cond is None else cond.to(device))
     with torch.no_grad():
         for fn in p.per_call:
             fn(ctx)
-    h = (handle or (lambda ops, n, owners: Handle(ops, n, owners)))(p.ops, len(t_all), list(p.keep))
-    h.run(it, 1, 0 if device == "cpu" else torch.cuda.current_stream().cuda_stream, False)
-    return g.t.view(B, Hh, -1)[..., :Dd].clone(), p
+    (handle or emulator.Handle)(p.ops, len(t_all), list(p.keep)).run(
+        it, 1, 0 if device == "cpu" else torch.cuda.current_stream().cuda_stream, False)
+    return g.t.view(B, H, -1)[..., :D].reshape(x.shape).clone(), p

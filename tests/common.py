@@ -1,4 +1,6 @@
 """Helpers shared by the parity tests: build product modules / oracle closures for a golden case."""
+import os
+
 import numpy as np
 import torch
 
@@ -40,6 +42,11 @@ def oracle_cond_emb(spec, cond):
         sd = synth_state_dict(nc.state_dict(), seed=3)
         return onets.mlp_condition(sd, cond, torch.nn.functional.silu, 1)
     return cond * 1.
+
+
+def load_golden(name):
+    """tests/golden/<name>.npz"""
+    return np.load(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", name + ".npz"), allow_pickle=False)
 
 
 def tape_of(npz, name):

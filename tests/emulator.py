@@ -5,10 +5,12 @@ the raw pointers) and compare it with the reference goldens, so that lowering bu
 table columns, phase packing ...) are caught here without a GPU; the kernels themselves are then checked
 against the same goldens on the H100.  Never imported by the product.
 
-This is also the one decoder of a descriptor's operands: every ``*_operands`` / ``run_*`` function takes a memory backend
-``mem`` -- ``RawHost`` (raw host addresses, no bounds check) or ``Owned`` (views of the tensors that own the memory, on the
-host or the device, with every operand's extent checked against its owner).  tests/program_audit.py uses the same
-functions on the device state of a real plan.
+``OPS`` runs every operator kind; the fp64 semantics live in tests/opref.py (forward operators), tests/mha_ref.py,
+tests/grad_ref.py (backward operators of a differentiable loop) and tests/cg_ref.py (classifier operators), and this module
+is the one decoder of a descriptor's operands: every ``*_operands`` / ``run_*`` function takes ``(descriptor, iteration,
+mem)``, with a memory backend ``mem`` -- ``RawHost`` (raw host addresses, no bounds check) or ``Owned`` (views of the
+tensors that own the memory, on the host or the device, with every operand's extent checked against its owner).
+tests/program_audit.py uses the same ``*_operands`` functions on the device state of a real plan.
 """
 import bisect
 import ctypes
@@ -16,6 +18,9 @@ import ctypes
 import numpy as np
 import torch
 
+import cg_ref
+import grad_ref
+import mha_ref
 import opref
 from cleandiffuser_b200.engine import cabi
 
@@ -186,7 +191,7 @@ def run_conv(c, it, mem=HOST):
     out.copy_(opref.store(y, c.out_dtype).to(out.dtype))
 
 
-def lnmod_operands(m, mem=HOST):
+def lnmod_operands(m, it, mem=HOST):
     """(x, shift, scale, output view) of a CDS_OP_LNMOD descriptor"""
     x = view(mem, m.in_, (m.batch, m.L, m.C), (m.L * m.C, m.C, 1), cabi.F32)
     sh = view(mem, m.shift, (m.batch, m.C), (m.mod_bstride, 1), cabi.F32)
@@ -194,24 +199,47 @@ def lnmod_operands(m, mem=HOST):
     return x, sh, sc, view(mem, m.out, (m.batch, m.L, m.C), (m.L * m.C, m.C, 1), m.out_dtype)
 
 
-def run_lnmod(m, mem=HOST):
-    x, sh, sc, out = lnmod_operands(m, mem)
+def run_lnmod(m, it, mem=HOST):
+    x, sh, sc, out = lnmod_operands(m, it, mem)
     out.copy_(opref.store(opref.lnmod(x, sh, sc, m.eps), m.out_dtype).to(out.dtype))
 
 
-def attn_operands(a, mem=HOST):
+def attn_operands(a, it, mem=HOST):
     """(q|k|v view as stored, output view) of a CDS_OP_ATTN descriptor"""
     qkv = view(mem, a.qkv, (a.batch, a.L, 3 * a.C), (a.L * 3 * a.C, 3 * a.C, 1), a.qkv_dtype)
     return qkv, view(mem, a.out, (a.batch, a.L, a.C), (a.L * a.C, a.C, 1), a.out_dtype)
 
 
-def run_attn(a, mem=HOST):
+def run_attn(a, it, mem=HOST):
     """CDS_OP_ATTN: q|k|v (bf16 values widened exactly) through tests/opref.py's fp64 reference"""
-    qkv, out = attn_operands(a, mem)
+    qkv, out = attn_operands(a, it, mem)
     out.copy_(opref.store(opref.attn(qkv, a.heads, a.qkv_dtype), a.out_dtype).to(out.dtype))
 
 
-def run_cast(k, mem=HOST):
+def mha_operands(m, it, mem=HOST):
+    """(q view as stored, k|v as the fp32 sum step + sample (the kernel's adds of the widened parts), output view, whether both
+    k|v parts are present) of a CDS_OP_MHA descriptor"""
+    esize = 2 if m.in_dtype == cabi.BF16 else 4
+    q = view(mem, m.q, (m.batch, m.Lq, m.C), (m.q_bstride, m.q_lstride, 1), m.in_dtype)
+    kv = None
+    if m.kv_step:
+        kv = view(mem, m.kv_step + esize * it * m.kv_step_stride, (m.Lk, 2 * m.C), (m.kv_step_lstride, 1),
+                  m.in_dtype).float()[None].expand(m.batch, m.Lk, 2 * m.C)
+    if m.kv_sample:
+        s = view(mem, m.kv_sample, (m.batch, m.Lk, 2 * m.C), (m.kv_sample_bstride, m.kv_sample_lstride, 1),
+                 m.in_dtype).float()
+        kv = s if kv is None else s + kv
+    out = view(mem, m.out, (m.batch, m.Lq, m.C), (m.out_bstride, m.out_lstride, 1), m.out_dtype)
+    return q, kv, out, bool(m.kv_step and m.kv_sample)
+
+
+def run_mha(m, it, mem=HOST):
+    """CDS_OP_MHA: q and the k|v sum through tests/mha_ref.py"""
+    q, kv, out, _ = mha_operands(m, it, mem)
+    out.copy_(opref.store(mha_ref.mha(q, kv, m.heads, m.diag if m.masked else None), m.out_dtype).to(out.dtype))
+
+
+def run_cast(k, it, mem=HOST):
     x = view(mem, k.in_, (k.batch, k.L, k.C_in), (k.L * k.C_in, k.C_in, 1), cabi.F32)
     y = torch.zeros((k.batch, k.L, k.C_out), dtype=torch.float32, device=x.device)
     y[..., :k.C_in] = x
@@ -306,30 +334,154 @@ def run_update(u, it, mem=HOST):
         _store(u.x_cast, (rows, u.cast_C_in), (u.cast_C_out, 1), u.x_cast_dtype, x.reshape(rows, u.cast_C_in), mem)
 
 
+# ---------------------------------------------------------------- backward operators (tests/grad_ref.py)
+# Their operands are float32 numpy views (grad_ref's semantics are numpy code); _f32 stores an fp64 result
+def _f32(v):
+    return np.asarray(v, np.float64).astype(np.float32)
+
+
+def stash_operands(s, it, mem=HOST):
+    """(src, slot of iteration ``it`` or None, activation output or None) of a CDS_OP_STASH descriptor"""
+    src = _arr(s.src, (s.n,), (1,), mem)
+    slot = _arr(s.dst + 4 * it * s.dst_iter_stride, (s.n,), (1,), mem) if s.dst else None
+    return src, slot, _arr(s.act_out, (s.n,), (1,), mem)
+
+
+def run_stash(s, it, mem=HOST):
+    src, slot, act_out = stash_operands(s, it, mem)
+    if slot is not None:
+        slot[...] = src
+    if act_out is not None:
+        act_out[...] = _f32(grad_ref.act(s.act, src))
+
+
+def update_bwd_operands(u, it, mem=HOST):
+    """(gx (read, then written), x, pred, keyword arguments of grad_ref.update_bwd, gpred view) of a CDS_OP_UPDATE_BWD
+    descriptor"""
+    shape, st = (u.batch, u.row), (u.row, 1)
+    row = _arr(u.coef + 4 * it * u.coef_iter_stride, (cabi.ROW_FLOATS,), (1,), mem).astype(np.float64)
+    kw = dict(alpha=row[0], sigma=row[1], k0=row[2], k1=row[3], kind=int(row[7]), predict_noise=bool(u.predict_noise),
+              **{k: _arr(getattr(u, k), (u.row,), (1,), mem) for k in ("mask", "x_min", "x_max")})
+    x = _arr(u.x + 4 * it * u.x_iter_stride, shape, st, mem)
+    pr = _arr(u.pred + 4 * it * u.pred_iter_stride, shape, st, mem)
+    return _arr(u.gx, shape, st, mem), x, pr, kw, _arr(u.gpred, shape, st, mem)
+
+
+def run_update_bwd(u, it, mem=HOST):
+    gx, x, pr, kw, gpred = update_bwd_operands(u, it, mem)
+    gp, dx = grad_ref.update_bwd(gx, x, pr, **kw)
+    gpred[...] = _f32(gp)
+    gx[...] = _f32(dx)
+
+
+def dgrad_operands(d, it, mem=HOST):
+    """(dz, W, stashed pre-activation z of iteration ``it`` or None, output view, out_sum view or None) of a CDS_OP_DGRAD
+    descriptor"""
+    dz = _arr(d.dz, (d.rows, d.N), (d.ldz, 1), mem)
+    w = _arr(d.w, (d.N, d.K), (d.ldw, 1), mem)
+    z = _arr(d.z + 4 * it * d.z_iter_stride, (d.rows, d.K), (d.K, 1), mem) if d.z else None
+    return dz, w, z, _arr(d.out, (d.rows, d.K), (d.ldo, 1), mem), _arr(d.out_sum, (d.rows, d.K), (d.K, 1), mem)
+
+
+def run_dgrad(d, it, mem=HOST):
+    dz, w, z, out, out_sum = dgrad_operands(d, it, mem)
+    y = grad_ref.dgrad(dz, w, z, d.act)
+    out[...] = _f32(out.astype(np.float64) + y) if d.accumulate else _f32(y)
+    if out_sum is not None:
+        out_sum[...] = _f32(out_sum.astype(np.float64) + y)
+
+
+def wgrad_operands(g, it, mem=HOST):
+    """(dz, h of iteration ``it``, dw view, bias-gradient row of iteration ``it`` or None) of a CDS_OP_WGRAD descriptor"""
+    dz = _arr(g.dz, (g.rows, g.N), (g.ldz, 1), mem)
+    h = _arr(g.h + 4 * it * g.h_iter_stride, (g.rows, g.K), (g.ldh, 1), mem)
+    db = _arr(g.db + 4 * it * g.db_iter_stride, (g.N,), (1,), mem) if g.db else None
+    return dz, h, _arr(g.dw, (g.N, g.K), (g.lddw, 1), mem), db
+
+
+def run_wgrad(g, it, mem=HOST):
+    dz, h, dw, db = wgrad_operands(g, it, mem)
+    gw, gb = grad_ref.wgrad(dz, h, g.act)
+    dw[...] = _f32(dw.astype(np.float64) + gw) if g.accumulate else _f32(gw)
+    if db is not None:
+        db[...] = _f32(db.astype(np.float64) + gb) if g.accumulate else _f32(gb)
+
+
+# ---------------------------------------------------------------- classifier operators (tests/cg_ref.py)
+def gn_operands(g, it, mem=HOST):
+    """(h, gamma, beta, vec or None, res or None, output view) of a CDS_OP_GN descriptor"""
+    act = (g.batch, g.L, g.C)
+    h = view(mem, g.h, act, (g.h_bstride, g.h_lstride, 1), cabi.F32)
+    gamma, beta = view(mem, g.gamma, (g.C,), (1,), cabi.F32), view(mem, g.beta, (g.C,), (1,), cabi.F32)
+    res = view(mem, g.res, act, (g.res_bstride, g.res_lstride, 1), cabi.F32)
+    out = view(mem, g.out, act, (g.out_bstride, g.out_lstride, 1), cabi.F32)
+    return h, gamma, beta, vec(g.vec, it, g.batch, g.C, 1, mem), res, out
+
+
+def run_gn(g, it, mem=HOST):
+    h, gamma, beta, v, res, out = gn_operands(g, it, mem)
+    out.copy_(opref.store(cg_ref.gn(h, gamma, beta, g.groups, g.eps, g.act, v, res), g.out_dtype))
+
+
+def gn_bwd_operands(g, it, mem=HOST):
+    """(h, gamma, beta, dout, dh view) of a CDS_OP_GN_BWD descriptor"""
+    act = (g.batch, g.L, g.C)
+    h = view(mem, g.h, act, (g.h_bstride, g.h_lstride, 1), cabi.F32)
+    gamma, beta = view(mem, g.gamma, (g.C,), (1,), cabi.F32), view(mem, g.beta, (g.C,), (1,), cabi.F32)
+    dout = view(mem, g.dout, act, (g.dout_bstride, g.dout_lstride, 1), cabi.F32)
+    return h, gamma, beta, dout, view(mem, g.dh, act, (g.dh_bstride, g.dh_lstride, 1), cabi.F32)
+
+
+def run_gn_bwd(g, it, mem=HOST):
+    h, gamma, beta, dout, dh = gn_bwd_operands(g, it, mem)
+    dh.copy_(opref.store(cg_ref.gn_bwd(h, gamma, beta, dout, g.groups, g.eps, g.act), g.dh_dtype))
+
+
+def guide_operands(q, it, mem=HOST):
+    """(guidance scale of iteration ``it``, pred view (read and written), gradient) of a CDS_OP_GUIDE descriptor"""
+    s = view(mem, q.s + 4 * it, (1,), (1,), cabi.F32)[0]
+    pred = view(mem, q.pred, (q.batch, q.L, q.C), (q.L * q.C, q.C, 1), cabi.F32)
+    return s, pred, view(mem, q.g, (q.batch, q.L, q.C), (q.g_bstride, q.g_lstride, 1), cabi.F32)
+
+
+def run_guide(q, it, mem=HOST):
+    """fp32 multiply, then fp32 add: the kernel's exact arithmetic"""
+    s, pred, g = guide_operands(q, it, mem)
+    pred.copy_(pred + s * g)
+
+
+def head_grad_operands(q, it, mem=HOST):
+    """(h, w, b, seed view) of a CDS_OP_HEAD_GRAD descriptor, float32 numpy"""
+    h = _arr(q.h, (q.rows, q.K), (q.ldh, 1), mem)
+    return h, _arr(q.w, (q.K,), (1,), mem), _arr(q.b, (1,), (1,), mem), _arr(q.seed, (q.rows,), (1,), mem)
+
+
+def run_head_grad(q, it, mem=HOST):
+    h, w, b, seed = head_grad_operands(q, it, mem)
+    seed[...] = _f32(cg_ref.head_grad(h, w, b, q.scale, q.act)[1])
+
+
+# ---------------------------------------------------------------- programs
+# every operator kind: (its field of the cds_op union, its runner)
+OPS = {cabi.OP_CONV: ("conv", run_conv), cabi.OP_UPDATE: ("update", run_update), cabi.OP_LNMOD: ("lnmod", run_lnmod),
+       cabi.OP_ATTN: ("attn", run_attn), cabi.OP_PREP: ("prep", run_prep), cabi.OP_CAST: ("cast", run_cast),
+       cabi.OP_MHA: ("mha", run_mha), cabi.OP_STASH: ("stash", run_stash), cabi.OP_UPDATE_BWD: ("update_bwd", run_update_bwd),
+       cabi.OP_DGRAD: ("dgrad", run_dgrad), cabi.OP_WGRAD: ("wgrad", run_wgrad), cabi.OP_GN: ("gn", run_gn),
+       cabi.OP_GN_BWD: ("gn_bwd", run_gn_bwd), cabi.OP_GUIDE: ("guide", run_guide),
+       cabi.OP_HEAD_GRAD: ("head_grad", run_head_grad)}
+
+
 def run_program(ops, n_iters, first=0, mem=HOST):
     with np.errstate(over="ignore", invalid="ignore", divide="ignore"):
         for op in ops:                       # CDS_OPF_ONCE operators: once per run, before the first iteration
             if op.flags & cabi.OPF_ONCE:
                 assert op.kind == cabi.OP_CAST, op.kind
-                run_cast(op.u.cast, mem)
+                run_cast(op.u.cast, first, mem)
         for it in range(first, first + n_iters):
             for op in ops:
-                if op.flags & cabi.OPF_ONCE:
-                    continue
-                if op.kind == cabi.OP_CONV:
-                    run_conv(op.u.conv, it, mem)
-                elif op.kind == cabi.OP_UPDATE:
-                    run_update(op.u.update, it, mem)
-                elif op.kind == cabi.OP_LNMOD:
-                    run_lnmod(op.u.lnmod, mem)
-                elif op.kind == cabi.OP_ATTN:
-                    run_attn(op.u.attn, mem)
-                elif op.kind == cabi.OP_PREP:
-                    run_prep(op.u.prep, it, mem)
-                elif op.kind == cabi.OP_CAST:
-                    run_cast(op.u.cast, mem)
-                else:
-                    raise ValueError(op.kind)
+                if not op.flags & cabi.OPF_ONCE:
+                    field, run = OPS[op.kind]
+                    run(getattr(op.u, field), it, mem)
 
 
 class Handle:
@@ -373,3 +525,12 @@ def record_owners(monkeypatch):
     monkeypatch.setattr(runtime, "lower_denoiser", recording_lower)
     return lambda: [t for p in progs for t in p.keep if isinstance(t, torch.Tensor)] + \
         [t for n in nets for t in (*n.parameters(), *n.buffers())]
+
+
+def emulate(monkeypatch):
+    """For the rest of a test, the engine runs its programs on this interpreter: every device is usable, and each plan's
+    handle is a ``Handle`` over the tensors the lowering records (``record_owners``), so every operand is bounds-checked"""
+    from cleandiffuser_b200.engine import runtime
+    monkeypatch.setattr(runtime, "_device_ok", lambda device: True)
+    owners = record_owners(monkeypatch)
+    monkeypatch.setattr(runtime, "_make_handle", lambda device, ops, n: Handle(ops, n, owners()))

@@ -1,16 +1,18 @@
 """TEST INFRASTRUCTURE: numpy semantics of the backward operators of a differentiable reverse loop (include/cds.h:
-CDS_OP_STASH, CDS_OP_UPDATE_BWD, CDS_OP_DGRAD, CDS_OP_WGRAD), in fp64 with fp32 stores, like tests/opref.py does for the
-forward operators.  ``run_program`` / ``Handle`` extend tests/emulator.py's interpreter with them (every other operator kind
-is run by the emulator itself); the GPU parity tests compare the kernels against the same functions."""
+CDS_OP_STASH, CDS_OP_UPDATE_BWD, CDS_OP_DGRAD, CDS_OP_WGRAD, csrc/grad.cuh) for every activation they accept (NONE, MISH,
+SILU), in fp64 with fp32 stores, like tests/opref.py does for the forward operators, and the error bounds of their kernels.
+tests/emulator.py runs them on a program's descriptors; the GPU parity tests and tests/program_audit.py compare the kernels
+against the same functions."""
 import numpy as np
+import torch
 
-import emulator
+import opref
 from cleandiffuser_b200.engine import cabi
 
 
-def mish(x):
-    x = np.asarray(x, np.float64)
-    return x * np.tanh(np.where(x > 20, x, np.log1p(np.exp(np.minimum(x, 20)))))
+def act(kind, x):
+    """tests/opref.py's activation ``kind`` of a numpy array, in fp64"""
+    return opref.act(kind, torch.from_numpy(np.array(x, np.float64))).numpy()
 
 
 def mish_grad(x):
@@ -21,8 +23,11 @@ def mish_grad(x):
     return tsp + x * sig * (1.0 - tsp * tsp)
 
 
-def act(kind, x):
-    return mish(x) if kind == cabi.ACT_MISH else np.asarray(x, np.float64)
+def silu_grad(x):
+    """d/dx silu(x) (ATen's silu_backward: sig (1 + x (1 - sig)))"""
+    x = np.asarray(x, np.float64)
+    sig = 1.0 / (1.0 + np.exp(-x))
+    return sig * (1.0 + x * (1.0 - sig))
 
 
 def update_bwd(g, x, pr, *, alpha, sigma, k0, k1, kind, predict_noise, mask=None, x_min=None, x_max=None):
@@ -78,8 +83,8 @@ def update_bwd(g, x, pr, *, alpha, sigma, k0, k1, kind, predict_noise, mask=None
 def dgrad(dz, w, z=None, act_kind=cabi.ACT_NONE):
     """(dz W) * act'(z) in fp64"""
     y = np.asarray(dz, np.float64) @ np.asarray(w, np.float64)
-    if act_kind == cabi.ACT_MISH:
-        y = y * mish_grad(z)
+    if act_kind != cabi.ACT_NONE:
+        y = y * ACT_GRAD[act_kind][0](z)
     return y
 
 
@@ -94,6 +99,7 @@ def wgrad(dz, h, act_kind=cabi.ACT_NONE):
 # |kernel - fp64 reference|.  The operator tests (tests/test_grad_sampling_gpu.py) and the program audit
 # (tests/program_audit.py) both apply them.
 U32 = 2.0 ** -24
+TINY = 1e-35          # silu(z) for z < -88, where the fp32 1 + expf(-z) overflows and the kernel returns -0
 
 
 def mish_bound(z):
@@ -109,6 +115,24 @@ def mish_grad_bound(z):
     return (8 + 8 * abs(z)) * U32
 
 
+def silu_bound(z):
+    """fp32 silu(z) = z / (1 + expf(-z)): expf within 2 ulp (4 u), the add and the division u each: 6 u relative, 8 u allowed;
+    TINY covers the overflow of 1 + expf(-z) below z = -88"""
+    return 8 * U32 * np.abs(act(cabi.ACT_SILU, z)) + TINY
+
+
+def silu_grad_bound(z):
+    """fp32 silu'(z): sig carries 6 u relative (as in silu_bound), so 1 - sig an absolute 7 u (sig <= 1), z (1 - sig) 7 u |z| plus
+    its rounding, 1 + that and the product with sig a rounding each: (12 + 12 |z|) u covers them with the margin of 2x on the
+    roundings that the other bounds of the audit keep"""
+    return (12 + 12 * np.abs(np.asarray(z, np.float64))) * U32
+
+
+# the activations the backward kernels fuse: their fp32 evaluation's bound, and their derivative with its fp32 bound
+ACT_BOUND = {cabi.ACT_MISH: mish_bound, cabi.ACT_SILU: silu_bound}
+ACT_GRAD = {cabi.ACT_MISH: (mish_grad, mish_grad_bound), cabi.ACT_SILU: (silu_grad, silu_grad_bound)}
+
+
 def update_bwd_bound(g, alpha, sigma, k0, k1):
     """CDS_OP_UPDATE_BWD: a handful of fp32 operations per element, each within u of its exact result, on terms of size at
     most |g| (|k0| + |k1|) (1 + 1/alpha + 1/sigma)^2; 16 u of that (the clip decisions are exact: grad_ref.update_bwd takes
@@ -117,18 +141,20 @@ def update_bwd_bound(g, alpha, sigma, k0, k1):
 
 
 def dgrad_bound(dz, w, z=None, act_kind=cabi.ACT_NONE, before=None):
-    """CDS_OP_DGRAD, out [+]= (dz W) Mish'(z): each output is one thread's fma chain over N, so the dot-product bound
-    (N + 4) u |dz||W|, times |Mish'(z)| when the derivative is fused; the fp32 Mish' adds |dz W| mish_grad_bound(z).  An
-    accumulating store (``before``: the output before the launch, for accumulate = 1 and for out_sum) adds 2 u (|before| + |y|)."""
+    """CDS_OP_DGRAD, out [+]= (dz W) act'(z): each output is one thread's fma chain over N, so the dot-product bound
+    (N + 4) u |dz||W|, times |act'(z)| when the derivative is fused; the fp32 act' adds |dz W| times its bound (ACT_GRAD).
+    An accumulating store (``before``: the output before the launch, for accumulate = 1 and for out_sum) adds
+    2 u (|before| + |y|)."""
     dz, w = np.asarray(dz, np.float64), np.asarray(w, np.float64)
     dzw = dz @ w
     mag, y = np.abs(dz) @ np.abs(w), dzw
     bound = 0.0
-    if act_kind == cabi.ACT_MISH:
+    if act_kind != cabi.ACT_NONE:
+        grad, grad_bound = ACT_GRAD[act_kind]
         z = np.asarray(z, np.float64)
-        mg = mish_grad(z)
-        mag, y = mag * np.abs(mg), dzw * mg
-        bound = np.abs(dzw) * mish_grad_bound(z)
+        g = grad(z)
+        mag, y = mag * np.abs(g), dzw * g
+        bound = np.abs(dzw) * grad_bound(z)
     bound = bound + (dz.shape[1] + 4) * U32 * mag
     if before is not None:
         bound = bound + 2 * U32 * (np.abs(np.asarray(before, np.float64)) + np.abs(y))
@@ -149,54 +175,6 @@ def wgrad_bound(dz, h, act_kind=cabi.ACT_NONE, dw_before=None, db_before=None):
     if db_before is not None:
         bb = bb + 2 * U32 * (np.abs(np.asarray(db_before, np.float64)) + np.abs(gb))
     return bw, bb
-
-
-# ---------------------------------------------------------------- descriptor interpreters (memory backends of tests/emulator.py)
-def _f32(v):
-    return np.asarray(v, np.float64).astype(np.float32)
-
-
-def run_stash(s, it, arr):
-    src = arr(s.src, (s.n,), (1,))
-    arr(s.dst + 4 * it * s.dst_iter_stride, (s.n,), (1,))[...] = src
-    if s.act_out:
-        arr(s.act_out, (s.n,), (1,))[...] = _f32(act(s.act, src))
-
-
-def run_update_bwd(u, it, arr):
-    row = arr(u.coef + 4 * it * u.coef_iter_stride, (cabi.ROW_FLOATS,), (1,)).astype(np.float64)
-    shape, st = (u.batch, u.row), (u.row, 1)
-    gx = arr(u.gx, shape, st)
-    x = arr(u.x + 4 * it * u.x_iter_stride, shape, st)
-    pr = arr(u.pred + 4 * it * u.pred_iter_stride, shape, st)
-    vec = lambda p: None if not p else arr(p, (u.row,), (1,))          # noqa: E731
-    gp, dx = update_bwd(gx, x, pr, alpha=row[0], sigma=row[1], k0=row[2], k1=row[3], kind=int(row[7]),
-                        predict_noise=bool(u.predict_noise), mask=vec(u.mask), x_min=vec(u.x_min), x_max=vec(u.x_max))
-    arr(u.gpred, shape, st)[...] = _f32(gp)
-    gx[...] = _f32(dx)
-
-
-def run_dgrad(d, it, arr):
-    dz = arr(d.dz, (d.rows, d.N), (d.ldz, 1))
-    w = arr(d.w, (d.N, d.K), (d.ldw, 1))
-    z = arr(d.z + 4 * it * d.z_iter_stride, (d.rows, d.K), (d.K, 1)) if d.z else None
-    y = dgrad(dz, w, z, d.act)
-    out = arr(d.out, (d.rows, d.K), (d.ldo, 1))
-    out[...] = _f32(out.astype(np.float64) + y) if d.accumulate else _f32(y)
-    if d.out_sum:
-        s = arr(d.out_sum, (d.rows, d.K), (d.K, 1))
-        s[...] = _f32(s.astype(np.float64) + y)
-
-
-def run_wgrad(g, it, arr):
-    dz = arr(g.dz, (g.rows, g.N), (g.ldz, 1))
-    h = arr(g.h + 4 * it * g.h_iter_stride, (g.rows, g.K), (g.ldh, 1))
-    dw, db = wgrad(dz, h, g.act)
-    out = arr(g.dw, (g.N, g.K), (g.lddw, 1))
-    out[...] = _f32(out.astype(np.float64) + dw) if g.accumulate else _f32(dw)
-    if g.db:
-        b = arr(g.db + 4 * it * g.db_iter_stride, (g.N,), (1,))
-        b[...] = _f32(b.astype(np.float64) + db) if g.accumulate else _f32(db)
 
 
 # ---------------------------------------------------------------- differentiable calls audited operator by operator
@@ -228,36 +206,3 @@ def grad_agent(case, device):
         mask[0] = 1.
         agent = ContinuousDiffusionSDE(net, IdentityCondition(dropout=0.0), fix_mask=mask, **kw)
     return agent, dict(solver=spec["solver"], sample_steps=5, use_ema=False, w_cfg=1.0, requires_grad=True)
-
-
-# ---------------------------------------------------------------- programs with backward operators
-_GRAD_OPS = {cabi.OP_STASH: (run_stash, "stash"), cabi.OP_UPDATE_BWD: (run_update_bwd, "update_bwd"),
-             cabi.OP_DGRAD: (run_dgrad, "dgrad"), cabi.OP_WGRAD: (run_wgrad, "wgrad")}
-
-
-def run_program(ops, n_iters, first=0, mem=emulator.HOST):
-    """tests/emulator.py's run_program for programs that also hold backward operators: those run here, every other operator
-    through the emulator (one operator at a time, so that program order is kept)."""
-    arr = lambda ptr, shape, strides: emulator._arr(ptr, shape, strides, mem)       # noqa: E731
-    with np.errstate(over="ignore", invalid="ignore", divide="ignore"):
-        emulator.run_program([op for op in ops if op.flags & cabi.OPF_ONCE], 0, first, mem)   # CDS_OPF_ONCE operators
-        for it in range(first, first + n_iters):
-            for op in ops:
-                if op.flags & cabi.OPF_ONCE:
-                    continue
-                if op.kind in _GRAD_OPS:
-                    fn, field = _GRAD_OPS[op.kind]
-                    fn(getattr(op.u, field), it, arr)
-                else:
-                    emulator.run_program([op], 1, it, mem)
-
-
-class Handle(emulator.Handle):
-    """emulator.Handle whose interpreter also runs the backward operators"""
-
-    def run(self, first, count, stream, use_graph=True):
-        run_program(self.ops, count, first, self.mem)
-
-    def run_range(self, it, op_first, op_count, stream):
-        keep = [op for op in self.ops[op_first:op_first + op_count] if not (op.flags & cabi.OPF_ONCE)]
-        run_program(keep, 1, it, self.mem)

@@ -9,9 +9,10 @@ checks:
   - its output against tests/opref.py in fp64, computed from the same state before the launch, under the derived bound of
     the operator's kernel family: conv_cases.check (+ gn_offset_atol for GroupNorm on tensor cores), attn_cases.bound,
     mha_cases.bound, the LNMOD bound of tests/test_elementwise_gpu.py; UPDATE / PREP / CAST / GUIDE and STASH's slot
-    copy bit for bit against the interpreter run on host copies of their operands; GN / GN_BWD under cg_ref.gn_bound /
-    gn_bwd_bound, STASH's Mish under grad_ref.mish_bound, UPDATE_BWD / DGRAD / WGRAD under grad_ref.update_bwd_bound /
-    dgrad_bound / wgrad_bound (accumulating outputs as before + contribution), the bounds the operator tests apply;
+    copy bit for bit against the interpreter run on host copies of their operands; GN / GN_BWD / HEAD_GRAD under
+    cg_ref.gn_bound / gn_bwd_bound / head_grad_bound, STASH's Mish or SiLU under grad_ref.ACT_BOUND, UPDATE_BWD / DGRAD /
+    WGRAD under grad_ref.update_bwd_bound / dgrad_bound / wgrad_bound (accumulating outputs as before + contribution), the
+    bounds the operator tests apply;
   - that nothing outside its declared outputs changed: every other owner keeps its fingerprint, and inside the owner of an
     output view the elements outside the view keep theirs.
 The largest error as a fraction of the bound is recorded per (program, kernel instantiation).
@@ -41,7 +42,7 @@ DT_NAME = {cabi.F32: "f32", cabi.TF32: "tf32", cabi.BF16: "bf16"}
 KIND_NAME = {cabi.OP_CONV: "conv", cabi.OP_UPDATE: "update", cabi.OP_LNMOD: "lnmod", cabi.OP_ATTN: "attn",
              cabi.OP_PREP: "prep", cabi.OP_CAST: "cast", cabi.OP_MHA: "mha", cabi.OP_STASH: "stash",
              cabi.OP_UPDATE_BWD: "update_bwd", cabi.OP_DGRAD: "dgrad", cabi.OP_WGRAD: "wgrad", cabi.OP_GN: "gn",
-             cabi.OP_GN_BWD: "gn_bwd", cabi.OP_GUIDE: "guide"}
+             cabi.OP_GN_BWD: "gn_bwd", cabi.OP_GUIDE: "guide", cabi.OP_HEAD_GRAD: "head_grad"}
 
 
 def plan_owners(plan):
@@ -60,7 +61,7 @@ def declared_outputs(op, it):
     k = op.kind
     if k == cabi.OP_STASH:
         s = op.u.stash
-        outs = [(s.dst + 4 * it * s.dst_iter_stride, (s.n,), (1,), cabi.F32)]
+        outs = [(s.dst + 4 * it * s.dst_iter_stride, (s.n,), (1,), cabi.F32)] if s.dst else []
         return outs + ([(s.act_out, (s.n,), (1,), cabi.F32)] if s.act_out else [])
     if k == cabi.OP_UPDATE_BWD:
         u = op.u.update_bwd
@@ -82,6 +83,9 @@ def declared_outputs(op, it):
     if k == cabi.OP_GUIDE:
         q = op.u.guide
         return [(q.pred, (q.batch, q.L, q.C), (q.L * q.C, q.C, 1), cabi.F32)]
+    if k == cabi.OP_HEAD_GRAD:
+        q = op.u.head_grad
+        return [(q.seed, (q.rows,), (1,), cabi.F32)]
     if k == cabi.OP_CONV:
         c = op.u.conv
         return [(c.out, (c.batch, c.L_out * c.phases, c.C_out), (c.out_bstride, c.out_lstride, 1), c.out_dtype)]
@@ -134,18 +138,23 @@ def instantiation(op):
     if op.kind == cabi.OP_GN_BWD:
         return f"gn_bwd -> {DT_NAME[op.u.gn_bwd.dh_dtype]}"
     if op.kind == cabi.OP_STASH:
-        return "stash +act" if op.u.stash.act_out else "stash"
+        s = op.u.stash
+        if s.act == cabi.ACT_SILU:
+            return "stash silu" + ("" if s.dst else " (no slot)")
+        return "stash +act" if s.act_out else "stash"
     if op.kind == cabi.OP_UPDATE_BWD:
         u = op.u.update_bwd
         return f"update_bwd {'eps' if u.predict_noise else 'x0'}{' clip' if u.x_min or u.x_max else ''}" \
             f"{' mask' if u.mask else ''}"
     if op.kind == cabi.OP_DGRAD:
         d = op.u.dgrad
-        return f"dgrad{' mish' if d.act == cabi.ACT_MISH else ''}{' +=' if d.accumulate else ''}" \
-            f"{' +out_sum' if d.out_sum else ''}"
+        act = {cabi.ACT_MISH: " mish", cabi.ACT_SILU: " silu"}.get(d.act, "")
+        return f"dgrad{act}{' +=' if d.accumulate else ''}{' +out_sum' if d.out_sum else ''}"
     if op.kind == cabi.OP_WGRAD:
         g = op.u.wgrad
         return f"wgrad{' mish' if g.act == cabi.ACT_MISH else ''}{' +bias' if g.db else ''}"
+    if op.kind == cabi.OP_HEAD_GRAD:
+        return f"head_grad{' silu' if op.u.head_grad.act == cabi.ACT_SILU else ''}"
     return KIND_NAME[op.kind]
 
 
@@ -181,8 +190,8 @@ def _frac(err, bound, finite):
 
 
 class Auditor:
-    """Audits the operator program ``ops`` run by ``handle`` (a cabi.Plan, or an emulator / mha_ref Handle over the same
-    descriptors).  ``owners``: the tensors the descriptors point into (plan_owners); ``sync``: waits for the handle's work."""
+    """Audits the operator program ``ops`` run by ``handle`` (a cabi.Plan, or an emulator.Handle over the same descriptors).
+    ``owners``: the tensors the descriptors point into (plan_owners); ``sync``: waits for the handle's work."""
 
     def __init__(self, name, ops, handle, owners, stream=0, sync=lambda: None):
         self.name, self.ops, self.handle, self.stream, self.sync = name, list(ops), handle, stream, sync
@@ -229,10 +238,11 @@ class Auditor:
         return after
 
     # ---- references (computed from the state before the launch); each returns check() -> [(frac, label)] --------------
-    def _conv(self, c, it):
+    def _conv(self, op, it):
         """The fp64 reference is computed chunk by chunk after the launch (a first pass before it only sums |ref| for the
         bound's scale s) when the launch cannot change the conv's operands, i.e. no operand shares a tensor with the output;
         otherwise every chunk is computed before the launch and kept (in host memory when large)."""
+        c = op.u.conv
         x, w, kw, out = emulator.conv_operands(c, it, self.mem)
         B, div = c.batch, kw["sample_row_div"]
         gn = c.groups > 0 and c.math in cabi.TC_MODES
@@ -276,8 +286,9 @@ class Auditor:
             return res
         return check
 
-    def _lnmod(self, m, x_state=None):
-        x, sh, sc, out = emulator.lnmod_operands(m, self.mem)
+    def _lnmod(self, op, it):
+        m = op.u.lnmod
+        x, sh, sc, out = emulator.lnmod_operands(m, it, self.mem)
         parts, total = [], 0.0
         park = 8 * m.batch * m.L * m.C > PARK
         for b0, b1 in _chunks(m.batch, m.L * m.C):
@@ -298,8 +309,9 @@ class Auditor:
             return res
         return check
 
-    def _attn(self, a):
-        qkv, out = emulator.attn_operands(a, self.mem)
+    def _attn(self, op, it):
+        a = op.u.attn
+        qkv, out = emulator.attn_operands(a, it, self.mem)
         ch = cabi.attn_choice(a)
         case = dict(want=(ch["family"], ch["param"]), heads=a.heads, hd=a.C // a.heads, L=a.L)
         parts, park = [], 16 * a.batch * a.L * a.C > PARK
@@ -316,8 +328,9 @@ class Auditor:
             return res
         return check
 
-    def _mha(self, m, it):
-        q, kv, out, both = mha_ref.mha_operands(m, it, self.mem)
+    def _mha(self, op, it):
+        m = op.u.mha
+        q, kv, out, both = emulator.mha_operands(m, it, self.mem)
         diag = m.diag if m.masked else None
         case = dict(heads=m.heads, hd=m.C // m.heads, diag=diag, kv="both" if both else "one")
         parts, park = [], 16 * m.batch * m.Lq * m.C > PARK
@@ -335,18 +348,15 @@ class Auditor:
             return res
         return check
 
+    def _host(self):
+        """host copies of the owners, taken at the first access to each"""
+        return emulator.Owned(self.mem.owners, host=True)
+
     def _exact(self, op, it):
         """UPDATE / PREP / CAST / GUIDE: the interpreter on host copies of the operands; the kernel must give the same bits
-        (GUIDE: cg_ref.run_guide is the kernel's fp32 multiply, then fp32 add)"""
-        host = emulator.Owned(self.mem.owners, host=True)
-        if op.kind == cabi.OP_UPDATE:
-            emulator.run_update(op.u.update, it, host)
-        elif op.kind == cabi.OP_PREP:
-            emulator.run_prep(op.u.prep, it, host)
-        elif op.kind == cabi.OP_GUIDE:
-            cg_ref.run_guide(op.u.guide, it, host)
-        else:
-            emulator.run_cast(op.u.cast, host)
+        (GUIDE: emulator.run_guide is the kernel's fp32 multiply, then fp32 add)"""
+        host = self._host()
+        emulator.run_program([op], 1, it, host)
         outs = declared_outputs(op, it)
         want = [emulator.view(host, *o) for o in outs]
 
@@ -356,7 +366,7 @@ class Auditor:
                     for j, (g, w) in enumerate(zip(got, want))]
         return check
 
-    # ---- classifier guidance (cg_ref) and the backward operators of a differentiable loop (grad_ref) -------------------
+    # ---- classifier operators (cg_ref) and the backward operators of a differentiable loop (grad_ref) ------------------
     def _bounded(self, outs, refs):
         """check() of the declared outputs ``outs`` against [(fp64 reference, bound)] (torch on any device, or numpy); a TF32
         output must also have the low 13 bits of every element clear"""
@@ -374,103 +384,78 @@ class Auditor:
             return res
         return check
 
-    def _host_arr(self):
-        """numpy float32 views (ptr, shape, strides) of host copies of the owners, for grad_ref's numpy references"""
-        host = emulator.Owned(self.mem.owners, host=True)
-        return lambda ptr, shape, strides: emulator._arr(ptr, shape, strides, host)
-
     def _gn(self, op, it):
         g = op.u.gn
-        v = emulator.view
-        h = v(self.mem, g.h, (g.batch, g.L, g.C), (g.h_bstride, g.h_lstride, 1), cabi.F32)
-        gamma, beta = v(self.mem, g.gamma, (g.C,), (1,), cabi.F32), v(self.mem, g.beta, (g.C,), (1,), cabi.F32)
-        vec = emulator.vec(g.vec, it, g.batch, g.C, 1, self.mem)
-        res = v(self.mem, g.res, (g.batch, g.L, g.C), (g.res_bstride, g.res_lstride, 1), cabi.F32) if g.res else None
+        h, gamma, beta, vec, res, _ = emulator.gn_operands(g, it, self.mem)
         ref = cg_ref.gn(h, gamma, beta, g.groups, g.eps, g.act, vec, res)
         bound = cg_ref.gn_bound(h, gamma, beta, g.groups, g.eps, ref, g.act, vec, res, g.out_dtype)
         return self._bounded(declared_outputs(op, it), [(ref, bound)])
 
     def _gn_bwd(self, op, it):
         g = op.u.gn_bwd
-        v = emulator.view
-        h = v(self.mem, g.h, (g.batch, g.L, g.C), (g.h_bstride, g.h_lstride, 1), cabi.F32)
-        gamma, beta = v(self.mem, g.gamma, (g.C,), (1,), cabi.F32), v(self.mem, g.beta, (g.C,), (1,), cabi.F32)
-        dout = v(self.mem, g.dout, (g.batch, g.L, g.C), (g.dout_bstride, g.dout_lstride, 1), cabi.F32)
+        h, gamma, beta, dout, _ = emulator.gn_bwd_operands(g, it, self.mem)
         ref = cg_ref.gn_bwd(h, gamma, beta, dout, g.groups, g.eps, g.act)
         bound = cg_ref.gn_bwd_bound(h, gamma, beta, dout, g.groups, g.eps, ref, g.act, g.dh_dtype)
         return self._bounded(declared_outputs(op, it), [(ref, bound)])
 
+    def _head_grad(self, op, it):
+        q = op.u.head_grad
+        h, w, b, _ = emulator.head_grad_operands(q, it, self._host())
+        _, seed = cg_ref.head_grad(h, w, b, q.scale, q.act)
+        return self._bounded(declared_outputs(op, it), [(seed, cg_ref.head_grad_bound(h, w, b, q.scale, q.act))])
+
     def _stash(self, op, it):
-        """the slot copy bit for bit; the Mish of the pre-activation under grad_ref.mish_bound"""
+        """the slot copy bit for bit; the Mish or SiLU of the pre-activation under grad_ref.ACT_BOUND"""
         s = op.u.stash
-        arr = self._host_arr()
-        src = arr(s.src, (s.n,), (1,)).copy()
+        src, _, _ = emulator.stash_operands(s, it, self._host())
         outs = declared_outputs(op, it)
-        refs = []
-        if s.act_out:
-            assert s.act == cabi.ACT_MISH, s.act
-            refs = [(grad_ref.mish(src), grad_ref.mish_bound(src.astype(np.float64)))]
-        bounded = self._bounded(outs[1:], refs)
+        refs = [(grad_ref.act(s.act, src), grad_ref.ACT_BOUND[s.act](src.astype(np.float64)))] if s.act_out else []
+        bounded = self._bounded(outs[-1:], refs)
 
         def check():
-            got = emulator.view(self.mem, *outs[0]).cpu()
-            return [(0.0 if same_bits(got, torch.from_numpy(src)) else math.inf, "slot bit for bit")] + bounded()
+            res = []
+            if s.dst:
+                got = emulator.view(self.mem, *outs[0]).cpu()
+                res.append((0.0 if same_bits(got, torch.from_numpy(src)) else math.inf, "slot bit for bit"))
+            return res + bounded()
         return check
 
     def _update_bwd(self, op, it):
-        u = op.u.update_bwd
-        arr = self._host_arr()
-        row = arr(u.coef + 4 * it * u.coef_iter_stride, (cabi.ROW_FLOATS,), (1,)).astype(np.float64)
-        shape, st = (u.batch, u.row), (u.row, 1)
-        gx = arr(u.gx, shape, st).copy()
-        x, pr = arr(u.x + 4 * it * u.x_iter_stride, shape, st), arr(u.pred + 4 * it * u.pred_iter_stride, shape, st)
-        vec = lambda p: None if not p else arr(p, (u.row,), (1,))          # noqa: E731
-        alpha, sigma, k0, k1 = row[0], row[1], row[2], row[3]
-        gp, dx = grad_ref.update_bwd(gx, x, pr, alpha=alpha, sigma=sigma, k0=k0, k1=k1, kind=int(row[7]),
-                                     predict_noise=bool(u.predict_noise), mask=vec(u.mask), x_min=vec(u.x_min),
-                                     x_max=vec(u.x_max))
-        bound = grad_ref.update_bwd_bound(gx, alpha, sigma, k0, k1)
+        gx, x, pr, kw, _ = emulator.update_bwd_operands(op.u.update_bwd, it, self._host())
+        gp, dx = grad_ref.update_bwd(gx, x, pr, **kw)
+        bound = grad_ref.update_bwd_bound(gx, kw["alpha"], kw["sigma"], kw["k0"], kw["k1"])
         return self._bounded(declared_outputs(op, it), [(dx, bound), (gp, bound)])
 
     def _dgrad(self, op, it):
         d = op.u.dgrad
-        arr = self._host_arr()
-        dz, w = arr(d.dz, (d.rows, d.N), (d.ldz, 1)), arr(d.w, (d.N, d.K), (d.ldw, 1))
-        z = arr(d.z + 4 * it * d.z_iter_stride, (d.rows, d.K), (d.K, 1)) if d.z else None
+        dz, w, z, out, out_sum = emulator.dgrad_operands(d, it, self._host())
         y = grad_ref.dgrad(dz, w, z, d.act)
-        before = arr(d.out, (d.rows, d.K), (d.ldo, 1)).astype(np.float64) if d.accumulate else None
+        before = out.astype(np.float64) if d.accumulate else None
         refs = [(y if before is None else before + y, grad_ref.dgrad_bound(dz, w, z, d.act, before))]
-        if d.out_sum:
-            s0 = arr(d.out_sum, (d.rows, d.K), (d.K, 1)).astype(np.float64)
+        if out_sum is not None:
+            s0 = out_sum.astype(np.float64)
             refs.append((s0 + y, grad_ref.dgrad_bound(dz, w, z, d.act, s0)))
         return self._bounded(declared_outputs(op, it), refs)
 
     def _wgrad(self, op, it):
         g = op.u.wgrad
-        arr = self._host_arr()
-        dz = arr(g.dz, (g.rows, g.N), (g.ldz, 1))
-        h = arr(g.h + 4 * it * g.h_iter_stride, (g.rows, g.K), (g.ldh, 1))
+        dz, h, dw, db = emulator.wgrad_operands(g, it, self._host())
         gw, gb = grad_ref.wgrad(dz, h, g.act)
-        w0 = arr(g.dw, (g.N, g.K), (g.lddw, 1)).astype(np.float64) if g.accumulate else None
-        b0 = arr(g.db + 4 * it * g.db_iter_stride, (g.N,), (1,)).astype(np.float64) if g.db and g.accumulate else None
+        w0 = dw.astype(np.float64) if g.accumulate else None
+        b0 = db.astype(np.float64) if db is not None and g.accumulate else None
         bw, bb = grad_ref.wgrad_bound(dz, h, g.act, w0, b0)
         refs = [(gw if w0 is None else w0 + gw, bw)] + ([(gb if b0 is None else b0 + gb, bb)] if g.db else [])
         return self._bounded(declared_outputs(op, it), refs)
 
+    # the reference check of every operator kind
+    REFERENCE = {cabi.OP_CONV: _conv, cabi.OP_UPDATE: _exact, cabi.OP_LNMOD: _lnmod, cabi.OP_ATTN: _attn,
+                 cabi.OP_PREP: _exact, cabi.OP_CAST: _exact, cabi.OP_MHA: _mha, cabi.OP_STASH: _stash,
+                 cabi.OP_UPDATE_BWD: _update_bwd, cabi.OP_DGRAD: _dgrad, cabi.OP_WGRAD: _wgrad, cabi.OP_GN: _gn,
+                 cabi.OP_GN_BWD: _gn_bwd, cabi.OP_GUIDE: _exact, cabi.OP_HEAD_GRAD: _head_grad}
+
     def reference(self, op, it):
-        if op.kind == cabi.OP_CONV:
-            return self._conv(op.u.conv, it)
-        if op.kind == cabi.OP_LNMOD:
-            return self._lnmod(op.u.lnmod)
-        if op.kind == cabi.OP_ATTN:
-            return self._attn(op.u.attn)
-        if op.kind == cabi.OP_MHA:
-            return self._mha(op.u.mha, it)
-        special = {cabi.OP_GN: self._gn, cabi.OP_GN_BWD: self._gn_bwd, cabi.OP_STASH: self._stash,
-                   cabi.OP_UPDATE_BWD: self._update_bwd, cabi.OP_DGRAD: self._dgrad, cabi.OP_WGRAD: self._wgrad}
-        if op.kind in special:
-            return special[op.kind](op, it)
-        return self._exact(op, it)
+        """check() -> [(fraction of the bound, label)] of ``op`` at iteration ``it``, from the state before its launch"""
+        return self.REFERENCE[op.kind](self, op, it)
 
     # ---- the audit -------------------------------------------------------------------------------------------------------
     def _launch(self, it, i, n):

@@ -1,5 +1,5 @@
 """ChiTransformer without a GPU: the module against the reference's goldens (tests/golden/chitransformer.npz), the lowered
-program executed by the numpy interpreter of the C ABI (tests/emulator.py, with CDS_OP_MHA from tests/mha_ref.py), the cases the lowering declines, and the host
+program executed by the numpy interpreter of the C ABI (tests/emulator.py), the cases the lowering declines, and the host
 side of CDS_OP_MHA (which instantiation each case of tests/mha_cases.py reaches, the refusals, and that the error bound
 rejects typical kernel faults)."""
 import os
@@ -57,9 +57,7 @@ def test_module_forward_matches_reference(gold, name):
 
 @pytest.fixture
 def emulate(monkeypatch):
-    monkeypatch.setattr(runtime, "_device_ok", lambda device: True)
-    owners = emulator.record_owners(monkeypatch)      # every operand is bounds-checked against its owner
-    monkeypatch.setattr(runtime, "_make_handle", lambda device, ops, n: mha_ref.Handle(ops, n, owners()))
+    emulator.emulate(monkeypatch)      # every operand is bounds-checked against its owner
     monkeypatch.setenv("CDS_BACKEND", "cuda")       # any fallback to the PyTorch loop is a failure here
 
 

@@ -1,6 +1,6 @@
 """Classifier guidance inside the replayed loop, on CPU: this package's CumRewClassifier / HalfJannerUNet1d against goldens
 written by the reference (tests/golden/make_golden_classifier.py -> classifier.npz), the lowered input-gradient program on the
-numpy interpreter (tests/cg_ref.py over tests/grad_ref.py over tests/emulator.py) against fp64 autograd, and guided sample()
+numpy interpreter (tests/emulator.py) against fp64 autograd, and guided sample()
 through the lowered program with classifier.gradients never called.  The other guided calls keep the host callback."""
 import numpy as np
 import pytest
@@ -9,18 +9,17 @@ import torch
 import cg_ref
 import emulator
 import make_golden_classifier as mg
+from common import load_golden, tape_of
 from cleandiffuser_b200.engine import cabi, runtime
 from cleandiffuser_b200.testing import NoiseTape
 
-G = cg_ref.golden()
+G = load_golden("classifier")
 MATHS = {"fp32": cabi.MATH_FP32, "tf32": cabi.MATH_TF32_TC}
 
 
 @pytest.fixture
 def emulated(monkeypatch):
-    monkeypatch.setattr(runtime, "_device_ok", lambda device: True)
-    owners = emulator.record_owners(monkeypatch)      # every operand is bounds-checked against its owner
-    monkeypatch.setattr(runtime, "_make_handle", lambda device, ops, n: cg_ref.Handle(ops, n, owners()))
+    emulator.emulate(monkeypatch)      # every operand is bounds-checked against its owner
     monkeypatch.setenv("CDS_BACKEND", "cuda")            # a fallback to the PyTorch loop raises
 
 
@@ -50,7 +49,7 @@ def test_lowered_input_gradient_matches_fp64_autograd(name, tkind, math):
 
 
 def _sample(agent, prior, kw, name):
-    tape = NoiseTape(cg_ref.tape_of(G, name))
+    tape = NoiseTape(tape_of(G, f"sample/{name}"))
     with tape.active():
         x0, log = agent.sample(prior, **kw)
     assert tape.pos == len(tape.draws)
@@ -81,7 +80,7 @@ def test_guided_sample_runs_in_the_lowered_program(emulated, name, math, monkeyp
         agent.classifier = _Wrapped(cg_ref.make_sample_agent(name)[0].classifier)
         with monkeypatch.context() as m:
             m.setattr(runtime, "_device_ok", lambda device: True)
-            m.setattr(runtime, "_make_handle", lambda device, ops, n: cg_ref.Handle(ops, n))
+            m.setattr(runtime, "_make_handle", lambda device, ops, n: emulator.Handle(ops, n))
             m.setenv("CDS_BACKEND", "cuda")
             m.setenv("CDS_MATH", math)
             ref, _ = _sample(agent, prior, kw, name)

@@ -8,6 +8,7 @@ import torch
 
 import cg_ref
 import make_golden_classifier as mg
+from common import load_golden, tape_of
 from cleandiffuser_b200.engine import cabi, runtime
 from cleandiffuser_b200.testing import NoiseTape, load_synth
 
@@ -195,9 +196,9 @@ def test_diffuser_hopper_call_graph_against_callback(math, monkeypatch):
 def test_goldens_on_the_gpu(name, monkeypatch):
     monkeypatch.setenv("CDS_BACKEND", "cuda")
     monkeypatch.setenv("CDS_MATH", "fp32")
-    G = cg_ref.golden()
+    G = load_golden("classifier")
     agent, prior, kw = cg_ref.make_sample_agent(name, device=DEV)
-    tape = NoiseTape(cg_ref.tape_of(G, name))
+    tape = NoiseTape(tape_of(G, f"sample/{name}"))
     with tape.active():
         x0, log = agent.sample(prior, **kw)
     assert runtime.STATS["guidance_path"] == "graph"

@@ -61,9 +61,7 @@ def test_edm_torch_path_matches_reference(golden, name, monkeypatch):
 def test_lowered_edm_program(golden, name, math, monkeypatch):
     """The engine program of ContinuousEDM.sample (PREP -> denoiser -> CDS_UPD_EDM / _HEUN per network evaluation) on the
     numpy interpreter of the ABI."""
-    monkeypatch.setattr(runtime, "_device_ok", lambda device: True)
-    owners = emulator.record_owners(monkeypatch)      # every operand is bounds-checked against its owner
-    monkeypatch.setattr(runtime, "_make_handle", lambda device, ops, n: emulator.Handle(ops, n, owners()))
+    emulator.emulate(monkeypatch)      # every operand is bounds-checked against its owner
     monkeypatch.setenv("CDS_BACKEND", "cuda")
     monkeypatch.setenv("CDS_MATH", math)
     spec = cases.edm_cases()[name]

@@ -332,7 +332,7 @@ def test_cast_is_bit_exact(C_in, C_out, out_dtype):
         k = op.u.cast
         k.batch, k.L, k.C_in, k.C_out, k.in_, k.out, k.out_dtype = B, L, C_in, C_out, _ptr(dd, "in"), _ptr(dd, "out"), out_dtype
         return op
-    emulator.run_cast(op_of(cpu).u.cast)
+    emulator.run_cast(op_of(cpu).u.cast, ITER)
     cabi.run_op(0, op_of(gpu), 0, torch.cuda.current_stream().cuda_stream)
     torch.cuda.synchronize()
     _compare(cpu, gpu, ("out",))

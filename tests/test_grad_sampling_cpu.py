@@ -1,7 +1,7 @@
 """``sample(requires_grad=True)`` over DQLMlp, lowered to the forward + backward operator programs and executed by the numpy
-interpreter (tests/emulator.py, extended by tests/grad_ref.py) on CPU tensors: the parameter and condition gradients must match fp64
-autograd of the PyTorch reverse loop under the same noise tape.  Also: the fallbacks, the unchanged requires_grad=False
-program, and the gradient rule of clip_prediction against torch.clip's."""
+interpreter (tests/emulator.py) on CPU tensors: the parameter and condition gradients must match fp64 autograd of the
+PyTorch reverse loop under the same noise tape.  Also: the fallbacks, the unchanged requires_grad=False program, and the
+gradient rule of clip_prediction against torch.clip's."""
 import copy
 
 import numpy as np
@@ -19,9 +19,7 @@ from cleandiffuser_b200.testing import NoiseTape, ToyClassifier, load_synth
 
 @pytest.fixture(autouse=True)
 def _emulate(monkeypatch):
-    monkeypatch.setattr(runtime, "_device_ok", lambda device: True)
-    owners = emulator.record_owners(monkeypatch)      # every operand is bounds-checked against its owner
-    monkeypatch.setattr(runtime, "_make_handle", lambda device, ops, n: grad_ref.Handle(ops, n, owners()))
+    emulator.emulate(monkeypatch)      # every operand is bounds-checked against its owner
     monkeypatch.setenv("CDS_BACKEND", "cuda")       # any fallback to the PyTorch loop is a failure here
     monkeypatch.setenv("CDS_MATH", "fp32")
 

@@ -61,9 +61,7 @@ def test_legacy_ddpm_torch_path_matches_reference(golden, name, monkeypatch):
 @pytest.mark.parametrize("math", ["fp32", "tf32"])
 @pytest.mark.parametrize("name", NAMES)
 def test_legacy_ddpm_lowered_program(golden, name, math, monkeypatch):
-    monkeypatch.setattr(runtime, "_device_ok", lambda device: True)
-    owners = emulator.record_owners(monkeypatch)      # every operand is bounds-checked against its owner
-    monkeypatch.setattr(runtime, "_make_handle", lambda device, ops, n: emulator.Handle(ops, n, owners()))
+    emulator.emulate(monkeypatch)      # every operand is bounds-checked against its owner
     monkeypatch.setenv("CDS_BACKEND", "cuda")
     monkeypatch.setenv("CDS_MATH", math)
     spec = cases.legacy_cases()[name]
@@ -142,9 +140,7 @@ def test_legacy_edm_torch_path_matches_reference(golden, name, monkeypatch):
 @pytest.mark.parametrize("math", ["fp32", "tf32"])
 @pytest.mark.parametrize("name", EDM_NAMES)
 def test_legacy_edm_lowered_program(golden, name, math, monkeypatch):
-    monkeypatch.setattr(runtime, "_device_ok", lambda device: True)
-    owners = emulator.record_owners(monkeypatch)      # every operand is bounds-checked against its owner
-    monkeypatch.setattr(runtime, "_make_handle", lambda device, ops, n: emulator.Handle(ops, n, owners()))
+    emulator.emulate(monkeypatch)      # every operand is bounds-checked against its owner
     monkeypatch.setenv("CDS_BACKEND", "cuda")
     monkeypatch.setenv("CDS_MATH", math)
     spec = cases.legacy_edm_cases()[name]

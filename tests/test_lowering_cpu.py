@@ -18,9 +18,7 @@ from cleandiffuser_b200.testing import NoiseTape
 
 @pytest.fixture(autouse=True)
 def _emulate(monkeypatch):
-    monkeypatch.setattr(runtime, "_device_ok", lambda device: True)
-    owners = emulator.record_owners(monkeypatch)      # every operand is bounds-checked against its owner
-    monkeypatch.setattr(runtime, "_make_handle", lambda device, ops, n: emulator.Handle(ops, n, owners()))
+    emulator.emulate(monkeypatch)      # every operand is bounds-checked against its owner
     monkeypatch.setenv("CDS_BACKEND", "cuda")       # any fallback to the PyTorch loop is a failure here
     monkeypatch.setenv("CDS_MATH", "fp32")
 

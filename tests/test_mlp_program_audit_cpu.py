@@ -5,11 +5,10 @@ import pytest
 import torch
 
 import emulator
-import mha_ref
 import mlp_programs as mp
 import opref
 import program_audit as pa
-from cleandiffuser_b200.engine import cabi, lower, runtime
+from cleandiffuser_b200.engine import cabi, lower
 
 # The interpreter stores the rounding of the exact value: at most half a unit of the output type, 2^-11 2^e for TF32 and
 # 2^-8 2^e for bf16 (e: the exponent of |ref|, so 2^e <= |ref|), against the bound's 2^-10 |ref| and 2^-8 |ref|
@@ -19,9 +18,7 @@ NAMES = ["idql", "dql", "veteran50", "sfbc", "sfbc-cfg", "dbc10"]
 
 @pytest.fixture(autouse=True)
 def _emulate(monkeypatch):
-    monkeypatch.setattr(runtime, "_device_ok", lambda device: True)
-    owners = emulator.record_owners(monkeypatch)
-    monkeypatch.setattr(runtime, "_make_handle", lambda device, ops, n: mha_ref.Handle(ops, n, owners()))
+    emulator.emulate(monkeypatch)      # every operand is bounds-checked against its owner
     monkeypatch.setenv("CDS_BACKEND", "cuda")
     monkeypatch.delenv("CDS_BRANCHES", raising=False)
 
@@ -118,7 +115,7 @@ def test_lnmod_broadcast_row_read_per_row_is_caught(monkeypatch):
         bad = cabi.Op.from_buffer_copy(op)
         bad.u.lnmod.mod_bstride = bad.u.lnmod.C
         try:
-            emulator.run_lnmod(bad.u.lnmod, mem)
+            emulator.run_lnmod(bad.u.lnmod, it, mem)
         except AssertionError as e:
             past.append(str(e))
             _fail_with_nan(op, it, mem)

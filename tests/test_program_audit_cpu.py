@@ -1,8 +1,8 @@
 """The machinery of tests/test_program_audit_gpu.py without a GPU: the same auditor drives the interpreter's handle
-(tests/emulator.py, tests/mha_ref.py) over programs lowered for CPU tensors, at small batches.  The interpreter computes
-what the fp64 reference computes, so every operator must pass with a fraction at most the half unit of the stored rounding;
-injected faults must be caught and pinned on the right operator.  The classifier-guided and differentiable programs run on
-tests/cg_ref.py's interpreter, and their faults are subtly wrong kernels run in place of one operator."""
+(tests/emulator.py) over programs lowered for CPU tensors, at small batches.  The interpreter computes what the fp64
+reference computes, so every operator must pass with a fraction at most the half unit of the stored rounding; injected
+faults must be caught and pinned on the right operator.  The faults of the classifier-guided and differentiable programs
+are subtly wrong kernels run in place of one operator."""
 import pytest
 import torch
 
@@ -10,7 +10,6 @@ import cg_ref
 import chi_cases as cc
 import emulator
 import grad_ref
-import mha_ref
 import opref
 import program_audit as pa
 from cleandiffuser_b200 import workloads
@@ -26,9 +25,7 @@ PASS_FRAC = 0.5 + 1e-3
 
 @pytest.fixture(autouse=True)
 def _emulate(monkeypatch):
-    monkeypatch.setattr(runtime, "_device_ok", lambda device: True)
-    owners = emulator.record_owners(monkeypatch)
-    monkeypatch.setattr(runtime, "_make_handle", lambda device, ops, n: mha_ref.Handle(ops, n, owners()))
+    emulator.emulate(monkeypatch)      # every operand is bounds-checked against its owner
     monkeypatch.setenv("CDS_BACKEND", "cuda")
     monkeypatch.setenv("CDS_MATH", "tf32")
 
@@ -147,14 +144,8 @@ def test_the_extent_check_rejects_a_stride_past_the_owner(monkeypatch):
 
 
 # ---- classifier guidance and differentiable sampling (tests/cg_ref.py, tests/grad_ref.py) -----------------------------------
-def _cg_handles(monkeypatch):
-    owners = emulator.record_owners(monkeypatch)
-    monkeypatch.setattr(runtime, "_make_handle", lambda device, ops, n: cg_ref.Handle(ops, n, owners()))
-
-
 def _guided_plan(monkeypatch, math_mode):
     """a guided sample() of tests/golden/make_golden_classifier.py (horizon 8, batch 8, 5 DDPM steps), classifier lowered"""
-    _cg_handles(monkeypatch)
     monkeypatch.setenv("CDS_MATH", math_mode)
     agent, prior, kw = cg_ref.make_sample_agent("discrete_ddpm_eps")
     agent.sample(prior, **kw)
@@ -164,7 +155,6 @@ def _guided_plan(monkeypatch, math_mode):
 
 
 def _grad_plan(monkeypatch, case, math_mode="tf32", batch=16):
-    _cg_handles(monkeypatch)
     monkeypatch.setenv("CDS_MATH", math_mode)
     agent, kw = grad_ref.grad_agent(case, "cpu")
     g = torch.Generator().manual_seed(2)
@@ -224,7 +214,7 @@ def test_gn_variance_over_n_minus_1_is_caught(monkeypatch):
     def gn_unbiased(op, it):
         with monkeypatch.context() as m:
             m.setattr(cg_ref, "_stats", stats_unbiased)
-            cg_ref.run_gn(op.u.gn, it, mem)
+            emulator.run_gn(op.u.gn, it, mem)
     aud = _audit(plan, _Faulty(plan.handle, ops, j, gn_unbiased, replace=True), iters=(1,))
     assert _pinned(aud.failures, j), aud.failures[:5]
 
@@ -233,7 +223,7 @@ def test_gn_time_row_of_iteration_0_is_caught(monkeypatch):
     plan = _guided_plan(monkeypatch, "tf32")
     ops, mem = plan.program.ops, plan.handle.mem
     j = next(i for i, op in enumerate(ops) if op.kind == cabi.OP_GN and op.u.gn.vec.step)
-    aud = _audit(plan, _Faulty(plan.handle, ops, j, lambda op, it: cg_ref.run_gn(op.u.gn, 0, mem), replace=True), iters=(0, 1))
+    aud = _audit(plan, _Faulty(plan.handle, ops, j, lambda op, it: emulator.run_gn(op.u.gn, 0, mem), replace=True), iters=(0, 1))
     assert _pinned(aud.failures, j) and all(m.startswith("cpu it 1 ") for m in aud.failures), aud.failures[:5]
 
 
@@ -260,13 +250,12 @@ def test_dgrad_reading_the_forward_slot_of_its_own_index_is_caught(monkeypatch):
     plan = _grad_plan(monkeypatch, "dql-eps")
     ops, mem = plan.back.ops, plan.back_handle.mem
     j = next(i for i, op in enumerate(ops) if op.kind == cabi.OP_DGRAD and op.u.dgrad.z)
-    arr = lambda ptr, shape, strides: emulator._arr(ptr, shape, strides, mem)       # noqa: E731
 
     def forward_order(op, it):
         bad = cabi.Op.from_buffer_copy(op)
         d = bad.u.dgrad
         d.z, d.z_iter_stride = d.z + 4 * (plan.n_iters - 1) * d.z_iter_stride, -d.z_iter_stride
-        grad_ref.run_dgrad(d, it, arr)
+        emulator.run_dgrad(d, it, mem)
     fa, ba = _grad_audit(plan, _Faulty(plan.back_handle, ops, j, forward_order, replace=True))
     assert not fa.failures and _pinned(ba.failures, j, "bwd"), (fa.failures + ba.failures)[:5]
     # the middle iteration reads its own slot either way (at the last one, forward iteration 0, the clip to [-1, 1] at
@@ -279,13 +268,12 @@ def test_wgrad_bias_into_the_neighbouring_row_is_flagged(monkeypatch):
     plan = _grad_plan(monkeypatch, "dql-x0")
     ops, mem = plan.back.ops, plan.back_handle.mem
     j = next(i for i, op in enumerate(ops) if op.kind == cabi.OP_WGRAD and op.u.wgrad.db_iter_stride)
-    arr = lambda ptr, shape, strides: emulator._arr(ptr, shape, strides, mem)       # noqa: E731
 
     def neighbour(op, it):
         bad = cabi.Op.from_buffer_copy(op)
         g = bad.u.wgrad
         g.db += 4 * (1 if it < plan.n_iters - 1 else -1) * g.db_iter_stride
-        grad_ref.run_wgrad(g, it, arr)
+        emulator.run_wgrad(g, it, mem)
     fa, ba = _grad_audit(plan, _Faulty(plan.back_handle, ops, j, neighbour, replace=True))
     assert not fa.failures and _pinned(ba.failures, j, "bwd"), (fa.failures + ba.failures)[:5]
     assert any("outside the declared outputs" in m for m in ba.failures), ba.failures[:5]

@@ -1,6 +1,6 @@
 """QGPO's classifier guidance inside the replayed loop, on CPU: this package's QGPOClassifier / QGPONNClassifier against goldens
 written by the reference (tests/golden/make_golden_qgpo.py -> qgpo.npz), the lowered input-gradient program on the numpy
-interpreter (tests/qgpo_ref.py over tests/cg_ref.py) against fp64 autograd, and QGPO-shaped guided sample() through the
+interpreter (tests/emulator.py) against fp64 autograd, and QGPO-shaped guided sample() through the
 lowered program with classifier.gradients never called.  The other guided calls keep the host callback."""
 import os
 
@@ -8,21 +8,22 @@ import numpy as np
 import pytest
 import torch
 
+import cg_ref
 import emulator
 import make_golden_qgpo as mg
+import program_audit as pa
 import qgpo_ref
+from common import load_golden, tape_of
 from cleandiffuser_b200.engine import cabi, runtime
 from cleandiffuser_b200.testing import NoiseTape
 
-G = qgpo_ref.golden()
+G = load_golden("qgpo")
 MATHS = {"fp32": cabi.MATH_FP32, "tf32": cabi.MATH_TF32_TC}
 
 
 @pytest.fixture
 def emulated(monkeypatch):
-    monkeypatch.setattr(runtime, "_device_ok", lambda device: True)
-    owners = emulator.record_owners(monkeypatch)      # every operand is bounds-checked against its owner
-    monkeypatch.setattr(runtime, "_make_handle", lambda device, ops, n: qgpo_ref.Handle(ops, n, owners()))
+    emulator.emulate(monkeypatch)      # every operand is bounds-checked against its owner
     monkeypatch.setenv("CDS_BACKEND", "cuda")            # a fallback to the PyTorch loop raises
 
 
@@ -58,7 +59,7 @@ def test_lowered_input_gradient_matches_fp64_autograd(name, math):
     x, t, obs = _net_case(name)
     # the engine evaluates one time per iteration: iteration k of a table holding every row's time
     for k in range(len(t)):
-        got, _ = qgpo_ref.lowered_gradient(clf, x, t, obs, k, MATHS[math], "cpu")
+        got, _ = cg_ref.lowered_gradient(clf, x, t, k, MATHS[math], "cpu", cond=obs)
         want = qgpo_ref.input_gradient_fp64(clf, x, t[k].expand(len(t)), obs)
         rel = float((got.double() - want).norm() / want.norm())
         # fp32: summation order only (the interpreter's GEMMs are fp64 with fp32 stores).  TF32: the interpreter reads the
@@ -67,7 +68,7 @@ def test_lowered_input_gradient_matches_fp64_autograd(name, math):
 
 
 def _sample(agent, prior, kw, name):
-    tape = NoiseTape(qgpo_ref.tape_of(G, name))
+    tape = NoiseTape(tape_of(G, f"sample/{name}"))
     with tape.active():
         x0, log = agent.sample(prior, **kw)
     assert tape.pos == len(tape.draws)
@@ -195,15 +196,13 @@ def test_plan_repacks_after_classifier_update_and_load(emulated, how, monkeypatc
 
 @pytest.mark.parametrize("math", list(MATHS))
 def test_program_audit_of_the_qgpo_iteration_on_the_interpreter(emulated, math, monkeypatch):
-    """tests/qgpo_audit.py (tests/program_audit.py's audit with QGPO's operators) drives the interpreter over the guided program: every operator of every iteration within its
+    """tests/program_audit.py drives the interpreter over the guided program: every operator of every iteration within its
     bound and nothing written outside its declared outputs (the same audit runs on the H100)"""
-    import program_audit as pa
-    import qgpo_audit
     monkeypatch.setenv("CDS_MATH", math)
     agent, prior, kw = qgpo_ref.make_sample_agent("ddpm_eps")
     _sample(agent, prior, kw, "ddpm_eps")
     plan = next(iter(agent._engine_plans.values()))
-    aud = qgpo_audit.Auditor(f"qgpo-{math}", plan.program.ops, plan.handle, pa.plan_owners(plan))
+    aud = pa.Auditor(f"qgpo-{math}", plan.program.ops, plan.handle, pa.plan_owners(plan))
     aud.audit_once(0)
     for it in range(plan.n_iters):
         aud.audit_iteration(it)

@@ -1,16 +1,18 @@
-"""QGPO's classifier guidance inside the replayed loop on the H100: CDS_OP_DGRAD / CDS_OP_STASH with SiLU and CDS_OP_HEAD_GRAD
-against fp64 (tests/qgpo_ref.py), QGPONNClassifier's lowered input gradient against fp64 autograd at the D4RL MuJoCo shapes,
-QGPO-shaped sample() calls against the host-callback path and the goldens, graph replay / reproducibility, and an
-operator-by-operator audit of the guided iteration (tests/qgpo_audit.py over tests/program_audit.py)."""
+"""QGPO's classifier guidance inside the replayed loop on the H100: CDS_OP_DGRAD / CDS_OP_STASH with SiLU (tests/grad_ref.py)
+and CDS_OP_HEAD_GRAD (tests/cg_ref.py) against fp64, QGPONNClassifier's lowered input gradient against fp64 autograd at the
+D4RL MuJoCo shapes, QGPO-shaped sample() calls against the host-callback path and the goldens, graph replay /
+reproducibility, and an operator-by-operator audit of the guided iteration (tests/program_audit.py)."""
 import numpy as np
 import pytest
 import torch
 
+import cg_ref
 import emulator
+import grad_ref
 import make_golden_qgpo as mg
 import program_audit as pa
-import qgpo_audit
 import qgpo_ref
+from common import load_golden, tape_of
 from cleandiffuser_b200.engine import cabi, runtime
 from cleandiffuser_b200.testing import NoiseTape, load_synth
 
@@ -39,7 +41,7 @@ def _frac(got, want, bound):
 @pytest.mark.parametrize("N", WIDTHS)
 @pytest.mark.parametrize("K", WIDTHS)
 def test_dgrad_silu_matches_fp64(rows, N, K):
-    """out = (dz W) silu'(z) under qgpo_ref.dgrad_bound, and bitwise equal over two runs"""
+    """out = (dz W) silu'(z) under grad_ref.dgrad_bound, and bitwise equal over two runs"""
     g = torch.Generator().manual_seed(rows + 7 * N + K)
     dz, w, z = torch.randn(rows, N, generator=g), torch.randn(N, K, generator=g) / N ** 0.5, 3 * torch.randn(2, rows, K, generator=g)
     dz, w, z = dz.to(DEV), w.to(DEV), z.to(DEV)
@@ -53,7 +55,7 @@ def test_dgrad_silu_matches_fp64(rows, N, K):
     _run(op, 1)                                             # iteration 1: the second slot of z
     first = out.clone()
     args = (dz.cpu().numpy(), w.cpu().numpy(), z[1].cpu().numpy(), cabi.ACT_SILU)
-    frac = _frac(out, qgpo_ref.dgrad(*args), qgpo_ref.dgrad_bound(*args))
+    frac = _frac(out, grad_ref.dgrad(*args), grad_ref.dgrad_bound(*args))
     assert frac <= 1.0, frac
     _run(op, 1)
     assert torch.equal(out, first)
@@ -76,8 +78,8 @@ def test_head_grad_matches_fp64(rows, K, act):
     _run(op)
     first = seed.clone()
     hh, ww, bb = h[:, :K].cpu().numpy(), w.cpu().numpy(), b.cpu().numpy()
-    z, want = qgpo_ref.head_grad(hh, ww, bb, 10.0, act)
-    frac = _frac(seed[:rows], want, qgpo_ref.head_grad_bound(hh, ww, bb, 10.0, act))
+    z, want = cg_ref.head_grad(hh, ww, bb, 10.0, act)
+    frac = _frac(seed[:rows], want, cg_ref.head_grad_bound(hh, ww, bb, 10.0, act))
     assert frac <= 1.0, frac
     assert bool((seed[rows:] == 7.0).all()), "HEAD_GRAD wrote past its rows"
     assert np.abs(z).max() > 10, "the cases should reach the tanh's saturation"
@@ -98,7 +100,7 @@ def test_stash_silu_without_slot(n):
     s.n, s.act, s.src, s.act_out = n, cabi.ACT_SILU, src.data_ptr(), out.data_ptr()
     _run(op)
     x = src.cpu().numpy()
-    frac = _frac(out[:n], qgpo_ref.silu(x), qgpo_ref.silu_bound(x))
+    frac = _frac(out[:n], grad_ref.act(cabi.ACT_SILU, x), grad_ref.silu_bound(x))
     assert frac <= 1.0, frac
     assert bool((out[n:] == 7.0).all())
 
@@ -117,7 +119,7 @@ def test_input_gradient_matches_fp64_autograd(name, batch, math):
     x = torch.randn(batch, kw["act_dim"], generator=g).clamp(-1, 1).to(DEV)
     obs = torch.randn(batch, kw["obs_dim"], generator=g).to(DEV)
     t = torch.tensor([0.9, 0.3], device=DEV)
-    got, _ = qgpo_ref.lowered_gradient(clf, x, t, obs, 1, MATHS[math], DEV, handle=_handle)
+    got, _ = cg_ref.lowered_gradient(clf, x, t, 1, MATHS[math], DEV, cond=obs, handle=_handle)
     torch.cuda.synchronize()
     want = qgpo_ref.input_gradient_fp64(clf, x, t[1].expand(batch), obs)
     rel = float((got.double() - want).norm() / want.norm())
@@ -205,13 +207,13 @@ def test_qgpo_call_graph_against_callback(call, math, monkeypatch):
 def test_goldens_on_the_gpu(name, monkeypatch):
     monkeypatch.setenv("CDS_BACKEND", "cuda")
     monkeypatch.setenv("CDS_MATH", "fp32")
-    G = qgpo_ref.golden()
+    G = load_golden("qgpo")
     agent, prior, kw = qgpo_ref.make_sample_agent(name, device=DEV)
 
     def refuse(*a, **k):
         raise AssertionError("classifier.gradients called: guidance left the program")
     monkeypatch.setattr(agent.classifier, "gradients", refuse)
-    tape = NoiseTape(qgpo_ref.tape_of(G, name))
+    tape = NoiseTape(tape_of(G, f"sample/{name}"))
     with tape.active():
         x0, log = agent.sample(prior, **kw)
     assert runtime.STATS["guidance_path"] == "graph"
@@ -236,7 +238,7 @@ def test_graph_replay_equals_direct_launches_and_repeats_bitwise(math, monkeypat
 
 @pytest.mark.parametrize("math", list(MATHS))
 def test_every_operator_of_the_qgpo_iteration_matches_fp64(math, monkeypatch):
-    """tests/qgpo_audit.py over every iteration of the hopper-medium-replay call: each operator within its bound, nothing
+    """tests/program_audit.py over every iteration of the hopper-medium-replay call: each operator within its bound, nothing
     written outside its declared outputs; then whole iterations by graph replay give the operator-by-operator bits"""
     monkeypatch.setenv("CDS_BACKEND", "cuda")
     monkeypatch.setenv("CDS_MATH", math)
@@ -250,7 +252,7 @@ def test_every_operator_of_the_qgpo_iteration_matches_fp64(math, monkeypatch):
     torch.cuda.synchronize()
     start = torch.rand(plan.x.shape, generator=torch.Generator().manual_seed(7)).to(DEV) * 2 - 1
     plan.x.copy_(start)
-    aud = qgpo_audit.Auditor(f"qgpo-{math}", ops, plan.handle, pa.plan_owners(plan), st, torch.cuda.synchronize)
+    aud = pa.Auditor(f"qgpo-{math}", ops, plan.handle, pa.plan_owners(plan), st, torch.cuda.synchronize)
     aud.audit_once(0)
     for it in range(n):
         aud.audit_iteration(it)
@@ -260,7 +262,7 @@ def test_every_operator_of_the_qgpo_iteration_matches_fp64(math, monkeypatch):
     assert plan.handle.launches_per_iter() == pa.launches_per_iter(ops)
 
     mem = emulator.Owned(pa.plan_owners(plan))
-    written = [mem.owners[i] for i in qgpo_audit.written_owners(mem, ops, range(n))]
+    written = [mem.owners[i] for i in pa.written_owners(mem, ops, range(n))]
     outs = {}
     for mode in ("op by op", "graph"):
         plan.x.copy_(start)

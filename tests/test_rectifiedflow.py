@@ -44,9 +44,7 @@ def test_rf_torch_path_matches_reference(golden, name, monkeypatch):
 @pytest.mark.parametrize("math", ["fp32", "tf32"])
 @pytest.mark.parametrize("name", NAMES)
 def test_rf_lowered_program(golden, name, math, monkeypatch):
-    monkeypatch.setattr(runtime, "_device_ok", lambda device: True)
-    owners = emulator.record_owners(monkeypatch)      # every operand is bounds-checked against its owner
-    monkeypatch.setattr(runtime, "_make_handle", lambda device, ops, n: emulator.Handle(ops, n, owners()))
+    emulator.emulate(monkeypatch)      # every operand is bounds-checked against its owner
     monkeypatch.setenv("CDS_BACKEND", "cuda")
     monkeypatch.setenv("CDS_MATH", math)
     agent, inp, kw = build(cases.rf_cases()[name])
