@@ -410,6 +410,10 @@ def _unet_body(p: Program, net, x: View, horizon: int, k: int, film_of: Callable
                    bias=_const_vec(p.packed(lambda m=up: m.conv.bias)))
 
     fc = net.final_conv
+    if fc[0].in_channels != x.C:
+        # dim_mult[0] != 1 (a single-stage UNet included): the module's final_conv cannot take the last stage's channels
+        # and its forward raises; the weight packing would zero-pad them instead
+        raise Unsupported(f"final_conv takes {fc[0].in_channels} channels, the last stage gives {x.C}")
     y = _lower_conv_block(p, fc, x, p.act(horizon, fc[0].out_channels), final_k)
     last = fc[3]
     return p.conv(y, w_rows(lambda: last.weight[:, :, 0]), p.act(horizon, last.out_channels, dtype=torch.float32),
