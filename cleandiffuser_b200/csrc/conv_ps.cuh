@@ -18,12 +18,16 @@
 //   columns per register block of the accumulators instead of one N-column wgmma each, so the A tile is read from shared
 //   memory fewer times (conv_ps_mma_position: 7 wgmmas per k step instead of 14 for taps = 5).  The CTA has one tile, so
 //   once the MMAs are done the operand ring is idle and the accumulators are written over it as a 128-row fp32 tile.
-// * epilogue (the same 8 warps): thread = one trajectory x NH = N/2 columns (ONE GroupNorm group) x all P positions, so the
-//   GroupNorm statistics over (P positions x C_out/8 channels) are plain in-thread sums: no shuffles.  Two passes over the
-//   tile (statistics, then normalise + Mish + store).
-// * CTA tile = 128 trajectories x N = C_out/4 columns (2 GroupNorm groups: one per epilogue column slice); grid =
-//   ceil(batch/128) x 4 CTAs (128 CTAs at batch 4096), one tile per CTA, 4-stage smem ring over the channel chunks, warp 8
-//   is the TMA producer.
+// * epilogue (the same 8 warps): thread = one trajectory x NH = N/2 columns x all P positions.  When the column slice is ONE
+//   GroupNorm group, the statistics over (P positions x C_out/8 channels) are plain in-thread sums: no shuffles; when the
+//   CTA tile is one group (the 256-wide layers with a shortcut conv, N = 32), the two threads of a row add their halves
+//   through shared memory.  Two passes over the tile (statistics, then normalise + Mish + store).
+// * CTA tile = 128 trajectories x N = C_out/4 columns (2 GroupNorm groups), or C_out/8 (1 group) with a 256-wide shortcut
+//   layer; grid = ceil(batch/128) x C_out/N CTAs (128 CTAs at batch 4096 for N = C_out/4), one tile per CTA, 4-stage smem
+//   ring over the channel chunks, warp 8 is the TMA producer.
+// * two-phase transposed conv (ConvTranspose1d(k=4, s=2, p=1) as 3 taps x 2 C_out phase-major columns, L 4 -> 8): the same
+//   GEMM over 2 C_out columns; the epilogue adds the bias only (one pass), and column c of phase ph at output position l'
+//   is stored at position 2 l' + ph.
 //
 // Algorithmic HBM bytes per launch: 2*(batch*P*C_in + batch*P*C_out) (+ shortcut input), weights once through L2.
 #pragma once
@@ -37,8 +41,10 @@ struct ConvPsParams {
   CUtensorMap tm_out;             // output as a TMA-store target: box {16 channels, 1 position, 32 trajectories} (one epilogue warp's
   int out_tma;                    // lanes x 16 columns), staged in shared memory; valid when out_tma != 0
   int batch, C_out, taps;         // taps 1, 3 or 5 with pad = taps / 2 (conv_ps_eligible)
+  int phases;                     // 2: columns [0,C_out) / [C_out,2C_out) are output positions 2l / 2l+1 (transposed conv)
+  int bias_only;                  // epilogue: 0 = GroupNorm(8) + Mish + additive terms, 1 = bias only
   int kchunks, kchunks2;          // channel chunks of the main conv / of the shortcut conv
-  int n_tiles;                    // column tiles per trajectory tile (C_out / N)
+  int n_tiles;                    // column tiles per trajectory tile (C_out * phases / N)
   int in_batch_mod, res_batch_mod;
   cds_vec bias, shift;
   const float* gn_gamma; const float* gn_beta; float gn_eps;
@@ -176,6 +182,7 @@ conv_ps_kernel(const __grid_constant__ ConvPsParams p, const int* __restrict__ i
   __shared__ __align__(8) uint64_t empty_bar[kStages];
   // per-column constants: 0 bias  1 GN gamma  2 GN beta  3 additive time row  4 shortcut bias
   __shared__ __align__(16) float s_col[5][N];
+  __shared__ float2 s_stat[kPsEpiThreads];            // GroupNorm partial sums when a group spans both column slices
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const uint32_t smem_base = (ptx::smem_u32(smem_raw) + 1023u) & ~1023u;
@@ -184,7 +191,9 @@ conv_ps_kernel(const __grid_constant__ ConvPsParams p, const int* __restrict__ i
   if (threadIdx.x == 0) { CDS_TRACE(0, gtimer()); CDS_TRACE(1, clock64()); }
 
   const int tile_b = blockIdx.x / p.n_tiles;          // trajectory tile
-  const int n_off = (blockIdx.x % p.n_tiles) * N;     // first output channel of this CTA
+  const int n_off = (blockIdx.x % p.n_tiles) * N;     // first GEMM column of this CTA
+  const int ph = n_off / p.C_out;                     // its output phase (a CTA tile lies inside one phase)
+  const int ch0 = n_off - ph * p.C_out;               // its first output channel
   const int b0 = tile_b * 128;
   const int n_main = p.kchunks;
   const int n_chunks = n_main + (HAS_RES ? p.kchunks2 : 0);
@@ -212,7 +221,7 @@ conv_ps_kernel(const __grid_constant__ ConvPsParams p, const int* __restrict__ i
         uint8_t* sb = smem_al + s * Cfg::kStageBytes + P * Cfg::kATile;
         if (!HAS_RES || c < n_main) {
           for (int j = 0; j < p.taps; ++j)
-            ptx::tma_load_2d(sb + (p.taps - 1 - j) * Cfg::kBTile, &p.tm_b, &full_bar[s], c * KE, j * p.C_out + n_off);   // slot = taps-1-j
+            ptx::tma_load_2d(sb + (p.taps - 1 - j) * Cfg::kBTile, &p.tm_b, &full_bar[s], c * KE, j * p.C_out * p.phases + n_off);   // slot = taps-1-j
         } else {
           ptx::tma_load_2d(sb, &p.tm_b2, &full_bar[s], (c - n_main) * KE, n_off);
         }
@@ -251,10 +260,10 @@ conv_ps_kernel(const __grid_constant__ ConvPsParams p, const int* __restrict__ i
       const float* bstep = p.bias.step ? p.bias.step + (int64_t)iter * p.bias.step_stride : nullptr;
       const float* hstep = p.shift.step ? p.shift.step + (int64_t)iter * p.shift.step_stride : nullptr;
       for (int n = threadIdx.x; n < N; n += kPsEpiThreads) {
-        const int c = n_off + n;
+        const int c = ch0 + n;
         s_col[0][n] = bstep ? __ldg(bstep + c) : 0.f;
-        s_col[1][n] = __ldg(p.gn_gamma + c);
-        s_col[2][n] = __ldg(p.gn_beta + c);
+        s_col[1][n] = p.bias_only ? 0.f : __ldg(p.gn_gamma + c);
+        s_col[2][n] = p.bias_only ? 0.f : __ldg(p.gn_beta + c);
         s_col[3][n] = hstep ? __ldg(hstep + c) : 0.f;
         s_col[4][n] = (HAS_RES && p.res_bias) ? __ldg(p.res_bias + c) : 0.f;
       }
@@ -264,9 +273,9 @@ conv_ps_kernel(const __grid_constant__ ConvPsParams p, const int* __restrict__ i
     else if (p.taps == 3) conv_ps_mma<3, KC, N, P, HAS_RES, TF32>(p, full_bar, empty_bar, smem_base, acc);
     else conv_ps_mma<1, KC, N, P, HAS_RES, TF32>(p, full_bar, empty_bar, smem_base, acc);
     // ===================================== epilogue =====================================
-    // thread = one trajectory (accumulator row) x NH = N/2 columns (ONE GroupNorm group) x all P positions
+    // thread = one trajectory (accumulator row) x NH = N/2 columns (one GroupNorm group, or half of one) x all P positions
     constexpr int NH = N / 2;
-    static_assert(NH == 16 || NH == 32, "one GroupNorm group of 16 or 32 channels per epilogue column slice");
+    static_assert(NH == 16 || NH == 32, "a GroupNorm group of 16 or 32 channels per epilogue column slice");
     const int q = warp & 3, half = warp >> 2;
     const int b = b0 + 32 * q + lane;
     const bool valid = b < p.batch;
@@ -276,26 +285,38 @@ conv_ps_kernel(const __grid_constant__ ConvPsParams p, const int* __restrict__ i
     if (threadIdx.x == 0) CDS_TRACE(10, clock64());
 
     // ---- pass 1: GroupNorm statistics of (accumulator + bias) over P positions x NH channels, all in this thread
-    float s1 = 0.f, s2 = 0.f;
+    float ga = 1.f, gc = 0.f;
+    if (!p.bias_only) {
+      float s1 = 0.f, s2 = 0.f;
 #pragma unroll
-    for (int lp = 0; lp < P; ++lp) {
+      for (int lp = 0; lp < P; ++lp) {
 #pragma unroll
-      for (int h = 0; h < NH / 16; ++h) {
-        float v[16];
-        ptx::acc_ld<16>(a_row + lp * N + col0 + 16 * h, v);
+        for (int h = 0; h < NH / 16; ++h) {
+          float v[16];
+          ptx::acc_ld<16>(a_row + lp * N + col0 + 16 * h, v);
 #pragma unroll
-        for (int k = 0; k < 4; ++k) {
-          const float4 bb = reinterpret_cast<const float4*>(&s_col[0][col0 + 16 * h])[k];
-          const float x0 = v[4 * k] + bb.x, x1 = v[4 * k + 1] + bb.y, x2 = v[4 * k + 2] + bb.z, x3 = v[4 * k + 3] + bb.w;
-          s1 += (x0 + x1) + (x2 + x3);
-          s2 = fmaf(x0, x0, s2); s2 = fmaf(x1, x1, s2); s2 = fmaf(x2, x2, s2); s2 = fmaf(x3, x3, s2);
+          for (int k = 0; k < 4; ++k) {
+            const float4 bb = reinterpret_cast<const float4*>(&s_col[0][col0 + 16 * h])[k];
+            const float x0 = v[4 * k] + bb.x, x1 = v[4 * k + 1] + bb.y, x2 = v[4 * k + 2] + bb.z, x3 = v[4 * k + 3] + bb.w;
+            s1 += (x0 + x1) + (x2 + x3);
+            s2 = fmaf(x0, x0, s2); s2 = fmaf(x1, x1, s2); s2 = fmaf(x2, x2, s2); s2 = fmaf(x3, x3, s2);
+          }
         }
       }
+      // one group per CTA tile: warps q and q + 4 hold its two column halves of the same rows; both threads of a row add
+      // the halves in the same order, so they normalise with the same statistics
+      const bool whole_tile = p.C_out == 8 * N;
+      if (whole_tile) {
+        s_stat[threadIdx.x] = make_float2(s1, s2);
+        ptx::named_bar_sync(1, kPsEpiThreads);
+        const float2 lo = s_stat[threadIdx.x & 127], hi = s_stat[(threadIdx.x & 127) + 128];
+        s1 = lo.x + hi.x; s2 = lo.y + hi.y;
+      }
+      const float inv_cnt = 1.f / (float)(P * (whole_tile ? N : NH));
+      const float mean = s1 * inv_cnt;
+      ga = rsqrt_ftz(fmaxf(fmaf(s2, inv_cnt, -mean * mean), 0.f) + p.gn_eps);
+      gc = -mean * ga;
     }
-    const float inv_cnt = 1.f / (float)(P * NH);
-    const float mean = s1 * inv_cnt;
-    const float ga = rsqrt_ftz(fmaxf(fmaf(s2, inv_cnt, -mean * mean), 0.f) + p.gn_eps);
-    const float gc = -mean * ga;
 
     // ---- pass 2: normalise, affine, Mish, additive terms, store; 16-column chunks
     const bool add_res = p.res != nullptr;
@@ -314,7 +335,7 @@ conv_ps_kernel(const __grid_constant__ ConvPsParams p, const int* __restrict__ i
         float resv[16];
 #pragma unroll
         for (int j = 0; j < 16; ++j) resv[j] = 0.f;
-        if (valid) load_row<16>(p.res, (int64_t)rb * p.res_bstride + (int64_t)lp * p.res_lstride + n_off + n0, kActDtype, resv);
+        if (valid) load_row<16>(p.res, (int64_t)rb * p.res_bstride + (int64_t)lp * p.res_lstride + ch0 + n0, kActDtype, resv);
 #pragma unroll
         for (int j = 0; j < 16; ++j) addv[j] += resv[j];
       }
@@ -333,13 +354,22 @@ conv_ps_kernel(const __grid_constant__ ConvPsParams p, const int* __restrict__ i
       const float4* ga4 = reinterpret_cast<const float4*>(&s_col[1][n0]);
       const float4* be4 = reinterpret_cast<const float4*>(&s_col[2][n0]);
       float o[16];
+      if (p.bias_only) {
 #pragma unroll
-      for (int k = 0; k < 4; ++k) {
-        const float4 bb = b4[k], gm = ga4[k], be = be4[k];
-        o[4 * k + 0] = mish_fma(fmaf(fmaf(v[4 * k + 0] + bb.x, ga, gc), gm.x, be.x), addv[4 * k + 0]);
-        o[4 * k + 1] = mish_fma(fmaf(fmaf(v[4 * k + 1] + bb.y, ga, gc), gm.y, be.y), addv[4 * k + 1]);
-        o[4 * k + 2] = mish_fma(fmaf(fmaf(v[4 * k + 2] + bb.z, ga, gc), gm.z, be.z), addv[4 * k + 2]);
-        o[4 * k + 3] = mish_fma(fmaf(fmaf(v[4 * k + 3] + bb.w, ga, gc), gm.w, be.w), addv[4 * k + 3]);
+        for (int k = 0; k < 4; ++k) {
+          const float4 bb = b4[k];
+          o[4 * k + 0] = v[4 * k + 0] + bb.x; o[4 * k + 1] = v[4 * k + 1] + bb.y;
+          o[4 * k + 2] = v[4 * k + 2] + bb.z; o[4 * k + 3] = v[4 * k + 3] + bb.w;
+        }
+      } else {
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+          const float4 bb = b4[k], gm = ga4[k], be = be4[k];
+          o[4 * k + 0] = mish_fma(fmaf(fmaf(v[4 * k + 0] + bb.x, ga, gc), gm.x, be.x), addv[4 * k + 0]);
+          o[4 * k + 1] = mish_fma(fmaf(fmaf(v[4 * k + 1] + bb.y, ga, gc), gm.y, be.y), addv[4 * k + 1]);
+          o[4 * k + 2] = mish_fma(fmaf(fmaf(v[4 * k + 2] + bb.z, ga, gc), gm.z, be.z), addv[4 * k + 2]);
+          o[4 * k + 3] = mish_fma(fmaf(fmaf(v[4 * k + 3] + bb.w, ga, gc), gm.w, be.w), addv[4 * k + 3]);
+        }
       }
       if (p.out_tma) {
         // 32 trajectories (lanes) x 16 columns of position lp through shared memory and ONE bulk store: a warp-level st.global
@@ -366,11 +396,11 @@ conv_ps_kernel(const __grid_constant__ ConvPsParams p, const int* __restrict__ i
         ptx::fence_proxy_async();
         __syncwarp();
         if (lane == 0) {
-          ptx::tma_store_3d(&p.tm_out, stg, n_off + n0, lp, b0 + 32 * q);
+          ptx::tma_store_3d(&p.tm_out, stg, ch0 + n0, lp * p.phases + ph, b0 + 32 * q);
           ptx::bulk_commit_group();
         }
       } else if (valid) {
-        store_row<16>(p.out, (int64_t)b * p.out_bstride + (int64_t)lp * p.out_lstride + n_off + n0, kActDtype, o);
+        store_row<16>(p.out, (int64_t)b * p.out_bstride + (int64_t)(lp * p.phases + ph) * p.out_lstride + ch0 + n0, kActDtype, o);
       }
     }
     if (lane == 0) ptx::bulk_wait_group<0>();        // the bulk stores are complete before the CTA retires
@@ -385,9 +415,12 @@ conv_ps_kernel(const __grid_constant__ ConvPsParams p, const int* __restrict__ i
 constexpr int kPsPositions = 4;
 constexpr int kPsKC = 32;            // channel chunk: 32 (SWIZZLE_64B tiles, 4-stage ring) pipelines better than 64 (2 stages)
 
-// CTA tile width: a quarter of the layer (two GroupNorm groups); 0 = the kernel is not instantiated for this layer
+// CTA tile width: a quarter of the layer (two GroupNorm groups), an eighth (one group) for the 256-wide layers with a shortcut
+// conv, whose 2 x 4 x 64 accumulator columns would not fit over the ring, and 64 columns (inside one phase) for a two-phase
+// transposed conv; 0 = the kernel is not instantiated for this layer
 inline int conv_ps_width(const cds_conv_op& c) {
-  if (c.C_out == 256) return 64;
+  if (c.phases == 2) return c.C_out >= 128 && c.C_out % 64 == 0 ? 64 : 0;
+  if (c.C_out == 256) return c.res_w ? 32 : 64;
   if (c.C_out == 128) return 32;
   return 0;
 }
@@ -395,10 +428,13 @@ inline int conv_ps_width(const cds_conv_op& c) {
 // Can the position-sliced kernel serve this op?  (a subset of conv_tc_eligible: same layouts, same weight packing)
 inline bool conv_ps_eligible(const cds_conv_op& c) {
   if (!conv_tc_eligible(c)) return false;
-  if (c.L_in != kPsPositions || c.L_out != kPsPositions || c.stride != 1 || c.phases != 1) return false;
+  if (c.L_in != kPsPositions || c.L_out != kPsPositions || c.stride != 1 || conv_ps_width(c) == 0) return false;
   if (c.taps < 1 || c.taps > 5 || (c.taps & 1) == 0 || c.pad != c.taps / 2) return false;
-  if (c.groups != 8 || c.act != CDS_ACT_MISH || conv_ps_width(c) == 0) return false;
-  if (c.res_w && conv_ps_width(c) > 32) return false;    // 2 x 4 x 64 accumulator columns do not fit over the ring: conv_tc
+  if (c.phases == 1) {
+    if (c.groups != 8 || c.act != CDS_ACT_MISH) return false;
+  } else if (c.phases != 2 || c.taps != 3 || c.groups != 0 || c.act != CDS_ACT_NONE || c.res || c.res_w || c.shift.step) {
+    return false;                                        // the upsample of the UNets: bias only
+  }
   if (c.C_in % 64 != 0 || (c.res_w && c.res_C % 64 != 0)) return false;
   if (c.bias.sample || c.scale.step || c.scale.sample || c.shift.sample) return false;
   if (conv_is_tf32(c)) { if (c.out_dtype != CDS_TF32 || (c.res && c.res_dtype == CDS_BF16)) return false; }
@@ -436,7 +472,7 @@ inline bool conv_ps_prepare(const cds_conv_op& c, ConvPsLaunch* out) {
     if (!encode_act_map(&p.tm_a, c.in, 3, dims, str, box, kc, tf32)) return false;
   }
   {
-    uint64_t dims[2] = {(uint64_t)c.C_in, (uint64_t)c.taps * c.C_out};
+    uint64_t dims[2] = {(uint64_t)c.C_in, (uint64_t)c.taps * c.C_out * c.phases};
     uint64_t str[1] = {(uint64_t)c.C_in};
     uint32_t box[2] = {(uint32_t)ke, (uint32_t)L.n};
     if (!encode_act_map(&p.tm_b, c.w, 2, dims, str, box, kc, tf32)) return false;
@@ -453,8 +489,9 @@ inline bool conv_ps_prepare(const cds_conv_op& c, ConvPsLaunch* out) {
     if (!encode_act_map(&p.tm_b2, c.res_w, 2, d2, s2, b2, kc, tf32)) return false;
   }
   p.batch = c.batch; p.C_out = c.C_out; p.taps = c.taps;
+  p.phases = c.phases; p.bias_only = c.groups == 0;
   p.kchunks = c.C_in / ke; p.kchunks2 = L.has_res ? c.res_C / ke : 0;
-  p.n_tiles = c.C_out / L.n;
+  p.n_tiles = c.C_out * c.phases / L.n;
   p.in_batch_mod = c.in_batch_mod; p.res_batch_mod = c.res_batch_mod;
   p.bias = c.bias; p.shift = c.shift;
   p.gn_gamma = c.gn_gamma; p.gn_beta = c.gn_beta; p.gn_eps = c.gn_eps;
@@ -466,7 +503,7 @@ inline bool conv_ps_prepare(const cds_conv_op& c, ConvPsLaunch* out) {
     PFN_encodeTiled enc = get_encode_tiled();
     const bool ok = ((uintptr_t)c.out % 16) == 0 && ((int64_t)c.out_lstride * oes) % 16 == 0 && ((int64_t)c.out_bstride * oes) % 16 == 0 &&
                     !getenv("CDS_NO_TMA_STORE");
-    cuuint64_t gdim[3] = {(cuuint64_t)c.C_out, (cuuint64_t)c.L_out, (cuuint64_t)c.batch};
+    cuuint64_t gdim[3] = {(cuuint64_t)c.C_out, (cuuint64_t)(c.L_out * c.phases), (cuuint64_t)c.batch};
     cuuint64_t gstr[2] = {(cuuint64_t)c.out_lstride * oes, (cuuint64_t)c.out_bstride * oes};
     cuuint32_t bx[3] = {16u, 1u, 32u};
     cuuint32_t es[3] = {1u, 1u, 1u};

@@ -11,9 +11,12 @@ process of its own, so that each one loads only its own libcds.so.
    the same numbers bench.py logs as ``op NN conv ...``), in ``--windows`` windows that alternate the two builds; each
    window is the mean of 20 profiles.  Reported per operator as median (min..max) over the windows.
 3. ``bench.py --steps 5 --warmup 3 --no-cpu-baseline --no-eager-baseline --dump-outputs`` ``--bench-runs`` times per
-   build, alternating: the headline values, the other configurations', and x0.npy, which must be byte-identical.
+   build, alternating: the headline values, the other configurations', and x0.npy.  The runs of one build must be
+   byte-identical; between the builds the largest difference is reported (a change of kernel for an operator sums in
+   another order).
 
-Writes OUT/ps_ab.json and prints a summary; exits 1 if any output differs.  Needs a GPU.
+The operators are matched by shape; the kernel family each build picks is reported beside them.  Writes OUT/ps_ab.json
+and prints a summary; exits 1 if a ps_* case differs or a build's x0.npy differs between its runs.  Needs a GPU.
 """
 import argparse
 import json
@@ -73,15 +76,17 @@ def worker_profile(root):
         plan.x.copy_(torch.randn(plan.x.shape, generator=g, device="cuda:0") * 0.5)
         stream = torch.cuda.current_stream().cuda_stream
         plan.handle.profile(50, stream, len(ops))
-        desc = []
+        desc, fams = [], []
         for op in ops:
             if op.kind == 0:
                 c = op.u.conv
                 desc.append(f"conv L{c.L_in}->{c.L_out * c.phases} C{c.C_in}->{c.C_out} k{c.taps}"
-                            f"{' resW' if c.res_w else ''} {cabi.conv_choice(c)['family']}")
+                            f"{' resW' if c.res_w else ''}")
+                fams.append(cabi.conv_choice(c)["family"])
             else:
                 desc.append(f"kind {op.kind}")
-        print(json.dumps({"ready": True, "ops": desc}), flush=True)
+                fams.append("")
+        print(json.dumps({"ready": True, "ops": desc, "families": fams}), flush=True)
         for line in sys.stdin:
             if line.strip() != "profile":
                 break
@@ -111,13 +116,14 @@ def compare_cases(roots, out):
 
 
 def profile_windows(roots, windows):
-    procs, ops = {}, None
+    procs, ops, fams = {}, None, {}
     for tag, root in roots.items():
         procs[tag] = subprocess.Popen([sys.executable, __file__, "--worker", "profile", "--root", root],
                                       stdin=subprocess.PIPE, stdout=subprocess.PIPE, text=True)
         hello = json.loads(procs[tag].stdout.readline())
         assert ops is None or ops == hello["ops"], "the two builds lowered different programs"
         ops = hello["ops"]
+        fams[tag] = hello["families"]
     times = {tag: [] for tag in roots}
     try:
         for _ in range(windows):
@@ -134,18 +140,19 @@ def profile_windows(roots, windows):
         row = {"op": i, "what": name}
         for tag in roots:
             us = [w[i] * 1e3 for w in times[tag]]
-            row[tag] = {"median_us": statistics.median(us), "min_us": min(us), "max_us": max(us)}
+            row[tag] = {"median_us": statistics.median(us), "min_us": min(us), "max_us": max(us), "family": fams[tag][i]}
         rows.append(row)
     totals = {tag: [sum(w) * 1e3 for w in times[tag]] for tag in roots}
     return rows, totals
 
 
-def bench_runs(roots, runs, out):
+def bench_runs(roots, runs, out, tmp):
+    import numpy as np
     res = {tag: [] for tag in roots}
     x0 = {}
     for r in range(runs):
         for tag, root in roots.items():
-            dump = os.path.join(out, f"x0_{tag}_{r}")
+            dump = os.path.join(tmp, f"x0_{tag}_{r}")
             p = subprocess.run([sys.executable, "bench.py", "--steps", "5", "--warmup", "3", "--no-cpu-baseline",
                                 "--no-eager-baseline", "--dump-outputs", dump], cwd=root, capture_output=True, text=True)
             with open(os.path.join(out, f"bench_{tag}_{r}.log"), "w") as f:
@@ -157,9 +164,13 @@ def bench_runs(roots, runs, out):
             res[tag].append({"value": line["value"], "ms_per_step": line["ms_per_step"], "other_configs": others,
                              "clocks": line.get("clocks")})
             x0[(tag, r)] = open(os.path.join(dump, "x0.npy"), "rb").read()
-    ref = x0[("base", 0)]
-    x0_differ = sorted(f"{t}/{r}" for (t, r), v in x0.items() if v != ref)
-    return res, x0_differ
+    nondet = sorted(f"{t}/{r}" for (t, r), v in x0.items() if v != x0[(t, 0)])
+    load = lambda t: np.load(os.path.join(tmp, f"x0_{t}_0", "x0.npy")).astype(np.float64)
+    base, new = load("base"), load("new")
+    diff = {"max_abs": float(np.abs(new - base).max()), "max_abs_base": float(np.abs(base).max()),
+            "max_rel": float((np.abs(new - base) / np.maximum(np.abs(base), 1e-30)).max()),
+            "elements_differ": int((new != base).sum()), "elements": int(base.size)}
+    return res, nondet, diff
 
 
 def main():
@@ -182,27 +193,31 @@ def main():
     args.out = os.path.abspath(args.out)
     os.makedirs(args.out, exist_ok=True)
     report = {"gpu_before": _gpu_info(), "roots": roots}
-    report["cases"] = compare_cases(roots, args.out)
+    import tempfile
+    with tempfile.TemporaryDirectory() as tmp:
+        report["cases"] = compare_cases(roots, tmp)
     print(f"ps cases: {len(report['cases']['cases'])} compared, differ: {report['cases']['differ']}", flush=True)
     rows, totals = profile_windows(roots, args.windows)
     report["per_op"], report["iteration_total_us"] = rows, totals
     for row in rows:
         if "conv" in row["what"]:
             b, n = row["base"], row["new"]
-            print(f"op {row['op']:2d} {row['what']:40s} base {b['median_us']:7.1f} ({b['min_us']:.1f}..{b['max_us']:.1f})"
-                  f"  new {n['median_us']:7.1f} ({n['min_us']:.1f}..{n['max_us']:.1f}) us", flush=True)
+            print(f"op {row['op']:2d} {row['what']:34s} base {b['family']:2s} {b['median_us']:7.1f} ({b['min_us']:.1f}..{b['max_us']:.1f})"
+                  f"  new {n['family']:2s} {n['median_us']:7.1f} ({n['min_us']:.1f}..{n['max_us']:.1f}) us", flush=True)
     for tag, t in totals.items():
         print(f"iteration total {tag}: median {statistics.median(t):.1f} ({min(t):.1f}..{max(t):.1f}) us", flush=True)
-    report["bench"], report["x0_differ"] = bench_runs(roots, args.bench_runs, args.out)
+    with tempfile.TemporaryDirectory() as tmp:
+        report["bench"], report["x0_nondeterministic"], report["x0_base_vs_new"] = bench_runs(roots, args.bench_runs, args.out, tmp)
     for tag, runs in report["bench"].items():
         print(f"bench {tag}: " + ", ".join(f"{r['value']:.0f}" for r in runs) + " traj/s; other configs "
               + "; ".join(json.dumps(r["other_configs"]) for r in runs), flush=True)
-    print(f"x0.npy differs from base run 0: {report['x0_differ']}", flush=True)
+    print(f"x0.npy differs from its own build's run 0: {report['x0_nondeterministic']}", flush=True)
+    print(f"x0.npy, new vs base: {json.dumps(report['x0_base_vs_new'])}", flush=True)
     report["gpu_after"] = _gpu_info()
     print("gpu:", report["gpu_before"], "/", report["gpu_after"], flush=True)
     with open(os.path.join(args.out, "ps_ab.json"), "w") as f:
         json.dump(report, f, indent=1)
-    return 1 if report["cases"]["differ"] or report["x0_differ"] else 0
+    return 1 if report["cases"]["differ"] or report["x0_nondeterministic"] else 0
 
 
 if __name__ == "__main__":
