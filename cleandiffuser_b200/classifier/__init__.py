@@ -1,9 +1,13 @@
 """Classifiers for classifier guidance: ``logp(x, noise, c)`` and its input gradient ``gradients(x, noise, c)``.
 
-Same surface as the reference's (cleandiffuser/classifier/base.py, rew_classifiers.py): ``model`` is trained, ``model_ema`` (an
-eval-mode copy updated by ``ema_update``) is what ``logp`` evaluates.  When a ``CumRewClassifier`` over ``HalfJannerUNet1d``
-or a ``QGPOClassifier`` over ``QGPONNClassifier`` guides ``sample()``, the engine evaluates the input gradient inside the
-replayed loop and ``gradients`` is not called.
+Same surface as the reference's (cleandiffuser/classifier/base.py, rew_classifiers.py, mse_classifier.py,
+qgpo_classifier.py): ``model`` is trained, ``model_ema`` (an eval-mode copy updated by ``ema_update``) is what ``logp``
+evaluates.  When one of these guides ``sample()``, the engine evaluates the input gradient inside the replayed loop and
+``gradients`` is not called:
+  - ``CumRewClassifier`` over ``HalfJannerUNet1d``, or over ``MLPNNClassifier`` with ``out_dim = 1``;
+  - ``MSEClassifier`` over ``MLPNNClassifier`` (ReLU, SiLU or Mish hidden layers, identity output), given ``condition_cg``;
+  - ``QGPOClassifier`` over ``QGPONNClassifier``, given ``condition_cg``.
+Any other classifier keeps a host callback between the denoiser and the update (``engine/lower.py``, ``guidable``).
 """
 from copy import deepcopy
 from typing import Dict, Optional
@@ -96,6 +100,25 @@ class CumRewClassifier(BaseClassifier):
 
     def logp(self, x, noise, c=None):
         return self.model_ema(x, noise)
+
+
+class MSEClassifier(BaseClassifier):
+    """Gaussian log-likelihood of a condition c under a regression network (mse_classifier.py):
+    ``logp = -temperature * mean((model_ema(x, noise) - c)^2, -1)``, trained with ``mse_loss(model(x, noise), y)``.
+    ``temperature`` is a plain attribute; a guided ``sample()`` reads it on every call."""
+
+    def __init__(self, nn_classifier: torch.nn.Module, temperature: float = 1.0, ema_rate: float = 0.995,
+                 grad_clip_norm: Optional[float] = None, optim_params: Optional[dict] = None, device: str = "cpu"):
+        super().__init__(nn_classifier, ema_rate, grad_clip_norm, optim_params, device)
+        self.temperature = temperature
+
+    def loss(self, x: torch.Tensor, noise: torch.Tensor, y: torch.Tensor):
+        return F.mse_loss(self.model(x, noise), y)
+
+    def logp(self, x: torch.Tensor, noise: torch.Tensor, c: torch.Tensor):
+        """x (batch, x_dim), noise (batch,), c (batch, out_dim) -> (batch, 1)"""
+        pred_y = self.model_ema(x, noise)
+        return -self.temperature * ((pred_y - c) ** 2).mean(-1, keepdim=True)
 
 
 class QGPOClassifier(BaseClassifier):

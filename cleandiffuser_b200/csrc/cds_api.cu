@@ -212,7 +212,7 @@ int validate(const cds_op& op, Step* out) {
     case CDS_OP_STASH: {
       const cds_stash_op& t = op.u.stash;
       if (t.n <= 0 || !t.src || (!t.dst && !t.act_out)) return fail(CDS_ERR_INVALID, "stash: bad arguments");
-      if (t.act_out && t.act != CDS_ACT_NONE && t.act != CDS_ACT_MISH && t.act != CDS_ACT_SILU)
+      if (t.act_out && t.act != CDS_ACT_NONE && t.act != CDS_ACT_MISH && t.act != CDS_ACT_SILU && t.act != CDS_ACT_RELU)
         return fail(CDS_ERR_UNSUPPORTED, "stash: act %d", t.act);
       return CDS_OK;
     }
@@ -226,7 +226,7 @@ int validate(const cds_op& op, Step* out) {
       const cds_dgrad_op& d = op.u.dgrad;
       if (d.rows <= 0 || d.N <= 0 || d.K <= 0 || !d.dz || !d.w || !d.out || d.ldz < d.N || d.ldw < d.K || d.ldo < d.K)
         return fail(CDS_ERR_INVALID, "dgrad: bad arguments");
-      if (d.act != CDS_ACT_NONE && d.act != CDS_ACT_MISH && d.act != CDS_ACT_SILU)
+      if (d.act != CDS_ACT_NONE && d.act != CDS_ACT_MISH && d.act != CDS_ACT_SILU && d.act != CDS_ACT_RELU)
         return fail(CDS_ERR_UNSUPPORTED, "dgrad: act %d", d.act);
       if (d.act != CDS_ACT_NONE && !d.z) return fail(CDS_ERR_INVALID, "dgrad: activation derivative without a pre-activation");
       return CDS_OK;

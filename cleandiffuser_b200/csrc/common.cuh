@@ -49,6 +49,7 @@ __device__ __forceinline__ float apply_act(int act, float x) {
     case CDS_ACT_MISH_SILU: return act_silu(act_mish(x));
     case CDS_ACT_LEAKY_RELU: return x > 0.f ? x : 0.01f * x;
     case CDS_ACT_GELU_ERF: return 0.5f * x * (1.f + erff(x * 0.7071067811865476f));
+    case CDS_ACT_RELU: return x > 0.f ? x : 0.f;
     default: return x;
   }
 }

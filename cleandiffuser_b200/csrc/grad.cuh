@@ -24,7 +24,18 @@ __device__ __forceinline__ float silu_grad(float x) {
   return sig * (1.f + x * (1.f - sig));
 }
 
-__device__ __forceinline__ float act_grad(int act, float x) { return act == CDS_ACT_SILU ? silu_grad(x) : mish_grad(x); }
+// d/dx relu(x), ATen's threshold_backward: 1 where x > 0, else 0 (0 at x == 0)
+__device__ __forceinline__ float relu_grad(float x) { return x > 0.f ? 1.f : 0.f; }
+
+// the derivative of the activations CDS_OP_DGRAD accepts (cds_api.cu rejects every other act before a launch)
+__device__ __forceinline__ float act_grad(int act, float x) {
+  switch (act) {
+    case CDS_ACT_SILU: return silu_grad(x);
+    case CDS_ACT_RELU: return relu_grad(x);
+    case CDS_ACT_MISH:
+    default: return mish_grad(x);
+  }
+}
 
 static __global__ void __launch_bounds__(256) stash_kernel(const cds_stash_op p, const int* __restrict__ iter_ptr) {
   const int iter = *iter_ptr;

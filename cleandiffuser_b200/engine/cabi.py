@@ -10,7 +10,7 @@ import os
 
 _LIB_PATH = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "csrc", "libcds.so")
 
-ABI_VERSION = 8
+ABI_VERSION = 9
 OPF_BRANCH_SHIFT = 8   # cds_op.flags bits 8..15: branch index (independent chains run on parallel streams)
 OPF_ONCE = 1          # cds_op.flags: run once per plan run (before its first iteration), not in every iteration
 OP_CONV, OP_UPDATE, OP_LNMOD, OP_ATTN, OP_PREP, OP_CAST, OP_MHA = range(7)
@@ -18,6 +18,7 @@ OP_STASH, OP_UPDATE_BWD, OP_DGRAD, OP_WGRAD = 7, 8, 9, 10      # backward operat
 OP_GN, OP_GN_BWD, OP_GUIDE = 11, 12, 13       # classifier guidance inside the loop (csrc/classifier.cuh)
 OP_HEAD_GRAD = 14                             # QGPOClassifier's energy head and the seed of its backward (csrc/classifier.cuh)
 ACT_NONE, ACT_MISH, ACT_SILU, ACT_GELU_TANH, ACT_MISH_SILU, ACT_LEAKY_RELU, ACT_GELU_ERF = range(7)
+ACT_RELU = 7                                  # nn.ReLU (MLPNNClassifier's default activation): CDS_OP_STASH / CDS_OP_DGRAD
 MATH_FP32, MATH_BF16_TC, MATH_TF32_TC = 0, 1, 2
 TC_MODES = (MATH_BF16_TC, MATH_TF32_TC)
 F32, BF16, TF32 = 0, 1, 2      # cds_dtype; TF32 = fp32 storage, values rounded to TF32 when written

@@ -1045,14 +1045,22 @@ def lower_denoiser(p: Program, net: nn.Module, x: View, x_shape, has_cond: bool,
 def guidable(clf, x_shape, cond_cg=None) -> Optional[str]:
     """None when ``lower_classifier_grad`` can put the input gradient of ``clf`` at x_t into the loop, else the reason it cannot.
     The classifiers are recognised structurally (class names and the attributes the lowering reads), so that the reference's own
-    instances qualify: a CumRewClassifier over a HalfJannerUNet1d, or a QGPOClassifier over a QGPONNClassifier guided with a
+    instances qualify: a CumRewClassifier over a HalfJannerUNet1d or over an out_dim-1 MLPNNClassifier, an MSEClassifier over an
+    MLPNNClassifier guided with a per-trajectory target ``cond_cg``, or a QGPOClassifier over a QGPONNClassifier guided with a
     per-trajectory condition ``cond_cg`` (the observations)."""
     name = type(clf).__name__
+    net_name = type(getattr(clf, "model_ema", None)).__name__
     if name == "CumRewClassifier":
+        if net_name == "MLPNNClassifier":
+            return _mlp_classifier_reason(clf, x_shape, cond_cg, mse=False)
         return _half_janner_reason(clf, x_shape)
+    if name == "MSEClassifier":
+        if net_name != "MLPNNClassifier":
+            return f"classifier network {net_name} (MLPNNClassifier only)"
+        return _mlp_classifier_reason(clf, x_shape, cond_cg, mse=True)
     if name == "QGPOClassifier":
         return _qgpo_reason(clf, x_shape, cond_cg)
-    return f"classifier {name} (CumRewClassifier or QGPOClassifier only)"
+    return f"classifier {name} (CumRewClassifier, MSEClassifier or QGPOClassifier only)"
 
 
 def lower_classifier_grad(p: Program, clf, x: View) -> View:
@@ -1060,13 +1068,15 @@ def lower_classifier_grad(p: Program, clf, x: View) -> View:
     as a view shaped like ``x`` (its channels may include x's zero padding)"""
     if type(clf).__name__ == "QGPOClassifier":
         return lower_qgpo_grad(p, clf, x)
+    if type(clf.model_ema).__name__ == "MLPNNClassifier":
+        return lower_mlp_classifier_grad(p, clf, x)
     return lower_half_janner_grad(p, clf, x)
 
 
 def _half_janner_reason(clf, x_shape) -> Optional[str]:
     net = getattr(clf, "model_ema", None)
     if type(net).__name__ != "HalfJannerUNet1d":
-        return f"classifier network {type(net).__name__} (HalfJannerUNet1d only)"
+        return f"classifier network {type(net).__name__} (HalfJannerUNet1d or MLPNNClassifier only)"
     if net.training:
         return "classifier model_ema in train mode"
     if len(x_shape) != 2 or x_shape[0] & (x_shape[0] - 1):
@@ -1117,6 +1127,59 @@ def _qgpo_reason(clf, x_shape, cond_cg) -> Optional[str]:
         return "no classifier condition (condition_cg=None)"
     if cond_cg.dim() != 2 or cond_cg.shape[1] != obs.in_features:
         return "classifier condition does not match obs_proj"
+    return None
+
+
+# hidden activations the lowered Linear stacks fuse into CDS_OP_STASH / CDS_OP_DGRAD
+_STACK_ACTS = {"ReLU": cabi.ACT_RELU, "SiLU": cabi.ACT_SILU, "Mish": cabi.ACT_MISH}
+
+
+def _mlp_classifier_layers(net):
+    """(hidden Linears, activation module type name, output Linear, out_activation type name) of MLPNNClassifier.mlp, or a
+    string saying which part is not an Mlp of Linear + activation stages under a Linear and an output activation"""
+    seq = getattr(getattr(net, "mlp", None), "mlp", None)
+    if not isinstance(seq, nn.Sequential) or len(seq) < 2 or not isinstance(seq[-2], nn.Linear):
+        return "classifier mlp is not an Mlp"
+    stages = list(seq)[:-2]
+    if not stages:
+        return "classifier mlp has no hidden layer"
+    if not all(isinstance(s, nn.Sequential) and len(s) == 2 and isinstance(s[0], nn.Linear) for s in stages):
+        return "classifier mlp hidden stages are not Linear + activation"
+    acts = sorted({type(s[1]).__name__ for s in stages})
+    if len(acts) != 1:
+        return f"classifier hidden activations differ ({', '.join(acts)})"
+    return [s[0] for s in stages], acts[0], seq[-2], type(seq[-1]).__name__
+
+
+def _emb_width(net) -> int:
+    """width of net.map_noise's output (the time-embedding columns of the first Linear)"""
+    dev = next(net.parameters()).device
+    with torch.no_grad():
+        return int(net.map_noise(torch.zeros(1, device=dev)).shape[-1])
+
+
+def _mlp_classifier_reason(clf, x_shape, cond_cg, mse: bool) -> Optional[str]:
+    net = clf.model_ema
+    if net.training:
+        return "classifier model_ema in train mode"
+    layers = _mlp_classifier_layers(net)
+    if isinstance(layers, str):
+        return layers
+    hidden, act, lin_o, out_act = layers
+    if act not in _STACK_ACTS:
+        return f"classifier activation {act} (ReLU, SiLU or Mish only)"
+    if out_act != "Identity":
+        return f"classifier out_activation {out_act} (Identity only)"
+    if any(a.out_features != b.in_features for a, b in zip(hidden, hidden[1:] + [lin_o])):
+        return "classifier mlp widths do not chain"
+    if len(x_shape) != 1 or hidden[0].in_features != x_shape[0] + _emb_width(net):
+        return "classifier x_dim does not match x"
+    if not mse:
+        return None if lin_o.out_features == 1 else f"classifier out_dim {lin_o.out_features} (1 only under CumRewClassifier)"
+    if cond_cg is None:
+        return "no classifier condition (condition_cg=None)"
+    if cond_cg.dim() != 2 or cond_cg.shape[1] != lin_o.out_features:
+        return "classifier condition is not (batch, out_dim)"
     return None
 
 
@@ -1304,6 +1367,50 @@ def _dgrad(p: Program, dz: torch.Tensor, w: torch.Tensor, out: torch.Tensor, z: 
     p.ops.append(op)
 
 
+class _LinearActStack:
+    """A stack of hidden Linears z_k = W_k h_{k-1} + b_k, h_k = act(z_k) inside a classifier's input gradient, forward and
+    backward, for one activation ``act`` (CDS_ACT_RELU / SILU / MISH).  The pre-activations z_k stay in dense fp32 buffers for
+    the backward; every h_k is CDS_OP_STASH without a slot."""
+
+    def __init__(self, p: Program, hidden: List[nn.Linear], act: int):
+        self.p, self.hidden, self.act = p, hidden, act
+        self.zs: List[View] = []
+
+    def dense(self, width: int) -> View:
+        """an exact fp32 (rows, 1, width) activation"""
+        return View(self.p.buf(self.p.rows, 1, width), 1, width)
+
+    def forward(self, h: View, first_w: WSpec, first_bias: cabi.Vec, act_last: bool) -> View:
+        """z_1 = first_w h + first_bias (the first Linear's columns that read h, its other columns and bias folded into the
+        bias rows), z_k (CDS_OP_CONV), h_k = act(z_k) (CDS_OP_STASH) between them and, when ``act_last``, after the last:
+        -> h_n, or z_n when not ``act_last``"""
+        p = self.p
+        for k, lin in enumerate(self.hidden):
+            z = self.dense(lin.out_features)
+            if k == 0:
+                p.conv(h, first_w, z, bias=first_bias)
+            else:
+                p.conv(h, w_linear(lin.weight), z, bias=_const_vec(p.packed(lambda m=lin: m.bias)))
+            self.zs.append(z)
+            h = z
+            if act_last or k + 1 < len(self.hidden):
+                h = self.dense(lin.out_features)
+                _act_stash(p, z, h, self.act)
+        return h
+
+    def backward(self, seed: torch.Tensor, w_out: torch.Tensor) -> torch.Tensor:
+        """dz_n = (seed W_out) act'(z_n), dz_k = (dz_{k+1} W_{k+1}) act'(z_k) (CDS_OP_DGRAD) -> dz_1 (rows, width of z_1)"""
+        p = self.p
+        up, w_up = seed, w_out
+        for k in range(len(self.hidden) - 1, -1, -1):
+            dz = p.buf(p.rows, self.hidden[k].out_features)
+            _dgrad(p, up, w_up, dz, self.zs[k], self.act)
+            up = dz
+            if k:
+                w_up = p.packed(lambda m=self.hidden[k]: m.weight)
+        return up
+
+
 def lower_qgpo_grad(p: Program, clf, x: View) -> View:
     """Append the input gradient d sum(logp) / d x of ``clf.model_ema`` (a QGPONNClassifier; ``guidable``) at x_t (rows, act_dim)
     to the iteration program -> the gradient as a dense (rows, 1, act_dim) fp32 view.
@@ -1312,7 +1419,7 @@ def lower_qgpo_grad(p: Program, clf, x: View) -> View:
     z_1 = W_1 [obs_proj(c) | act_proj(x) | map_noise(t)] + b_1 = W_1a act_proj(x) + (W_1e map_noise(t) + b_1) + W_1y obs_proj(c)
     Forward: a = act_proj(x) (CDS_OP_CONV);  z_1 (CDS_OP_CONV, its bias the per-iteration row W_1e e(t) + b_1 plus the
     per-trajectory row W_1y obs_proj(c), both filled once per call);  per hidden layer h_k = silu(z_k) (CDS_OP_STASH without a
-    slot) and z_{k+1} (CDS_OP_CONV): the pre-activations stay for the backward.
+    slot) and z_{k+1} (CDS_OP_CONV): the pre-activations stay for the backward (``_LinearActStack``).
     Backward: the seed d logp / d z (CDS_OP_HEAD_GRAD over silu(z_n)), dz_n = (seed W_o) silu'(z_n), ..., dz_1 (CDS_OP_DGRAD
     with SiLU), da = dz_1 W_1a, dx = da W_act (CDS_OP_DGRAD): the reference's factorisation through act_proj, kept so that the
     gradient's summation error stays that of the two products autograd forms."""
@@ -1331,39 +1438,73 @@ def lower_qgpo_grad(p: Program, clf, x: View) -> View:
         samp_tab.copy_(F.linear(net.obs_proj(ctx.cond_cg.to(torch.float32)), lin1.weight[:, :E]))
     p.per_call += [fill_time, fill_cond]
 
-    dense = lambda w: View(p.buf(R, 1, w), 1, w)                 # noqa: E731   exact fp32 activations
-    a = p.conv(x, w_linear(net.act_proj.weight), dense(E), bias=_const_vec(p.packed(lambda: net.act_proj.bias)))
-    zs = []
-    h = a
-    for k, lin in enumerate(hidden):
-        z = dense(lin.out_features)
-        if k == 0:
-            p.conv(h, w_linear(lin.weight, slice(E, 2 * E)), z, bias=_vec(step_tab, samp_tab))
-        else:
-            p.conv(h, w_linear(lin.weight), z, bias=_const_vec(p.packed(lambda m=lin: m.bias)))
-        zs.append(z)
-        if k + 1 < len(hidden):
-            h = dense(lin.out_features)
-            _act_stash(p, z, h, cabi.ACT_SILU)
+    stack = _LinearActStack(p, hidden, cabi.ACT_SILU)
+    a = p.conv(x, w_linear(net.act_proj.weight), stack.dense(E), bias=_const_vec(p.packed(lambda: net.act_proj.bias)))
+    z_n = stack.forward(a, w_linear(lin1.weight, slice(E, 2 * E)), _vec(step_tab, samp_tab), act_last=False)
 
     seed = p.buf(R, 1)
     op = cabi.Op()
     op.kind = cabi.OP_HEAD_GRAD
     q = op.u.head_grad
-    q.rows, q.K, q.h, q.ldh, q.act = R, zs[-1].C, zs[-1].ptr, zs[-1].C, cabi.ACT_SILU
+    q.rows, q.K, q.h, q.ldh, q.act = R, z_n.C, z_n.ptr, z_n.C, cabi.ACT_SILU
     q.w, q.b = p.packed(lambda: lin_o.weight.reshape(-1)).data_ptr(), p.packed(lambda: lin_o.bias).data_ptr()
     q.scale, q.seed = 10.0, seed.data_ptr()
     p.ops.append(op)
 
-    up, w_up = seed, p.packed(lambda: lin_o.weight)
-    for k in range(len(hidden) - 1, -1, -1):
-        dz = p.buf(R, hidden[k].out_features)
-        _dgrad(p, up, w_up, dz, zs[k], cabi.ACT_SILU)
-        up, w_up = dz, p.packed(lambda m=hidden[k]: m.weight)
+    dz1 = stack.backward(seed, p.packed(lambda: lin_o.weight))
     da = p.buf(R, E)
-    _dgrad(p, up, p.packed(lambda: lin1.weight[:, E:2 * E]), da)
+    _dgrad(p, dz1, p.packed(lambda: lin1.weight[:, E:2 * E]), da)
     dx = View(p.buf(R, 1, x.C), 1, x.C)
     _dgrad(p, da, p.packed(lambda: net.act_proj.weight), dx.t)
+    return dx
+
+
+def lower_mlp_classifier_grad(p: Program, clf, x: View) -> View:
+    """Append the input gradient d sum(logp) / d x of ``clf.model_ema`` (an MLPNNClassifier under an MSEClassifier or an
+    out_dim-1 CumRewClassifier; ``guidable``) at x_t (rows, x_dim) to the iteration program -> the gradient as a dense
+    (rows, 1, x.C) fp32 view (x.C may include zero padding channels, whose gradient is zero).
+
+    y = W_o h_n + b_o,  h_k = act(z_k),  z_k = W_k h_{k-1} + b_k,  z_1 = W_1 [x | map_noise(t)] + b_1 = W_1x x + (W_1e e(t) + b_1)
+    Forward (``_LinearActStack``): z_1 (CDS_OP_CONV, its bias the per-iteration row W_1e map_noise(t) + b_1 filled once per
+    call), h_k = act(z_k) (CDS_OP_STASH) and z_{k+1} (CDS_OP_CONV).
+      CumRew head, logp = y (out_dim 1):  the seed d logp / d y = 1, so y itself is not evaluated and h_n not formed.
+      MSE head, logp = -T mean_j (y_j - c_j)^2:  r = W_o h_n + (b_o - c) (CDS_OP_CONV, the per-trajectory bias row b_o - c filled
+      per call from condition_cg) and d logp / d y = -(2 T / out_dim) r.  The factor goes into a copy of W_o that every call
+      refills (T = clf.temperature, read per call): dz_n = (r (-(2 T / out_dim) W_o)) act'(z_n).
+    Backward: dz_n, ..., dz_1 (CDS_OP_DGRAD with act'), dx = dz_1 W_1x (CDS_OP_DGRAD)."""
+    net = clf.model_ema
+    R = p.rows
+    hidden, act, lin_o, _ = _mlp_classifier_layers(net)
+    lin1 = hidden[0]
+    X = lin1.in_features - _emb_width(net)
+    mse = type(clf).__name__ == "MSEClassifier"
+    step_tab = p.buf(p.n_iters, lin1.out_features)
+
+    def fill_time(ctx):
+        step_tab.copy_(F.linear(net.map_noise(ctx.t_all), lin1.weight[:, X:], lin1.bias))
+    fill_time.time_only = True
+    p.per_call.append(fill_time)
+
+    w_1x = lambda: _pad_cin(lin1.weight[:, :X], x.C)                                      # noqa: E731
+    stack = _LinearActStack(p, hidden, _STACK_ACTS[act])
+    h_n = stack.forward(x, w_rows(w_1x), _vec(step=step_tab), act_last=mse)
+    if mse:
+        D = lin_o.out_features
+        target, w_seed = p.buf(R, D), p.buf(D, lin_o.in_features)
+
+        def fill_target(ctx):
+            target.copy_(lin_o.bias[None, :] - ctx.cond_cg.to(torch.float32))
+            w_seed.copy_(lin_o.weight * (-(2.0 * float(clf.temperature) / D)))
+        p.per_call.append(fill_target)
+        r = stack.dense(D)
+        p.conv(h_n, w_linear(lin_o.weight), r, bias=_vec(sample=target))
+        seed = r.t.view(R, D)
+    else:
+        seed, w_seed = p.buf(R, 1), p.packed(lambda: lin_o.weight)
+        seed.fill_(1.0)
+    dz1 = stack.backward(seed, w_seed)
+    dx = stack.dense(x.C)
+    _dgrad(p, dz1, p.packed(w_1x), dx.t.view(R, x.C))
     return dx
 
 

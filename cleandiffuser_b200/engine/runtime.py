@@ -511,7 +511,8 @@ def try_sample(agent, *, model, xt, prior, solver, sample_steps, order, step_val
     ``guide``: optional host callback ``guide(n, i, x_t, pred)`` (n = iteration, i = its loop index) run between the denoiser
     and the update of every iteration (classifier guidance); the loop then runs step by step instead of as a replayed graph --
     unless ``classifier`` (the one ``guide`` evaluates, with weight ``w_cg`` and condition ``cond_cg``) is one ``lower.guidable``
-    accepts (a CumRewClassifier over HalfJannerUNet1d, a QGPOClassifier over QGPONNClassifier with a condition) under
+    accepts (a CumRewClassifier over HalfJannerUNet1d or an out_dim-1 MLPNNClassifier, an MSEClassifier over MLPNNClassifier
+    or a QGPOClassifier over QGPONNClassifier with a condition) under
     CDS_MATH = fp32 | tf32 with one sub-batch chain: its input gradient and the guidance term are then operators of the replayed
     program, and ``guide`` is not called."""
     def decline(cfg_mode):

@@ -5,6 +5,9 @@ parameter names and shapes (cleandiffuser/nn_classifier/half_jannerunet.py), so 
 (``CumRewClassifier``) the engine lowers its forward and input gradient into the replayed loop (``engine/lower.py``,
 ``lower_half_janner_grad``); everything else about it runs in PyTorch.  ``QGPONNClassifier`` (nn_classifier/mlp.py) is QGPO's
 energy network; under ``QGPOClassifier`` guidance its input gradient is lowered the same way (``lower_qgpo_grad``).
+``MLPNNClassifier`` (nn_classifier/mlp.py) is the general-purpose MLP over ``[x | map_noise(t)]``; under ``MSEClassifier``
+guidance, or ``CumRewClassifier`` guidance with ``out_dim = 1``, its input gradient is lowered by
+``lower_mlp_classifier_grad`` when its hidden activation is ReLU, SiLU or Mish and its output activation the identity.
 """
 from typing import List, Optional, Tuple
 
@@ -63,6 +66,21 @@ class HalfJannerUNet1d(BaseNNDiffusion):
         for block, down in (self.mid_block1, self.mid_block2):
             h = down(block(h, emb))
         return self.final_block(torch.cat([h.flatten(1), emb], dim=-1))
+
+
+class MLPNNClassifier(BaseNNDiffusion):
+    """x (b, x_dim), t (b,), y ignored -> (b, out_dim): ``Mlp([x | map_noise(t)])`` with ``activation`` after every hidden
+    Linear (one module instance, as in the reference) and ``out_activation`` after the output Linear.  State-dict keys
+    ``map_noise.*``, ``mlp.mlp.<i>.0.*`` (hidden Linears), ``mlp.mlp.<n>.*`` (output Linear)."""
+
+    def __init__(self, x_dim: int, out_dim: int, emb_dim: int, hidden_dims: List[int], activation: nn.Module = nn.ReLU(),
+                 out_activation: nn.Module = nn.Identity(), timestep_emb_type: str = "positional"):
+        super().__init__(emb_dim, timestep_emb_type)
+        self.mlp = Mlp(in_dim=x_dim + emb_dim, hidden_dims=hidden_dims, out_dim=out_dim, activation=activation,
+                       out_activation=out_activation)
+
+    def forward(self, x: torch.Tensor, t: torch.Tensor, y: Optional[torch.Tensor] = None):
+        return self.mlp(torch.cat([x, self.map_noise(t)], dim=-1))
 
 
 class QGPONNClassifier(BaseNNDiffusion):

@@ -27,6 +27,8 @@
  *   CDS_OP_GUIDE        GroupNorm + Mish over a kept pre-norm input, its backward, and pred += s[iter] * grad (further down)
  *   CDS_OP_HEAD_GRAD    the energy head of QGPO's classifier (qgpo_classifier.py / nn_classifier/mlp.py: 10 tanh(z / 10) over
  *                       an Mlp of Linear + SiLU): z = h . w + b per row and the seed of its backward (further down)
+ *   (no new kind)       classifier guidance with MSEClassifier / CumRewClassifier over MLPNNClassifier (mse_classifier.py,
+ *                       nn_classifier/mlp.py): CDS_OP_CONV, CDS_OP_STASH and CDS_OP_DGRAD with CDS_ACT_RELU / SILU / MISH
  *
  * Conventions
  *  - every function returns 0 on success, a negative cds_status otherwise; cds_last_error() gives the
@@ -53,7 +55,7 @@
 extern "C" {
 #endif
 
-#define CDS_ABI_VERSION 8
+#define CDS_ABI_VERSION 9
 
 typedef enum cds_status {
   CDS_OK = 0,
@@ -74,7 +76,9 @@ typedef enum cds_op_kind { CDS_OP_CONV = 0, CDS_OP_UPDATE = 1, CDS_OP_LNMOD = 2,
 typedef enum cds_act { CDS_ACT_NONE = 0, CDS_ACT_MISH = 1, CDS_ACT_SILU = 2, CDS_ACT_GELU_TANH = 3,
                        CDS_ACT_MISH_SILU = 4 /* silu(mish(x)): DiT's map_emb tail feeding every adaLN (dit.py:26,43,71) */,
                        CDS_ACT_LEAKY_RELU = 5 /* negative slope 0.01 (nn.LeakyReLU default; pearcemlp.py:44) */,
-                       CDS_ACT_GELU_ERF = 6 /* exact GELU 0.5 x (1 + erf(x / sqrt 2)) (nn.GELU default; pearcemlp.py:30) */ } cds_act;
+                       CDS_ACT_GELU_ERF = 6 /* exact GELU 0.5 x (1 + erf(x / sqrt 2)) (nn.GELU default; pearcemlp.py:30) */,
+                       CDS_ACT_RELU = 7 /* max(x, 0); derivative z > 0 ? 1 : 0, 0 at z == 0 like ATen's threshold_backward
+                                           (nn.ReLU, MLPNNClassifier's default activation: nn_classifier/mlp.py) */ } cds_act;
 /* math mode of CDS_OP_CONV:
  *   CDS_MATH_FP32     fp32 CUDA-core FMA (bit-faithful to the fp32 oracle up to summation order)
  *   CDS_MATH_BF16_TC  wgmma tensor cores, bf16 operands and bf16 inter-layer activations, fp32 accumulation
@@ -224,7 +228,7 @@ typedef struct cds_update_op {
  * one captured graph serves every backward iteration like it does every forward one. */
 
 /* dst[iter*dst_iter_stride + i] = src[i] when dst != NULL;  act_out[i] = act(src[i]) when act_out != NULL (i < n); at least one
- * of the two.  act: CDS_ACT_NONE / MISH / SILU */
+ * of the two.  act: CDS_ACT_NONE / MISH / SILU / RELU */
 typedef struct cds_stash_op {
   int64_t n;
   int32_t act;
@@ -253,8 +257,9 @@ typedef struct cds_update_bwd_op {
 
 /* Data gradient of a Linear layer:  out(r, k) [+]= (sum_n dz(r, n) W(n, k)) * act'(z(r, k))
  * dz (rows, N) row stride ldz; W (N, K) row stride ldw (a PyTorch [out, in] weight or a column block of one);
- * z = the stashed pre-activation of the layer's input (z + iter*z_iter_stride, dense (rows, K)), required when act = MISH or SILU
- *     (act' follows ATen: mish_backward, and silu_backward's sig * (1 + z * (1 - sig)));
+ * z = the stashed pre-activation of the layer's input (z + iter*z_iter_stride, dense (rows, K)), required when act = MISH, SILU
+ *     or RELU (act' follows ATen: mish_backward, silu_backward's sig * (1 + z * (1 - sig)), and threshold_backward's
+ *     z > 0 ? 1 : 0);
  * out (rows, K) row stride ldo, overwritten (accumulate = 0) or added to (1); out_sum (dense (rows, K), optional) += result.
  * fp32 CUDA cores; deterministic (every output is one thread's fixed-order sum). */
 typedef struct cds_dgrad_op {
