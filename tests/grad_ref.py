@@ -100,6 +100,11 @@ def wgrad(dz, h, act_kind=cabi.ACT_NONE):
 # (tests/program_audit.py) both apply them.
 U32 = 2.0 ** -24
 TINY = 1e-35          # silu(z) for z < -88, where the fp32 1 + expf(-z) overflows and the kernel returns -0
+# fp32 underflow: Mish(z) below z = -87 (expf(z) leaves the normal range; |Mish(z)| <= 103 e^-87 < TINY, and the kernel's
+# value may be 0), and any product or sum that falls below the normal range 2^-126, keeps only an absolute accuracy.  A
+# relative bound of such a result underflows in fp64 too (|Mish(-700)| ~ 1e-302), so a correctly computed fp32 -0 would
+# exceed it; these absolute terms are ~1e-35 and leave every normal-range bound as it was.
+NORMAL_MIN = 2.0 ** -126
 
 
 def mish_bound(z):
@@ -155,7 +160,7 @@ def dgrad_bound(dz, w, z=None, act_kind=cabi.ACT_NONE, before=None):
         g = grad(z)
         mag, y = mag * np.abs(g), dzw * g
         bound = np.abs(dzw) * grad_bound(z)
-    bound = bound + (dz.shape[1] + 4) * U32 * mag
+    bound = bound + (dz.shape[1] + 4) * (U32 * mag + NORMAL_MIN)
     if before is not None:
         bound = bound + 2 * U32 * (np.abs(np.asarray(before, np.float64)) + np.abs(y))
     return bound
@@ -164,11 +169,14 @@ def dgrad_bound(dz, w, z=None, act_kind=cabi.ACT_NONE, before=None):
 def wgrad_bound(dz, h, act_kind=cabi.ACT_NONE, dw_before=None, db_before=None):
     """CDS_OP_WGRAD -> (bound of dw (N, K), bound of db (N,)): each output sums the rows in order in one thread, so
     (rows + 8) u |dz|^T |act(h)| (the fp32 activation's relative error included) and (rows + 2) u sum_rows |dz| for the bias
-    column; an accumulating store adds 2 u (|before| + |contribution|)."""
+    column; an accumulating store adds 2 u (|before| + |contribution|).  Underflow: a Mish of a pre-activation far below
+    zero is exact only to TINY, and each of the rows + 8 roundings to NORMAL_MIN, absolutely."""
     dz = np.asarray(dz, np.float64)
     rows, adz = dz.shape[0], np.abs(dz)
     gw, gb = wgrad(dz, h, act_kind)
-    bw = (rows + 8) * U32 * (adz.T @ np.abs(act(act_kind, h)))
+    bw = (rows + 8) * (U32 * (adz.T @ np.abs(act(act_kind, h))) + NORMAL_MIN)
+    if act_kind == cabi.ACT_MISH:
+        bw = bw + TINY * adz.sum(0)[:, None]
     bb = (rows + 2) * U32 * adz.sum(0)
     if dw_before is not None:
         bw = bw + 2 * U32 * (np.abs(np.asarray(dw_before, np.float64)) + np.abs(gw))
