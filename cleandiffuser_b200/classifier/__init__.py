@@ -4,7 +4,7 @@ Same surface as the reference's (cleandiffuser/classifier/base.py, rew_classifie
 qgpo_classifier.py): ``model`` is trained, ``model_ema`` (an eval-mode copy updated by ``ema_update``) is what ``logp``
 evaluates.  When one of these guides ``sample()``, the engine evaluates the input gradient inside the replayed loop and
 ``gradients`` is not called:
-  - ``CumRewClassifier`` over ``HalfJannerUNet1d``, or over ``MLPNNClassifier`` with ``out_dim = 1``;
+  - ``CumRewClassifier`` over ``HalfJannerUNet1d``, over ``HalfDiT1d``, or over ``MLPNNClassifier`` with ``out_dim = 1``;
   - ``MSEClassifier`` over ``MLPNNClassifier`` (ReLU, SiLU or Mish hidden layers, identity output), given ``condition_cg``;
   - ``QGPOClassifier`` over ``QGPONNClassifier``, given ``condition_cg``.
 Any other classifier keeps a host callback between the denoiser and the update (``engine/lower.py``, ``guidable``).

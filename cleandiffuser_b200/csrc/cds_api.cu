@@ -16,6 +16,7 @@
 #include "elementwise.cuh"
 #include "classifier.cuh"
 #include "grad.cuh"
+#include "dit_grad.cuh"
 #include "mha.cuh"
 
 namespace {
@@ -179,13 +180,28 @@ int validate(const cds_op& op, Step* out) {
     }
     case CDS_OP_LNMOD: {
       const cds_lnmod_op& l = op.u.lnmod;
-      if (l.batch <= 0 || l.L <= 0 || l.C <= 0 || !l.in || !l.out || !l.shift || !l.scale)
+      if (l.batch <= 0 || l.L <= 0 || l.C <= 0 || !l.in || !l.out || (!l.shift && !l.dout) || !l.scale)
         return fail(CDS_ERR_INVALID, "lnmod: bad arguments");
+      if (l.dout) {
+        if (l.gated && !l.gate) return fail(CDS_ERR_INVALID, "lnmod backward: gated output without a gate");
+        if ((l.out_dtype != CDS_F32 && l.out_dtype != CDS_TF32) || (l.gated && l.gated_dtype != CDS_F32 && l.gated_dtype != CDS_TF32))
+          return fail(CDS_ERR_UNSUPPORTED, "lnmod backward: output dtype");
+      }
       return CDS_OK;
     }
     case CDS_OP_ATTN: {
       const cds_attn_op& a = op.u.attn;
       if (!a.qkv || !a.out) return fail(CDS_ERR_INVALID, "attn: bad arguments");
+      if (a.dout) {
+        if (a.batch <= 0 || a.L <= 0 || a.heads <= 0 || a.C <= 0 || a.C % a.heads != 0)
+          return fail(CDS_ERR_INVALID, "attn backward: bad arguments");
+        const int hd = a.C / a.heads;
+        if (hd != 16 && hd != 32 && hd != 64) return fail(CDS_ERR_UNSUPPORTED, "attn backward: head_dim %d", hd);
+        if (a.L > cds::kAttnBwdMaxL) return fail(CDS_ERR_UNSUPPORTED, "attn backward: L=%d (at most %d)", a.L, cds::kAttnBwdMaxL);
+        if ((a.qkv_dtype != CDS_F32 && a.qkv_dtype != CDS_TF32) || (a.out_dtype != CDS_F32 && a.out_dtype != CDS_TF32))
+          return fail(CDS_ERR_UNSUPPORTED, "attn backward: q|k|v and d q|k|v must be fp32 storage");
+        return CDS_OK;
+      }
       int rc = attn_pick(a, &out->attn_family, &out->attn_param);
       if (rc != CDS_OK) return rc;
       if (out->attn_family == CDS_ATTN_TF32_TMA && !cds::attention_tma_prepare(a, &out->attl))
@@ -212,7 +228,10 @@ int validate(const cds_op& op, Step* out) {
     case CDS_OP_STASH: {
       const cds_stash_op& t = op.u.stash;
       if (t.n <= 0 || !t.src || (!t.dst && !t.act_out)) return fail(CDS_ERR_INVALID, "stash: bad arguments");
-      if (t.act_out && t.act != CDS_ACT_NONE && t.act != CDS_ACT_MISH && t.act != CDS_ACT_SILU && t.act != CDS_ACT_RELU)
+      if (t.grad && (t.dst || !t.act_out || t.act == CDS_ACT_NONE))
+        return fail(CDS_ERR_INVALID, "stash backward: needs act_out and an activation, no slot");
+      if (t.act_out && t.act != CDS_ACT_NONE && t.act != CDS_ACT_MISH && t.act != CDS_ACT_SILU && t.act != CDS_ACT_RELU &&
+          t.act != CDS_ACT_GELU_TANH)
         return fail(CDS_ERR_UNSUPPORTED, "stash: act %d", t.act);
       return CDS_OK;
     }
@@ -294,6 +313,11 @@ int launch(const Step& s, const int* iter_ptr, int sm_count, cudaStream_t st, in
     }
     case CDS_OP_LNMOD: {
       const cds_lnmod_op& l = s.op.u.lnmod;
+      if (l.dout) {
+        cds::lnmod_bwd_kernel<<<cds::lnmod_bwd_grid(l, sm_count), 256, 0, st>>>(l);
+        CDS_CUDA(cudaGetLastError());
+        return CDS_OK;
+      }
       int64_t rows = (int64_t)l.batch * l.L;
       int64_t blocks = (rows + 7) / 8;
       int64_t cap = (int64_t)sm_count * 8;
@@ -302,7 +326,8 @@ int launch(const Step& s, const int* iter_ptr, int sm_count, cudaStream_t st, in
       return CDS_OK;
     }
     case CDS_OP_ATTN:
-      if (s.attn_family == CDS_ATTN_TF32_TMA) CDS_CUDA(cds::attention_tma_launch(s.op.u.attn, s.attl, s.attn_param, sm_count, st));
+      if (s.op.u.attn.dout) CDS_CUDA(cds::attn_bwd_launch(s.op.u.attn, st));
+      else if (s.attn_family == CDS_ATTN_TF32_TMA) CDS_CUDA(cds::attention_tma_launch(s.op.u.attn, s.attl, s.attn_param, sm_count, st));
       else CDS_CUDA(cds::attention_launch(s.op.u.attn, s.attn_family, s.attn_param, st));
       return CDS_OK;
     case CDS_OP_MHA:
@@ -316,7 +341,8 @@ int launch(const Step& s, const int* iter_ptr, int sm_count, cudaStream_t st, in
     }
     case CDS_OP_STASH: {
       const cds_stash_op& t = s.op.u.stash;
-      cds::stash_kernel<<<elementwise_grid(t.n, sm_count), 256, 0, st>>>(t, iter_ptr);
+      if (t.grad) cds::act_bwd_kernel<<<elementwise_grid(t.n, sm_count), 256, 0, st>>>(t);
+      else cds::stash_kernel<<<elementwise_grid(t.n, sm_count), 256, 0, st>>>(t, iter_ptr);
       CDS_CUDA(cudaGetLastError());
       return CDS_OK;
     }
@@ -382,6 +408,9 @@ int preload_kernels() {
   CDS_CUDA(cudaFuncGetAttributes(&a, cds::gn_bwd_kernel));
   CDS_CUDA(cudaFuncGetAttributes(&a, cds::guide_kernel));
   CDS_CUDA(cudaFuncGetAttributes(&a, cds::head_grad_kernel));
+  CDS_CUDA(cds::attn_bwd_preload_all());
+  CDS_CUDA(cudaFuncGetAttributes(&a, cds::lnmod_bwd_kernel));
+  CDS_CUDA(cudaFuncGetAttributes(&a, cds::act_bwd_kernel));
   CDS_CUDA(cudaFuncGetAttributes(&a, cds::set_iter_kernel));
   CDS_CUDA(cudaFuncGetAttributes(&a, cds::advance_iter_kernel));
   return CDS_OK;
@@ -413,6 +442,9 @@ static_assert(sizeof(cds_stash_op) <= sizeof(cds_conv_op) && sizeof(cds_update_b
 static_assert(sizeof(cds_gn_op) <= sizeof(cds_conv_op) && sizeof(cds_gn_bwd_op) <= sizeof(cds_conv_op) &&
               sizeof(cds_guide_op) <= sizeof(cds_conv_op) && sizeof(cds_head_grad_op) <= sizeof(cds_conv_op),
               "classifier-guidance operators must not grow the cds_op union");
+// ... nor do the backward modes of CDS_OP_ATTN, CDS_OP_LNMOD and CDS_OP_STASH
+static_assert(sizeof(cds_attn_op) <= sizeof(cds_conv_op) && sizeof(cds_lnmod_op) <= sizeof(cds_conv_op),
+              "backward modes must not grow the cds_op union");
 
 struct cds_plan {
   int device = 0;
@@ -744,6 +776,8 @@ int cds_run_op(int device, const cds_op* op, int32_t iter, void* stream) {
   Step s;
   int rc = validate(*op, &s);
   if (rc != CDS_OK) return rc;
+  // a plan's kernels get their shared-memory limits at cds_plan_finalize (preload_kernels); a stand-alone launch sets them here
+  if (op->kind == CDS_OP_ATTN && op->u.attn.dout) CDS_CUDA(cds::attn_bwd_preload_all());
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   int* d_iter = nullptr;
   CDS_CUDA(cudaMallocAsync(&d_iter, sizeof(int), st));

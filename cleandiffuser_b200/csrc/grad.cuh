@@ -27,11 +27,25 @@ __device__ __forceinline__ float silu_grad(float x) {
 // d/dx relu(x), ATen's threshold_backward: 1 where x > 0, else 0 (0 at x == 0)
 __device__ __forceinline__ float relu_grad(float x) { return x > 0.f ? 1.f : 0.f; }
 
-// the derivative of the activations CDS_OP_DGRAD accepts (cds_api.cu rejects every other act before a launch)
+// d/dx gelu_tanh(x), ATen's formula (aten/src/ATen/native/cuda/ActivationGeluKernel.cu, GeluBackwardCUDAKernelImpl with
+// approximate = "tanh"): 0.5 (1 + tanh(u)) + 0.5 x (1 - tanh(u)^2) sqrt(2/pi) (1 + 3 kappa x^2),  u = sqrt(2/pi) (x + kappa x^3)
+__device__ __forceinline__ float gelu_tanh_grad(float x) {
+  const float kBeta = 0.7978845608028654f, kKappa = 0.044715f;
+  const float x_sq = x * x;
+  const float inner = kBeta * (x + kKappa * x_sq * x);
+  const float t = tanhf(inner);
+  const float left = 0.5f * x, right = 1.f + t;
+  const float left_derivative = 0.5f * right;
+  const float right_derivative = left * (1.f - t * t) * (kBeta * (1.f + 3.f * kKappa * x_sq));
+  return left_derivative + right_derivative;
+}
+
+// the derivative of the activations CDS_OP_DGRAD and CDS_OP_STASH's backward mode accept (cds_api.cu rejects every other act before a launch)
 __device__ __forceinline__ float act_grad(int act, float x) {
   switch (act) {
     case CDS_ACT_SILU: return silu_grad(x);
     case CDS_ACT_RELU: return relu_grad(x);
+    case CDS_ACT_GELU_TANH: return gelu_tanh_grad(x);
     case CDS_ACT_MISH:
     default: return mish_grad(x);
   }

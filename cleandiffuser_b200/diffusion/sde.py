@@ -180,8 +180,8 @@ class BaseDiffusionSDE(DiffusionModel):
             from ..engine import runtime
             guide = None
             if self.classifier is not None and w_cg != 0.0:
-                # classifier guidance on the engine.  A classifier lower.guidable accepts (CumRewClassifier over HalfJannerUNet1d
-                # or MLPNNClassifier, MSEClassifier over MLPNNClassifier, QGPOClassifier over QGPONNClassifier) is lowered into
+                # classifier guidance on the engine.  A classifier lower.guidable accepts (CumRewClassifier over HalfJannerUNet1d,
+                # HalfDiT1d or MLPNNClassifier, MSEClassifier over MLPNNClassifier, QGPOClassifier over QGPONNClassifier) is lowered into
                 # the replayed program (runtime.try_sample); any other classifier runs step by step: the engine evaluates the denoiser, this
                 # callback adds the guidance term to the prediction in place (same tensor expression as classifier_guidance
                 # above), the engine applies the update.

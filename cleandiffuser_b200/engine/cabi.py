@@ -10,7 +10,7 @@ import os
 
 _LIB_PATH = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "csrc", "libcds.so")
 
-ABI_VERSION = 9
+ABI_VERSION = 10
 OPF_BRANCH_SHIFT = 8   # cds_op.flags bits 8..15: branch index (independent chains run on parallel streams)
 OPF_ONCE = 1          # cds_op.flags: run once per plan run (before its first iteration), not in every iteration
 OP_CONV, OP_UPDATE, OP_LNMOD, OP_ATTN, OP_PREP, OP_CAST, OP_MHA = range(7)
@@ -55,12 +55,16 @@ class ConvOp(C.Structure):
 class LnModOp(C.Structure):
     _fields_ = [("batch", C.c_int32), ("L", C.c_int32), ("C", C.c_int32), ("eps", C.c_float),
                 ("in_", _f32p), ("out", C.c_void_p), ("shift", _f32p), ("scale", _f32p), ("mod_bstride", C.c_int64),
-                ("out_dtype", C.c_int32)]
+                ("out_dtype", C.c_int32),
+                # backward mode (dout != NULL)
+                ("dout", _f32p), ("dout_bstride", C.c_int64), ("dout_lstride", C.c_int32), ("res", _f32p),
+                ("gate", _f32p), ("gate_bstride", C.c_int64), ("gated", _f32p), ("gated_dtype", C.c_int32)]
 
 
 class AttnOp(C.Structure):
     _fields_ = [("batch", C.c_int32), ("L", C.c_int32), ("C", C.c_int32), ("heads", C.c_int32),
-                ("qkv", _f32p), ("out", C.c_void_p), ("out_dtype", C.c_int32), ("qkv_dtype", C.c_int32)]
+                ("qkv", _f32p), ("out", C.c_void_p), ("out_dtype", C.c_int32), ("qkv_dtype", C.c_int32),
+                ("dout", _f32p)]                      # backward mode (dout != NULL)
 
 
 class MhaOp(C.Structure):
@@ -96,7 +100,7 @@ class UpdateOp(C.Structure):
 
 class StashOp(C.Structure):
     _fields_ = [("n", C.c_int64), ("act", C.c_int32), ("src", _f32p), ("dst", _f32p), ("dst_iter_stride", C.c_int64),
-                ("act_out", _f32p)]
+                ("act_out", _f32p), ("grad", _f32p)]          # backward mode: act_out = grad * act'(src)
 
 
 class UpdateBwdOp(C.Structure):

@@ -870,15 +870,11 @@ def _embed_tokens(p: Program, x: View, lin: nn.Linear, pos: View, X: View, in_ba
         p.conv(x, w_linear(lin.weight), X, bias=_const_vec(p.packed(lambda: lin.bias)), res=pos, in_batch_mod=in_batch_mod)
 
 
-def lower_dit(p: Program, net: nn.Module, x: View, horizon: int, has_cond: bool, in_batch_mod: int) -> View:
-    d = net.d_model
-    depth = len(net.blocks)
-    heads = net.blocks[0].attn.num_heads
-    if net.blocks[0].attn.dropout != 0.0 and net.training:
-        raise Unsupported("attention dropout in train mode")
-    R, L = p.rows, horizon
-
-    # ---- conditioning: emb = Mish(W2 Mish(W0 (map_noise(t) + cond_b) + b0) + b2);  every consumer applies SiLU first
+def _dit_conditioning(p: Program, net: nn.Module, L: int, has_cond: bool):
+    """DiT1d's conditioning inside the program -> (the per-trajectory adaLN table [rows, sum of the adaLN widths] of every block
+    and the final layer, the (L, d) position table): emb = Mish(W2 Mish(W0 (map_noise(t) + cond_b) + b0) + b2), every consumer
+    applies SiLU first"""
+    d, R = net.d_model, p.rows
     w0 = net.map_emb[0]
     t_rows, c_rows = p.buf(p.n_iters, d), p.buf(R, d)
     pos = p.buf(L, d)
@@ -902,7 +898,43 @@ def lower_dit(p: Program, net: nn.Module, x: View, horizon: int, has_cond: bool,
     mod = View(p.buf(R, 1, total), 1, total)
     p.conv(emb_s, w_rows(lambda: torch.cat([m.weight for m in mods], 0)), mod,
            bias=_const_vec(p.packed(lambda: torch.cat([m.bias for m in mods], 0))))
-    mod2d = mod.t.view(R, total)
+    return mod.t.view(R, total), pos
+
+
+def _dit_block(p: Program, blk: nn.Module, mod2d: torch.Tensor, o: int, heads: int, X: View, Y: View, QKV: View, ATT: View,
+               HID: View, X1: View, X2: View, hpre: Optional[View] = None):
+    """One DiTBlock: X (block input) -> X1 (after the attention residual) -> X2 (block output); the adaLN chunks of the block
+    start at column ``o`` of ``mod2d`` in the order shift_msa, scale_msa, gate_msa, shift_mlp, scale_mlp, gate_mlp.  The denoiser
+    passes one buffer for X, X1 and X2 (the residual stream updated in place) and fuses the GELU into the first MLP Linear; a
+    classifier's input gradient passes one X / X1 per block (the LayerNorm inputs its backward reads), and ``hpre``: the first MLP
+    Linear then writes the GELU's pre-activation there and CDS_OP_STASH forms HID = gelu_tanh(hpre)."""
+    d = X.C
+    p.lnmod(X, Y, mod2d, o, o + d, blk.norm1.eps)
+    at = blk.attn
+    p.token_linear(Y, w_linear(at.in_proj_weight), QKV, bias=_const_vec(p.packed(lambda a=at: a.in_proj_bias)))
+    p.attn(QKV, ATT, heads)
+    # reference quirk (dit.py:33-34): the residual wraps the MODULATED tokens Y, not the block input
+    p.token_linear(ATT, w_linear(at.out_proj.weight), X1, bias=_const_vec(p.packed(lambda a=at: a.out_proj.bias)),
+                   scale=_vec(sample=mod2d, col=o + 2 * d), res=Y)
+    p.lnmod(X1, Y, mod2d, o + 3 * d, o + 4 * d, blk.norm2.eps)
+    b1 = _const_vec(p.packed(lambda b=blk: b.mlp[0].bias))
+    if hpre is None:
+        p.token_linear(Y, w_linear(blk.mlp[0].weight), HID, bias=b1, act=cabi.ACT_GELU_TANH)
+    else:
+        p.token_linear(Y, w_linear(blk.mlp[0].weight), hpre, bias=b1)
+        _act_stash(p, hpre, HID, cabi.ACT_GELU_TANH)
+    p.token_linear(HID, w_linear(blk.mlp[3].weight), X2, bias=_const_vec(p.packed(lambda b=blk: b.mlp[3].bias)),
+                   scale=_vec(sample=mod2d, col=o + 5 * d), res=X1)
+
+
+def lower_dit(p: Program, net: nn.Module, x: View, horizon: int, has_cond: bool, in_batch_mod: int) -> View:
+    d = net.d_model
+    depth = len(net.blocks)
+    heads = net.blocks[0].attn.num_heads
+    if net.blocks[0].attn.dropout != 0.0 and net.training:
+        raise Unsupported("attention dropout in train mode")
+    L = horizon
+    mod2d, pos = _dit_conditioning(p, net, L, has_cond)
 
     # ---- tokens
     # residual stream X and the attention operands QKV stay fp32; what feeds a Linear layer (the modulated tokens Y, the
@@ -915,24 +947,13 @@ def lower_dit(p: Program, net: nn.Module, x: View, horizon: int, has_cond: bool,
     Y, ATT, HID = p.act(L, d), p.act(L, d), p.act(L, 4 * d)
     _embed_tokens(p, x, net.x_proj, View(pos, L, d, bstride=0), X, in_batch_mod)
     for i, blk in enumerate(net.blocks):
-        o = 6 * d * i       # chunk order: shift_msa, scale_msa, gate_msa, shift_mlp, scale_mlp, gate_mlp
-        p.lnmod(X, Y, mod2d, o, o + d, blk.norm1.eps)
-        at = blk.attn
-        p.token_linear(Y, w_linear(at.in_proj_weight), QKV, bias=_const_vec(p.packed(lambda a=at: a.in_proj_bias)))
-        p.attn(QKV, ATT, heads)
-        # reference quirk (dit.py:33-34): the residual wraps the MODULATED tokens Y, not the block input
-        p.token_linear(ATT, w_linear(at.out_proj.weight), X, bias=_const_vec(p.packed(lambda a=at: a.out_proj.bias)),
-                       scale=_vec(sample=mod2d, col=o + 2 * d), res=Y)
-        p.lnmod(X, Y, mod2d, o + 3 * d, o + 4 * d, blk.norm2.eps)
-        p.token_linear(Y, w_linear(blk.mlp[0].weight), HID, bias=_const_vec(p.packed(lambda b=blk: b.mlp[0].bias)),
-                       act=cabi.ACT_GELU_TANH)
-        p.token_linear(HID, w_linear(blk.mlp[3].weight), X, bias=_const_vec(p.packed(lambda b=blk: b.mlp[3].bias)),
-                       scale=_vec(sample=mod2d, col=o + 5 * d), res=X)
+        _dit_block(p, blk, mod2d, 6 * d * i, heads, X, Y, QKV, ATT, HID, X, X)
     o = 6 * d * depth
     fl = net.final_layer
     p.lnmod(X, Y, mod2d, o, o + d, fl.norm_final.eps)
     out = p.act(L, net.in_dim, f32)
-    return p.token_linear(Y, w_linear(fl.linear.weight), out, bias=_const_vec(p.packed(lambda: fl.linear.bias)))
+    p.token_linear(Y, w_linear(fl.linear.weight), out, bias=_const_vec(p.packed(lambda: fl.linear.bias)))
+    return out                 # shaped (rows, L, in_dim): CDS_OP_GUIDE reads it per token
 
 
 # =============================================================================== ChiTransformer
@@ -1009,7 +1030,8 @@ def lower_chitransformer(p: Program, net: nn.Module, x: View, horizon: int, has_
         p.token_linear(HID, w_linear(layer.linear2.weight), X, bias=bias(lambda m=layer: m.linear2.bias), res=X)
     _layernorm(p, net.ln_f, X, Y)
     out = p.act(L, net.head.out_features, f32)
-    return p.token_linear(Y, w_linear(net.head.weight), out, bias=bias(lambda: net.head.bias))
+    p.token_linear(Y, w_linear(net.head.weight), out, bias=bias(lambda: net.head.bias))
+    return out                 # shaped (rows, L, C): CDS_OP_GUIDE reads it per token
 
 
 def lower_denoiser(p: Program, net: nn.Module, x: View, x_shape, has_cond: bool, in_batch_mod: int) -> View:
@@ -1045,14 +1067,16 @@ def lower_denoiser(p: Program, net: nn.Module, x: View, x_shape, has_cond: bool,
 def guidable(clf, x_shape, cond_cg=None) -> Optional[str]:
     """None when ``lower_classifier_grad`` can put the input gradient of ``clf`` at x_t into the loop, else the reason it cannot.
     The classifiers are recognised structurally (class names and the attributes the lowering reads), so that the reference's own
-    instances qualify: a CumRewClassifier over a HalfJannerUNet1d or over an out_dim-1 MLPNNClassifier, an MSEClassifier over an
-    MLPNNClassifier guided with a per-trajectory target ``cond_cg``, or a QGPOClassifier over a QGPONNClassifier guided with a
-    per-trajectory condition ``cond_cg`` (the observations)."""
+    instances qualify: a CumRewClassifier over a HalfJannerUNet1d, a HalfDiT1d or an out_dim-1 MLPNNClassifier, an
+    MSEClassifier over an MLPNNClassifier guided with a per-trajectory target ``cond_cg``, or a QGPOClassifier over a
+    QGPONNClassifier guided with a per-trajectory condition ``cond_cg`` (the observations)."""
     name = type(clf).__name__
     net_name = type(getattr(clf, "model_ema", None)).__name__
     if name == "CumRewClassifier":
         if net_name == "MLPNNClassifier":
             return _mlp_classifier_reason(clf, x_shape, cond_cg, mse=False)
+        if net_name == "HalfDiT1d":
+            return _half_dit_reason(clf, x_shape)
         return _half_janner_reason(clf, x_shape)
     if name == "MSEClassifier":
         if net_name != "MLPNNClassifier":
@@ -1070,6 +1094,8 @@ def lower_classifier_grad(p: Program, clf, x: View) -> View:
         return lower_qgpo_grad(p, clf, x)
     if type(clf.model_ema).__name__ == "MLPNNClassifier":
         return lower_mlp_classifier_grad(p, clf, x)
+    if type(clf.model_ema).__name__ == "HalfDiT1d":
+        return lower_half_dit_grad(p, clf, x)
     return lower_half_janner_grad(p, clf, x)
 
 
@@ -1346,11 +1372,11 @@ def lower_half_janner_grad(p: Program, clf, x: View) -> View:
 
 
 def _act_stash(p: Program, z: View, out: View, act: int):
-    """CDS_OP_STASH without a slot: out = act(z) (dense (rows, C) fp32 views)"""
+    """CDS_OP_STASH without a slot: out = act(z) (dense (rows, L, C) fp32 views)"""
     op = cabi.Op()
     op.kind = cabi.OP_STASH
     s = op.u.stash
-    s.n, s.act, s.src, s.act_out = p.rows * z.C, act, z.ptr, out.ptr
+    s.n, s.act, s.src, s.act_out = p.rows * z.L * z.C, act, z.ptr, out.ptr
     p.ops.append(op)
 
 
@@ -1506,6 +1532,157 @@ def lower_mlp_classifier_grad(p: Program, clf, x: View) -> View:
     dx = stack.dense(x.C)
     _dgrad(p, dz1, p.packed(w_1x), dx.t.view(R, x.C))
     return dx
+
+
+# =============================================================================== HalfDiT1d's input gradient
+HALF_DIT_HEAD_DIMS = (16, 32, 64)          # the head_dim CDS_OP_ATTN's backward mode covers
+HALF_DIT_MAX_L = 128                       # the longest horizon CDS_OP_ATTN's backward mode covers
+
+
+def _affine_ln(m) -> bool:
+    return isinstance(m, nn.LayerNorm) and m.elementwise_affine and m.bias is not None and len(m.normalized_shape) == 1
+
+
+def _half_dit_reason(clf, x_shape) -> Optional[str]:
+    net = clf.model_ema
+    if net.training:
+        return "classifier model_ema in train mode"
+    if len(x_shape) != 2 or x_shape[1] != net.x_proj.in_features:
+        return "classifier in_dim does not match x"
+    d, heads = net.d_model, net.blocks[0].attn.num_heads
+    if d % heads or d // heads not in HALF_DIT_HEAD_DIMS:
+        return f"classifier head_dim {d / heads:g} (16, 32 or 64 only)"
+    if x_shape[0] > HALF_DIT_MAX_L:
+        return f"classifier horizon {x_shape[0]} (at most {HALF_DIT_MAX_L})"
+    fl, proj = getattr(net, "final_layer", None), getattr(net, "proj", None)
+    ok = isinstance(proj, nn.Sequential) and len(proj) == 6 and \
+        [type(m).__name__ for m in proj] == ["LayerNorm", "SiLU", "Linear", "LayerNorm", "SiLU", "Linear"] and \
+        _affine_ln(proj[0]) and _affine_ln(proj[3]) and isinstance(getattr(fl, "linear", None), nn.Linear) and \
+        isinstance(getattr(fl, "norm_final", None), nn.LayerNorm) and not fl.norm_final.elementwise_affine and \
+        fl.linear.in_features == d and proj[0].normalized_shape[0] == fl.linear.out_features == proj[2].in_features and \
+        proj[3].normalized_shape[0] == proj[2].out_features == proj[5].in_features
+    return None if ok else "classifier proj / final_layer without the reference's structure"
+
+
+def _lnmod_bwd(p: Program, x: View, scale: torch.Tensor, scale_col: int, eps: float, dout: View, dx: View,
+               res: Optional[View] = None, gate_col: Optional[int] = None, gated: Optional[View] = None,
+               mod_bstride: Optional[int] = None):
+    """CDS_OP_LNMOD in backward mode: dx = d x of LN(x) (1 + scale) + shift given dout [+ res]; gated = gate * dx (gate: column
+    ``gate_col`` of the same table).  ``scale``: a [rows, W] table (mod_bstride = its row stride) or one row (mod_bstride 0)."""
+    op = cabi.Op()
+    op.kind = cabi.OP_LNMOD
+    m = op.u.lnmod
+    m.batch, m.L, m.C, m.eps = p.rows, x.L, x.C, float(eps)
+    m.in_ = x.ptr
+    m.scale = scale.data_ptr() + 4 * int(scale_col)
+    m.mod_bstride = scale.stride(0) if mod_bstride is None else mod_bstride
+    m.dout, m.dout_bstride, m.dout_lstride = dout.ptr, dout.bstride, dout.lstride
+    if res is not None:
+        m.res = res.ptr
+    m.out, m.out_dtype = dx.ptr, dx.dtype
+    if gated is not None:
+        m.gate, m.gate_bstride = scale.data_ptr() + 4 * int(gate_col), m.mod_bstride
+        m.gated, m.gated_dtype = gated.ptr, gated.dtype
+    p.ops.append(op)
+    return dx
+
+
+def lower_half_dit_grad(p: Program, clf, x: View) -> View:
+    """Append the input gradient d sum(logp) / d x of ``clf.model_ema`` (a HalfDiT1d; ``guidable``) at x_t (rows, horizon, x.C)
+    to the iteration program -> the gradient as a (rows, horizon, x.C) fp32 view (x.C may include zero padding channels).
+
+    logp = proj(mean_L(FinalLayer1d(X_D, emb))),  X_{i+1} = DiTBlock_i(X_i, emb),  X_0 = x_proj(x) + pos;  emb depends on t only
+    (CumRewClassifier.logp passes no condition), so the adaLN table is DiT1d's conditioning path with a zero condition.
+    Forward: the blocks of ``lower_dit`` (``_dit_block``), each keeping X_i, X1_i, QKV_i and the GELU pre-activation H_i;
+    the final LN + modulate; mean_L and the final Linear as one GEMM over the flattened tokens (the weight tiled L times, / L);
+    proj's LayerNorms as CDS_OP_LNMOD with the [gamma - 1 | beta] table, SiLU as CDS_OP_STASH.
+    Backward, seeded with ones for every out_dim: proj through CDS_OP_DGRAD (SiLU') and CDS_OP_LNMOD's backward mode; the final
+    Linear's data gradient is one row per trajectory (CDS_OP_DGRAD with W / L), which the final LayerNorm backward reads
+    broadcast over the horizon.  Per block, in reverse (g = the gated copy the LayerNorm backward before it wrote):
+        dH  = (g_m dX2) W2 (token GEMM);  dH' = dH gelu_tanh'(H) (CDS_OP_STASH, backward mode);  dY2 = dH' W1 (token GEMM)
+        dX1 = dX2 + LNmod_bwd(X1; dY2), and g_a dX1           (CDS_OP_LNMOD, backward mode)
+        dA  = (g_a dX1) W_out;  dQKV = attn_bwd(QKV; dA) (CDS_OP_ATTN, backward mode)
+        dY1 = dX1 + dQKV W_in (token GEMM + residual)
+        dX  = LNmod_bwd(X; dY1), and g_m of the block before times dX
+    then dx = dX_0 W_x.  The token GEMMs are ``Program.token_linear`` with the transposed weights (wgmma on tensor-core programs
+    where the kernel takes them)."""
+    net = clf.model_ema
+    R, L, d = p.rows, x.L, net.d_model
+    heads, depth = net.blocks[0].attn.num_heads, len(net.blocks)
+    fl, proj = net.final_layer, net.proj
+    f32 = torch.float32
+    mod2d, pos = _dit_conditioning(p, net, L, False)
+
+    # ---- forward, keeping what the backward reads
+    Xs = [p.act(L, d, f32) for _ in range(depth + 1)]
+    X1s = [p.act(L, d, f32) for _ in range(depth)]
+    QKVs = [p.act(L, 3 * d) for _ in range(depth)]                   # fp32 storage on fp32 / TF32 programs
+    Hs = [p.act(L, 4 * d, f32) for _ in range(depth)]
+    Y, ATT, HID = p.act(L, d), p.act(L, d), p.act(L, 4 * d)
+    pos_v = View(pos, L, d, bstride=0)
+    if x.C != net.x_proj.in_features or x.tf32 or not p.tc:
+        # x_t as the denoiser reads it (the channel-padded copy of a tensor-core program, else x_t itself)
+        p.token_linear(x, w_rows(lambda: _pad_cin(net.x_proj.weight, x.C)), Xs[0],
+                       bias=_const_vec(p.packed(lambda: net.x_proj.bias)), res=pos_v)
+    else:
+        _embed_tokens(p, x, net.x_proj, pos_v, Xs[0], 0)
+    for i, blk in enumerate(net.blocks):
+        _dit_block(p, blk, mod2d, 6 * d * i, heads, Xs[i], Y, QKVs[i], ATT, HID, X1s[i], Xs[i + 1], hpre=Hs[i])
+    o = 6 * d * depth
+    p.lnmod(Xs[depth], Y, mod2d, o, o + d, fl.norm_final.eps)
+    d2, d4 = fl.linear.out_features, proj[2].out_features
+
+    def dense(width):
+        return View(p.buf(R, 1, width), 1, width)
+    feat = dense(d2)                                                 # mean_L(final_layer(X_D))
+    p.conv(View(Y.t, 1, L * d, Y.offset, Y.bstride, L * d, Y.tf32), w_rows(lambda: fl.linear.weight.repeat(1, L) / L), feat,
+           bias=_const_vec(p.packed(lambda: fl.linear.bias)))
+    ln_tabs = [p.packed(lambda m=m: torch.cat([m.weight - 1., m.bias])[None]) for m in (proj[0], proj[3])]
+    z0, h0, z1, z1n = dense(d2), dense(d2), dense(d4), dense(d4)
+    p.lnmod(feat, z0, ln_tabs[0].expand(R, 2 * d2), d2, 0, proj[0].eps)
+    _act_stash(p, z0, h0, cabi.ACT_SILU)
+    p.conv(h0, w_linear(proj[2].weight), z1, bias=_const_vec(p.packed(lambda: proj[2].bias)))
+    p.lnmod(z1, z1n, ln_tabs[1].expand(R, 2 * d4), d4, 0, proj[3].eps)
+
+    # ---- backward
+    ones = p.buf(R, proj[5].out_features)
+    ones.fill_(1.0)
+    dz1n, dz1, dz0, dfeat, drow = p.buf(R, d4), dense(d4), p.buf(R, d2), dense(d2), dense(d)
+    _dgrad(p, ones, p.packed(lambda: proj[5].weight), dz1n, z1n, cabi.ACT_SILU)
+    _lnmod_bwd(p, z1, ln_tabs[1], 0, proj[3].eps, View(dz1n, 1, d4), dz1, mod_bstride=0)
+    _dgrad(p, dz1.t.view(R, d4), p.packed(lambda: proj[2].weight), dz0, z0, cabi.ACT_SILU)
+    _lnmod_bwd(p, feat, ln_tabs[0], 0, proj[0].eps, View(dz0, 1, d2), dfeat, mod_bstride=0)
+    _dgrad(p, dfeat.t.view(R, d2), p.packed(lambda: fl.linear.weight / L), drow.t.view(R, d))
+
+    G = p.act(L, d)                                                  # a gated gradient: the input of a data-gradient GEMM
+    dH, dHp, dY = p.act(L, 4 * d, f32), p.act(L, 4 * d, f32), p.act(L, d, f32)
+    dXa, dXb, dA, dQKV = p.act(L, d, f32), p.act(L, d, f32), p.act(L, d, f32), p.act(L, 3 * d)
+    g_m = lambda i: 6 * d * i + 5 * d                                # noqa: E731
+    _lnmod_bwd(p, Xs[depth], mod2d, o + d, fl.norm_final.eps, View(drow.t, L, d, bstride=d, lstride=0), dXa,
+               gate_col=g_m(depth - 1), gated=G)
+    for i in range(depth - 1, -1, -1):
+        blk, at, ob = net.blocks[i], net.blocks[i].attn, 6 * d * i
+        p.token_linear(G, w_rows(lambda b=blk: b.mlp[3].weight.t()), dH)
+        op = cabi.Op()
+        op.kind = cabi.OP_STASH                                      # backward mode: dH' = dH gelu_tanh'(H)
+        a = op.u.stash
+        a.n, a.act, a.src, a.grad, a.act_out = R * L * 4 * d, cabi.ACT_GELU_TANH, Hs[i].ptr, dH.ptr, dHp.ptr
+        p.ops.append(op)
+        p.token_linear(dHp, w_rows(lambda b=blk: b.mlp[0].weight.t()), dY)
+        _lnmod_bwd(p, X1s[i], mod2d, ob + 4 * d, blk.norm2.eps, dY, dXb, res=dXa, gate_col=ob + 2 * d, gated=G)
+        p.token_linear(G, w_rows(lambda m=at: m.out_proj.weight.t()), dA)
+        op = cabi.Op()
+        op.kind = cabi.OP_ATTN                                       # backward mode: d q|k|v from q|k|v and d out
+        b = op.u.attn
+        b.batch, b.L, b.C, b.heads = R, L, d, heads
+        b.qkv, b.qkv_dtype, b.dout, b.out, b.out_dtype = QKVs[i].ptr, QKVs[i].dtype, dA.ptr, dQKV.ptr, dQKV.dtype
+        p.ops.append(op)
+        p.token_linear(dQKV, w_rows(lambda m=at: m.in_proj_weight.t()), dY, res=dXb)
+        gate = dict(gate_col=g_m(i - 1), gated=G) if i else {}
+        _lnmod_bwd(p, Xs[i], mod2d, ob + d, blk.norm1.eps, dY, dXa, **gate)
+    dx = p.act(L, x.C, f32)
+    p.token_linear(dXa, w_rows(lambda: _pad_cin(net.x_proj.weight, x.C).t()), dx)
+    return dx                  # (token_linear returns the flattened view of a tensor-core program)
 
 
 def guide(p: Program, pred: View, g: View, scale: torch.Tensor):

@@ -8,6 +8,8 @@ energy network; under ``QGPOClassifier`` guidance its input gradient is lowered 
 ``MLPNNClassifier`` (nn_classifier/mlp.py) is the general-purpose MLP over ``[x | map_noise(t)]``; under ``MSEClassifier``
 guidance, or ``CumRewClassifier`` guidance with ``out_dim = 1``, its input gradient is lowered by
 ``lower_mlp_classifier_grad`` when its hidden activation is ReLU, SiLU or Mish and its output activation the identity.
+``HalfDiT1d`` (the reference's nn_classifier/half_dit.py) is DiT1d with a FinalLayer1d to d_model / 2 channels, a mean over the horizon and a
+LayerNorm + SiLU + Linear head; under ``CumRewClassifier`` guidance its input gradient is lowered by ``lower_half_dit_grad``.
 """
 from typing import List, Optional, Tuple
 
@@ -16,6 +18,7 @@ import torch
 import torch.nn as nn
 
 from ..nn_diffusion.base import BaseNNDiffusion
+from ..nn_diffusion.dit1d import DiT1d, FinalLayer1d
 from ..nn_diffusion.unets import Downsample1d, ResidualBlock
 from ..utils import Mlp
 
@@ -99,3 +102,24 @@ class QGPONNClassifier(BaseNNDiffusion):
         x = self.act_proj(x)
         out = self.mlp(torch.cat([y, x, self.map_noise(t)], dim=-1))
         return torch.tanh(out / 10) * 10
+
+
+class HalfDiT1d(DiT1d):
+    """x (b, horizon, in_dim), noise (b,), condition (b, emb_dim) | None -> (b, out_dim): ``proj(mean_L(DiT1d(x)))`` where DiT1d's
+    final layer maps to d_model // 2 channels (weights and adaLN zero-initialised, as in the reference) and
+    ``proj = LayerNorm, SiLU, Linear(d_model // 2, d_model // 4), LayerNorm, SiLU, Linear(d_model // 4, out_dim)``.
+    Constructor, defaults and state-dict keys are the reference's (cleandiffuser/nn_classifier/half_dit.py)."""
+
+    def __init__(self, in_dim: int, out_dim: int, emb_dim: int, d_model: int = 384, n_heads: int = 6, depth: int = 12,
+                 dropout: float = 0.0, timestep_emb_type: str = "positional"):
+        super().__init__(in_dim, emb_dim, d_model, n_heads, depth, dropout, timestep_emb_type)
+        self.final_layer = FinalLayer1d(d_model, d_model // 2)
+        for lin in (self.final_layer.adaLN_modulation[-1], self.final_layer.linear):
+            nn.init.constant_(lin.weight, 0)
+            nn.init.constant_(lin.bias, 0)
+        self.proj = nn.Sequential(
+            nn.LayerNorm(d_model // 2), nn.SiLU(), nn.Linear(d_model // 2, d_model // 4),
+            nn.LayerNorm(d_model // 4), nn.SiLU(), nn.Linear(d_model // 4, out_dim))
+
+    def forward(self, x: torch.Tensor, noise: torch.Tensor, condition: Optional[torch.Tensor] = None):
+        return self.proj(super().forward(x, noise, condition).mean(1))

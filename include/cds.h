@@ -27,6 +27,8 @@
  *   CDS_OP_GUIDE        GroupNorm + Mish over a kept pre-norm input, its backward, and pred += s[iter] * grad (further down)
  *   CDS_OP_HEAD_GRAD    the energy head of QGPO's classifier (qgpo_classifier.py / nn_classifier/mlp.py: 10 tanh(z / 10) over
  *                       an Mlp of Linear + SiLU): z = h . w + b per row and the seed of its backward (further down)
+ *   (backward modes)    classifier guidance with CumRewClassifier over HalfDiT1d (nn_classifier/half_dit.py): CDS_OP_ATTN,
+ *                       CDS_OP_LNMOD and CDS_OP_STASH given an upstream gradient compute their own backward (csrc/dit_grad.cuh)
  *   (no new kind)       classifier guidance with MSEClassifier / CumRewClassifier over MLPNNClassifier (mse_classifier.py,
  *                       nn_classifier/mlp.py): CDS_OP_CONV, CDS_OP_STASH and CDS_OP_DGRAD with CDS_ACT_RELU / SILU / MISH
  *
@@ -55,7 +57,7 @@
 extern "C" {
 #endif
 
-#define CDS_ABI_VERSION 9
+#define CDS_ABI_VERSION 10
 
 typedef enum cds_status {
   CDS_OK = 0,
@@ -145,20 +147,42 @@ typedef struct cds_conv_op {
   int32_t sample_row_div;
 } cds_conv_op;
 
-/* out(b,l,:) = LayerNorm(in(b,l,:), eps, no affine) * (1 + scale(b,:)) + shift(b,:) */
+/* out(b,l,:) = LayerNorm(in(b,l,:), eps, no affine) * (1 + scale(b,:)) + shift(b,:)
+ *
+ * Backward mode (dout != NULL; the input gradient of HalfDiT1d): out = d in of that expression given dout, the shift unused:
+ *   dy = dout(b,l,:) * (1 + scale(b,:)),   xhat = (in - mean) * rstd
+ *   out = rstd * (dy - mean_c(dy) - xhat * mean_c(dy * xhat))  [+ res(b,l,:)]
+ *   gated(b,l,:) = gate(b,:) * out                                    (optional: gated != NULL)
+ * mean and rstd are recomputed from `in` with the forward's arithmetic (fp32, two passes: the mean, then the mean of squared
+ * deviations; rstd = rsqrt(var + eps)), one warp per token row, lane-strided sums reduced by a fixed xor butterfly.  dout +
+ * b*dout_bstride + l*dout_lstride (dout_lstride 0: one row per trajectory broadcast over L); res, gated dense (batch, L, C);
+ * gate + b*gate_bstride; out_dtype / gated_dtype CDS_F32 or CDS_TF32.  mod_bstride and gate_bstride may be 0 (one vector for
+ * every trajectory: the [gamma - 1 | beta] table of an affine LayerNorm). */
 typedef struct cds_lnmod_op {
   int32_t batch, L, C; float eps;
   const float* in; void* out;                   /* dense (batch, L, C); in fp32, out of out_dtype */
   const float* shift; const float* scale; int64_t mod_bstride;   /* per-trajectory vectors */
   int32_t out_dtype;                            /* cds_dtype: bf16 feeds the tensor-core Linear that follows */
+  /* backward mode */
+  const float* dout; int64_t dout_bstride; int32_t dout_lstride;
+  const float* res;
+  const float* gate; int64_t gate_bstride; float* gated; int32_t gated_dtype;
 } cds_lnmod_op;
 
-/* qkv dense (batch, L, 3*C) with [q | k | v] column blocks, heads split C evenly; out dense (batch, L, C) */
+/* qkv dense (batch, L, 3*C) with [q | k | v] column blocks, heads split C evenly; out dense (batch, L, C)
+ *
+ * Backward mode (dout != NULL; the input gradient of HalfDiT1d): given dout = d out (dense (batch, L, C) fp32), out = d q|k|v,
+ * dense (batch, L, 3*C) in qkv's layout.  Per (trajectory, head) the softmax P = softmax(q k^T / sqrt(hd)) is recomputed from
+ * q and k (the forward keeps nothing), then dV = P^T dO, dS = P * (dO V^T - rowsum(P * dO V^T)), dQ = dS K / sqrt(hd),
+ * dK = dS^T Q / sqrt(hd).  qkv fp32 storage (CDS_F32 / CDS_TF32), head_dim 16, 32 or 64, L <= 128 (else CDS_ERR_UNSUPPORTED);
+ * out_dtype CDS_F32 or CDS_TF32.  fp32 CUDA-core FMA, one CTA per (trajectory, head), every sum in a fixed order (no atomics):
+ * two runs are bitwise equal. */
 typedef struct cds_attn_op {
   int32_t batch, L, C, heads;
   const void* qkv; void* out;
   int32_t out_dtype;                            /* cds_dtype of out */
   int32_t qkv_dtype;                            /* cds_dtype of qkv: bf16 (head_dim 32, L <= 128) runs on tensor cores (mma.sync) */
+  const float* dout;                            /* backward mode */
 } cds_attn_op;
 
 /* Multi-head attention with separate query and key|value sources and an optional diagonal mask:
@@ -228,13 +252,16 @@ typedef struct cds_update_op {
  * one captured graph serves every backward iteration like it does every forward one. */
 
 /* dst[iter*dst_iter_stride + i] = src[i] when dst != NULL;  act_out[i] = act(src[i]) when act_out != NULL (i < n); at least one
- * of the two.  act: CDS_ACT_NONE / MISH / SILU / RELU */
+ * of the two.  act: CDS_ACT_NONE / MISH / SILU / RELU / GELU_TANH
+ * Backward mode (grad != NULL): act_out[i] = grad[i] * act'(src[i]), src the stashed pre-activation, dst NULL; act MISH, SILU,
+ * RELU (act' as CDS_OP_DGRAD applies it) or GELU_TANH (ATen's gelu_backward with approximate = "tanh"). */
 typedef struct cds_stash_op {
   int64_t n;
   int32_t act;
   const float* src;
   float* dst; int64_t dst_iter_stride;
   float* act_out;
+  const float* grad;
 } cds_stash_op;
 
 /* Backward of CDS_OP_UPDATE for kinds DDPM, DDIM, EPS and X with a single prediction (no CFG combine, no history):
