@@ -215,7 +215,7 @@ int validate(const cds_op& op, Step* out) {
     }
     case CDS_OP_PREP: {
       const cds_prep_op& p = op.u.prep;
-      if (p.batch <= 0 || p.row <= 0 || !p.x || !p.xin || !p.coef) return fail(CDS_ERR_INVALID, "prep: bad arguments");
+      if (p.batch <= 0 || p.row <= 0 || !p.x || (!p.xin && !p.gxin) || !p.coef) return fail(CDS_ERR_INVALID, "prep: bad arguments");
       return CDS_OK;
     }
     case CDS_OP_CAST: {
@@ -307,7 +307,8 @@ int launch(const Step& s, const int* iter_ptr, int sm_count, cudaStream_t st, in
     }
     case CDS_OP_PREP: {
       const cds_prep_op& p = s.op.u.prep;
-      cds::cm_prep_kernel<<<elementwise_grid((int64_t)p.batch * p.row, sm_count), 256, 0, st>>>(p, iter_ptr);
+      if (p.gxin) cds::prep_bwd_kernel<<<elementwise_grid((int64_t)p.batch * p.row, sm_count), 256, 0, st>>>(p, iter_ptr);
+      else cds::cm_prep_kernel<<<elementwise_grid((int64_t)p.batch * p.row, sm_count), 256, 0, st>>>(p, iter_ptr);
       CDS_CUDA(cudaGetLastError());
       return CDS_OK;
     }
@@ -402,6 +403,7 @@ int preload_kernels() {
   CDS_CUDA(cudaFuncGetAttributes(&a, cds::ln_modulate_kernel));
   CDS_CUDA(cudaFuncGetAttributes(&a, cds::stash_kernel));
   CDS_CUDA(cudaFuncGetAttributes(&a, cds::update_bwd_kernel));
+  CDS_CUDA(cudaFuncGetAttributes(&a, cds::prep_bwd_kernel));
   CDS_CUDA(cudaFuncGetAttributes(&a, cds::dgrad_kernel));
   CDS_CUDA(cudaFuncGetAttributes(&a, cds::wgrad_kernel));
   CDS_CUDA(cudaFuncGetAttributes(&a, cds::gn_kernel));
@@ -445,6 +447,8 @@ static_assert(sizeof(cds_gn_op) <= sizeof(cds_conv_op) && sizeof(cds_gn_bwd_op) 
 // ... nor do the backward modes of CDS_OP_ATTN, CDS_OP_LNMOD and CDS_OP_STASH
 static_assert(sizeof(cds_attn_op) <= sizeof(cds_conv_op) && sizeof(cds_lnmod_op) <= sizeof(cds_conv_op),
               "backward modes must not grow the cds_op union");
+// ... nor does CDS_OP_PREP's
+static_assert(sizeof(cds_prep_op) <= sizeof(cds_conv_op), "cds_prep_op must not grow the cds_op union");
 
 struct cds_plan {
   int device = 0;

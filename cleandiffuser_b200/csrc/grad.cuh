@@ -1,6 +1,8 @@
 // Backward operators of a differentiable reverse loop (sample(requires_grad=True) over DQLMlp):
 //   CDS_OP_STASH       per-iteration copy of a forward operand (+ the Mish of a pre-activation), 8..12 B / element
-//   CDS_OP_UPDATE_BWD  backward of the solver update + clip_prediction + fix_mask (kinds DDPM, DDIM, EPS, X), 24..36 B / element
+//   CDS_OP_UPDATE_BWD  backward of the solver update + clip_prediction + fix_mask (kinds DDPM, DDIM, EPS, X) and of the
+//                      consistency model's combine + clip + fix_mask (kind CM), 24..36 B / element
+//   CDS_OP_PREP        backward mode: gx += c_in * d xin (the consistency model's input scaling), 12 B / element
 //   CDS_OP_DGRAD       dH = dZ W with the Mish or SiLU derivative of the stashed pre-activation fused into the epilogue
 //   CDS_OP_WGRAD       dW += Z^T H, db += sum_rows dZ, accumulated over the iterations
 // The two GEMM-shaped operators run on fp32 CUDA cores with 32 x 32 output tiles staged through shared memory: every output
@@ -61,13 +63,16 @@ static __global__ void __launch_bounds__(256) stash_kernel(const cds_stash_op p,
   }
 }
 
-// One element of the update's backward.  Mirrors solver_update_value (elementwise.cuh) for kinds DDPM / DDIM / EPS / X in
-// reverse, op by op, with torch.clip's tensor-bound gradient rule for clip_prediction.
+// One element of the update's backward.  Mirrors solver_update_value (elementwise.cuh) for kinds DDPM / DDIM / EPS / X / CM
+// in reverse, op by op, with torch.clip's tensor-bound gradient rule for clip_prediction and for CM's final clip.  A kind
+// without a backward here (X2M, EDM, EDM_HEUN) writes NaN to both outputs: the host never builds such a program, and a
+// gradient of the wrong formula must not pass for a correct one.
 static __global__ void __launch_bounds__(256) update_bwd_kernel(const cds_update_bwd_op p, const int* __restrict__ iter_ptr) {
   const int iter = *iter_ptr;
   const float* row = p.coef + (int64_t)iter * p.coef_iter_stride;
   const float alpha = row[CDS_ROW_ALPHA], sigma = row[CDS_ROW_SIGMA], k0 = row[CDS_ROW_K0], k1 = row[CDS_ROW_K1];
   const int kind = (int)row[CDS_ROW_KIND];
+  const bool known = kind == CDS_UPD_DDPM || kind == CDS_UPD_DDIM || kind == CDS_UPD_EPS || kind == CDS_UPD_X || kind == CDS_UPD_CM;
   const float* xs = p.x + (int64_t)iter * p.x_iter_stride;
   const float* ps = p.pred + (int64_t)iter * p.pred_iter_stride;
   const int64_t total = (int64_t)p.batch * p.row;
@@ -76,6 +81,23 @@ static __global__ void __launch_bounds__(256) update_bwd_kernel(const cds_update
     const float x = xs[i], pr = ps[i];
     float g = p.gx[i];
     if (p.mask) g = mul_(g, 1.f - p.mask[e]);
+    if (!known) {
+      p.gpred[i] = p.gx[i] = __int_as_float(0x7fc00000);
+      continue;
+    }
+    if (kind == CDS_UPD_CM) {
+      // f = c_skip*x + c_out*pred with the forward's fp32 ops, then clip(f, x_min, x_max): the gradient passes where f lies
+      // inside the bounds or equals one (torch.clip's rule; none passes when x_min > x_max), and goes to neither operand elsewhere
+      const float f = add_(mul_(k0, x), mul_(k1, pr));
+      bool pass = true;
+      if (p.x_min && p.x_max) pass = f >= p.x_min[e] && f <= p.x_max[e];
+      else if (p.x_min) pass = f >= p.x_min[e];
+      else if (p.x_max) pass = f <= p.x_max[e];
+      const float gf = pass ? g : 0.f;
+      p.gpred[i] = mul_(k1, gf);
+      p.gx[i] = mul_(k0, gf);
+      continue;
+    }
     // d of the update with respect to x (direct), eps and xhat
     float dx = 0.f, deps = 0.f, dxhat = 0.f;
     if (kind == CDS_UPD_DDPM) {
@@ -134,6 +156,17 @@ static __global__ void __launch_bounds__(256) update_bwd_kernel(const cds_update
     p.gpred[i] = gp;
     p.gx[i] = dx;
   }
+}
+
+// Backward mode of CDS_OP_PREP (gxin != NULL): gx += K3 * gxin, with gx in the descriptor's x.  xin = K3*x is the network's
+// input, so its gradient gxin reaches x scaled by K3; the re-noise x += K2*z is additive and passes gx through unchanged.
+// 12 B / element.
+static __global__ void __launch_bounds__(256) prep_bwd_kernel(const cds_prep_op p, const int* __restrict__ iter_ptr) {
+  const int iter = *iter_ptr;
+  const float k3 = p.coef[(int64_t)iter * p.coef_iter_stride + CDS_ROW_K3];
+  const int64_t total = (int64_t)p.batch * p.row;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x)
+    p.x[i] = add_(p.x[i], mul_(k3, p.gxin[i]));
 }
 
 constexpr int kGradTile = 32;

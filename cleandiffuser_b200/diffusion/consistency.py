@@ -238,16 +238,16 @@ class ContinuousConsistencyModel(DiffusionModel):
         order = list(reversed([1] * diffusion_x_sampling_steps + list(range(1, sample_steps))))
 
         from ..engine import runtime
-        if requires_grad:
-            runtime.grad_fallback(self)
-        if not (requires_grad or preserve_history) and runtime._device_ok(torch.device(self.device)):
-            out = runtime.try_sample(self, model=model, xt=xt, prior=prior, solver="consistency", sample_steps=sample_steps,
-                                     order=order, step_values=None, alphas=None, sigmas=None, hs=None, stds=None, cond_emb=cvec,
-                                     w_cfg=1.0 if cvec is not None else 0.0, n_samples=n_samples, predict_noise=False,
-                                     consistency=True,
-                                     table=lambda: S.consistency_table(sigmas, order, self.sigma_data, self.sigma_min),
-                                     sched_id=(int(sample_steps), float(self.sigma_min), float(self.sigma_max), float(self.rho),
-                                               int(diffusion_x_sampling_steps), float(self.sigma_data)))
+        if not preserve_history and runtime._device_ok(torch.device(self.device)):
+            # requires_grad=True (consistency policies' Q loss through the sampler): the differentiable program, x0 comes back
+            # connected to autograd
+            engine = runtime.try_sample_grad if requires_grad else runtime.try_sample
+            out = engine(self, model=model, xt=xt, prior=prior, solver="consistency", sample_steps=sample_steps,
+                         order=order, step_values=None, alphas=None, sigmas=None, hs=None, stds=None, cond_emb=cvec,
+                         w_cfg=1.0 if cvec is not None else 0.0, n_samples=n_samples, predict_noise=False, consistency=True,
+                         table=lambda: S.consistency_table(sigmas, order, self.sigma_data, self.sigma_min),
+                         sched_id=(int(sample_steps), float(self.sigma_min), float(self.sigma_max), float(self.rho),
+                                   int(diffusion_x_sampling_steps), float(self.sigma_data)))
             if out is not None:
                 return out, log
 

@@ -73,9 +73,7 @@ class _RectifiedFlow(DiffusionModel):
         """``t_of(i)`` = the network's time input of loop index i, ``dt_of(i)`` = t_i - t_{i-1} (0-d tensors)."""
         order = list(reversed([1] * diffusion_x_sampling_steps + list(range(1, sample_steps + 1))))
         from ..engine import runtime
-        if requires_grad:
-            runtime.grad_fallback(self)
-        if not (requires_grad or preserve_history) and runtime._device_ok(torch.device(self.device)):
+        if not preserve_history and runtime._device_ok(torch.device(self.device)):
             rows = torch.zeros((len(order), S.ROW), dtype=torch.float32)
             for n, i in enumerate(order):
                 rows[n, S.R_KIND] = float(S.UPD_EPS)
@@ -84,10 +82,12 @@ class _RectifiedFlow(DiffusionModel):
                 rows[n, S.R_K1] = -float(dt_of(i))
             t_all = torch.stack([t_of(i).detach().cpu().to(t_dtype) for i in order])
             eff_w = w_cfg if cvec is not None else 0.0          # (the reference falls back to the unconditional branch)
-            out = runtime.try_sample(self, model=model, xt=xt, prior=prior, solver="rectified_flow_euler",
-                                     sample_steps=sample_steps, order=order, step_values=None, alphas=None, sigmas=None, hs=None,
-                                     stds=None, cond_emb=cvec, w_cfg=eff_w, n_samples=n_samples, table=(rows, 0, t_all),
-                                     clip_in_loop=False, predict_noise=True)
+            # requires_grad=True (flow policies' Q loss through the Euler steps): the differentiable program, whose backward
+            # of this EPS-shaped step is CDS_OP_UPDATE_BWD's; the final clip stays a PyTorch op that autograd sees
+            engine = runtime.try_sample_grad if requires_grad else runtime.try_sample
+            out = engine(self, model=model, xt=xt, prior=prior, solver="rectified_flow_euler", sample_steps=sample_steps,
+                         order=order, step_values=None, alphas=None, sigmas=None, hs=None, stds=None, cond_emb=cvec, w_cfg=eff_w,
+                         n_samples=n_samples, table=(rows, 0, t_all), clip_in_loop=False, predict_noise=True)
             if out is not None:
                 return out
         for i in order:

@@ -10,7 +10,7 @@ import os
 
 _LIB_PATH = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "csrc", "libcds.so")
 
-ABI_VERSION = 10
+ABI_VERSION = 11
 OPF_BRANCH_SHIFT = 8   # cds_op.flags bits 8..15: branch index (independent chains run on parallel streams)
 OPF_ONCE = 1          # cds_op.flags: run once per plan run (before its first iteration), not in every iteration
 OP_CONV, OP_UPDATE, OP_LNMOD, OP_ATTN, OP_PREP, OP_CAST, OP_MHA = range(7)
@@ -79,7 +79,8 @@ class MhaOp(C.Structure):
 
 class PrepOp(C.Structure):
     _fields_ = [("batch", C.c_int32), ("row", C.c_int32), ("x", _f32p), ("xin", _f32p), ("noise", _f32p),
-                ("coef", _f32p)]
+                ("coef", _f32p),
+                ("gxin", _f32p), ("coef_iter_stride", C.c_int64)]      # backward mode (gxin != NULL): x += K3 * gxin
 
 
 class CastOp(C.Structure):

@@ -595,14 +595,20 @@ class DQLGrad:
         d step_tab[n] = sum_rows dz1 (with d W_x += x_n^T dz1: W_x's "bias" is the per-iteration table row);
         d samp_tab += dz1;  gx += dz1 W_x
     ``step_tab`` / ``samp_tab`` are filled by the caller (they are autograd inputs: d step_tab carries into time_mlp, the time
-    columns of mid_layer[0] and its bias, d samp_tab into the observation columns and the condition)."""
+    columns of mid_layer[0] and its bias, d samp_tab into the observation columns and the condition).
 
-    def __init__(self, p: Program, bp: Program, net: nn.Module, x: View):
+    Consistency form (``xin`` given: the consistency model, whose network reads xin = c_in x written by the CDS_OP_PREP the
+    runtime puts in front): x_n (the re-noised x_t the update reads) and xin_n are both stashed, the first layer reads xin and
+    its weight gradient the stashed xin, and the last data gradient writes d xin into its own buffer ``gxin`` (overwritten,
+    not accumulated): the runtime's CDS_OP_PREP in backward mode then adds c_in * gxin to ``gx``."""
+
+    def __init__(self, p: Program, bp: Program, net: nn.Module, x: View, xin: Optional[View] = None):
         R, n, a = p.rows, p.n_iters, x.C
         lins = [net.mid_layer[0], net.mid_layer[2], net.mid_layer[4], net.final_layer]
         widths = [lin.out_features for lin in lins[:3]]
         self.step_tab, self.samp_tab = p.buf(n, widths[0]), p.buf(R, widths[0])
         self.xs, self.ps = p.buf(n, R, a), p.buf(n, R, a)
+        self.xins = p.buf(n, R, a) if xin is not None else None
         self.zs = [p.buf(n, R, w) for w in widths]
 
         def stash(src: View, dst: torch.Tensor, act_out: Optional[View] = None):
@@ -615,11 +621,14 @@ class DQLGrad:
             p.ops.append(op)
 
         stash(x, self.xs)
-        h = x
+        if xin is not None:
+            stash(xin, self.xins)
+        net_in = x if xin is None else xin
+        h = net_in
         for k, lin in enumerate(lins[:3]):
             z = View(p.buf(R, 1, widths[k]), 1, widths[k])
             if k == 0:
-                p.conv(x, w_linear(lin.weight, slice(0, a)), z, bias=_vec(self.step_tab, self.samp_tab))
+                p.conv(net_in, w_linear(lin.weight, slice(0, a)), z, bias=_vec(self.step_tab, self.samp_tab))
             else:
                 p.conv(h, w_linear(lin.weight), z, bias=_const_vec(p.packed(lambda m=lin: m.bias)))
             h = View(p.buf(R, 1, widths[k]), 1, widths[k])
@@ -672,8 +681,13 @@ class DQLGrad:
             wgrad(k, upstream, self.zs[k - 1], cabi.ACT_MISH)
             dgrad(k, upstream, dz[k - 1], self.zs[k - 1], out_sum=self.g_samp if k == 1 else None)
             upstream = dz[k - 1]
-        wgrad(0, upstream, self.xs, cabi.ACT_NONE)
-        dgrad(0, upstream, self.gx, None, accumulate=1)
+        if xin is None:
+            wgrad(0, upstream, self.xs, cabi.ACT_NONE)
+            dgrad(0, upstream, self.gx, None, accumulate=1)
+        else:
+            self.gxin = bp.buf(R, a)
+            wgrad(0, upstream, self.xins, cabi.ACT_NONE)
+            dgrad(0, upstream, self.gxin, None)
 
 
 # =============================================================================== IDQLMlp

@@ -160,12 +160,7 @@ class SamplerPlan:
             fo = 4 * off * row             # byte offset of the branch inside the (batch, row) fp32 buffers
             xin_ptr_t, xin_off = self.x, off * row
             if consistency:
-                op = cabi.Op()
-                op.kind = cabi.OP_PREP
-                q = op.u.prep
-                q.batch, q.row, q.x, q.xin, q.coef = sub, row, self.x.data_ptr() + fo, self.xin.data_ptr() + fo, self.coef.data_ptr()
-                q.noise = self.noise.data_ptr() if self.noise is not None else None
-                p.ops.append(op)
+                self._prep_op(p, sub, fo)
                 xin_ptr_t = self.xin
             xview = View(xin_ptr_t, L, Cn, offset=xin_off)
             pred = lower_denoiser(p, net, xview, x_shape, cfg_mode != 0, sub if cfg_mode == 2 else 0)
@@ -219,6 +214,16 @@ class SamplerPlan:
         self.handle: Optional[cabi.Plan] = None
         self.back_handle: Optional[cabi.Plan] = None
         self.version = None              # set by the first refresh_weights()
+
+    def _prep_op(self, p, sub, fo):
+        """Append the consistency model's re-noise and c_in scaling of ``sub`` trajectories at byte offset ``fo`` (x_t in place,
+        the network's input into ``self.xin``) to ``p``."""
+        op = cabi.Op()
+        op.kind = cabi.OP_PREP
+        q = op.u.prep
+        q.batch, q.row, q.x, q.xin, q.coef = sub, self.row, self.x.data_ptr() + fo, self.xin.data_ptr() + fo, self.coef.data_ptr()
+        q.noise = self.noise.data_ptr() if self.noise is not None else None
+        p.ops.append(op)
 
     def _update_op(self, p, pred, sub, fo, predict_noise, consistency=False):
         """Append the solver update of ``sub`` trajectories at byte offset ``fo`` of the resident buffers to ``p`` (``pred``:
@@ -591,16 +596,26 @@ class GradSamplerPlan(SamplerPlan):
     """The resident state of ``sample(requires_grad=True)`` over DQLMlp: a forward program (``lower.DQLGrad``'s network
     operators, which stash x_n, the hidden pre-activations and the raw prediction of every iteration, then the solver update)
     and a backward program that walks the iterations in reverse.  Each is one cds_plan replayed from a CUDA graph.  One branch,
-    no CFG combine, no solver history."""
+    no CFG combine, no solver history.
 
-    def __init__(self, device, net, batch, x_shape, n_iters, n_slots, *, predict_noise, has_mask, has_min, has_max, math):
+    consistency: the consistency model's program -- a CDS_OP_PREP (re-noise, c_in scaling) in front of the network, the CM
+    combine with its final clip in the update, and at the end of every backward iteration the PREP's backward mode, which adds
+    c_in * d xin to the direct part of d x_n.  Rectified flow needs nothing of its own: its Euler step is the EPS update."""
+
+    def __init__(self, device, net, batch, x_shape, n_iters, n_slots, *, predict_noise, has_mask, has_min, has_max, math,
+                 consistency=False):
         self._resident(device, net, batch, x_shape, n_iters, n_slots, cfg_mode=1, has_mask=has_mask, has_min=has_min,
                        has_max=has_max, keep_history=False, aux_history=False, math=math)
         self.n_branches, row = 1, self.row
         self.back = back = Program(device, batch, n_iters, math)
-        self.grad = g = DQLGrad(self.program, back, net, View(self.x, 1, row))
+        xin = None
+        if consistency:
+            self.xin = self.program.buf(batch, *x_shape)
+            self._prep_op(self.program, batch, 0)
+            xin = View(self.xin, 1, row)
+        self.grad = g = DQLGrad(self.program, back, net, View(self.x, 1, row), xin)
         self.pred = g.pred.t
-        u = self._update_op(self.program, g.pred.ptr, batch, 0, predict_noise)
+        u = self._update_op(self.program, g.pred.ptr, batch, 0, predict_noise, consistency)
 
         bop = cabi.Op()                                      # the update's backward opens every backward iteration
         bop.kind = cabi.OP_UPDATE_BWD
@@ -613,6 +628,13 @@ class GradSamplerPlan(SamplerPlan):
         b.coef, b.coef_iter_stride = _rev(self.coef)
         b.predict_noise = u.predict_noise
         back.ops.insert(0, bop)
+        if consistency:                                      # gx += c_in * d xin closes every backward iteration
+            pop = cabi.Op()
+            pop.kind = cabi.OP_PREP
+            q = pop.u.prep
+            q.batch, q.row, q.x, q.gxin = batch, row, g.gx.data_ptr(), g.gxin.data_ptr()
+            q.coef, q.coef_iter_stride = _rev(self.coef)
+            back.ops.append(pop)
         self.generation = 0                # forward runs so far: a backward must belong to the latest one
 
     def backward(self, grad_x0, generation):
@@ -657,11 +679,18 @@ def grad_fallback(agent):
     return None
 
 
+# the update kinds CDS_OP_UPDATE_BWD differentiates (csrc/grad.cuh): a table with any other kind keeps the PyTorch loop
+_GRAD_KINDS = frozenset((S.UPD_DDPM, S.UPD_DDIM, S.UPD_EPS, S.UPD_X, S.UPD_CM))
+
+
 def try_sample_grad(agent, *, model, xt, prior, solver, sample_steps, order, step_values, alphas, sigmas, hs, stds,
-                    cond_emb, w_cfg, n_samples, guided=False, sched_id=None):
+                    cond_emb, w_cfg, n_samples, guided=False, table=None, clip_in_loop=True, predict_noise=None, sched_id=None,
+                    consistency=False):
     """``sample(requires_grad=True)`` on the engine: x0 connected to autograd through ``_GradSampleFn``.  Covers DQLMlp with
-    the DDPM / DDIM / first-order DPM-Solver updates, one CFG branch and CDS_MATH = fp32 | tf32; everything else takes the
-    PyTorch loop (which autograd differentiates) through ``_fallback``."""
+    one CFG branch and CDS_MATH = fp32 | tf32 under the DDPM / DDIM / first-order DPM-Solver updates, ContinuousConsistencyModel
+    (``consistency``) and RectifiedFlow's Euler step; everything else takes the PyTorch loop (which autograd differentiates)
+    through ``_fallback``.  ``table`` / ``clip_in_loop`` / ``predict_noise`` / ``sched_id`` / ``consistency``: as in
+    ``try_sample``; the table's time column is what the network sees (c_noise for the consistency model)."""
     net = model["diffusion"]
 
     def decline(cfg_mode):
@@ -683,18 +712,23 @@ def try_sample_grad(agent, *, model, xt, prior, solver, sample_steps, order, ste
     device, cfg_mode = screened
     batch, x_shape = xt.shape[0], tuple(xt.shape[1:])
     tab = _schedule(agent, device, solver=solver, sample_steps=sample_steps, order=order, step_values=step_values, alphas=alphas,
-                    sigmas=sigmas, hs=hs, stds=stds, table=None, sched_id=sched_id)
+                    sigmas=sigmas, hs=hs, stds=stds, table=table, sched_id=sched_id)
+    kinds = {int(k) for k in tab.rows[:, S.R_KIND].tolist()} - _GRAD_KINDS
+    if kinds:
+        return _fallback(f"requires_grad=True: update kind {sorted(kinds)} has no backward operator")
+    n_iters = tab.rows.shape[0]
     has_mask = isinstance(agent.fix_mask, torch.Tensor)
-    has_min, has_max = agent.x_min is not None, agent.x_max is not None
-    pn = bool(agent.predict_noise)
+    has_min = clip_in_loop and getattr(agent, "x_min", None) is not None
+    has_max = clip_in_loop and getattr(agent, "x_max", None) is not None
+    pn = bool(agent.predict_noise) if predict_noise is None else bool(predict_noise)
     math = _math_mode()
     tape_slots = _tape_slots(tab.n_slots, batch, x_shape[0])
-    key = (id(net), batch, x_shape, len(order), tape_slots, cfg_mode, pn, has_mask, has_min, has_max, False, False, False, math,
-           0.0, None, "grad")
+    key = (id(net), batch, x_shape, n_iters, tape_slots, cfg_mode, pn, has_mask, has_min, has_max, False, False,
+           bool(consistency), math, 0.0, None, "grad")
 
     def factory():
-        plan = GradSamplerPlan(device, net, batch, x_shape, len(order), tape_slots, predict_noise=pn, has_mask=has_mask,
-                               has_min=has_min, has_max=has_max, math=math)
+        plan = GradSamplerPlan(device, net, batch, x_shape, n_iters, tape_slots, predict_noise=pn, has_mask=has_mask,
+                               has_min=has_min, has_max=has_max, math=math, consistency=consistency)
         plan.build(1.0)
         return plan
 

@@ -31,6 +31,8 @@
  *                       CDS_OP_LNMOD and CDS_OP_STASH given an upstream gradient compute their own backward (csrc/dit_grad.cuh)
  *   (no new kind)       classifier guidance with MSEClassifier / CumRewClassifier over MLPNNClassifier (mse_classifier.py,
  *                       nn_classifier/mlp.py): CDS_OP_CONV, CDS_OP_STASH and CDS_OP_DGRAD with CDS_ACT_RELU / SILU / MISH
+ *   (kind + mode)       sample(requires_grad=True) with ContinuousConsistencyModel over DQLMlp (consistency_model.py:401-426
+ *                       under autograd): CDS_OP_UPDATE_BWD's kind CM and CDS_OP_PREP's backward mode (gxin != NULL)
  *
  * Conventions
  *  - every function returns 0 on success, a negative cds_status otherwise; cds_last_error() gives the
@@ -57,7 +59,7 @@
 extern "C" {
 #endif
 
-#define CDS_ABI_VERSION 10
+#define CDS_ABI_VERSION 11
 
 typedef enum cds_status {
   CDS_OK = 0,
@@ -215,10 +217,17 @@ typedef struct cds_cast_op {
   int32_t out_dtype;             /* cds_dtype of out */
 } cds_cast_op;
 
-/* consistency model: if row.NOISE: x += K2 * noise[slot];  xin = K3 * x */
+/* consistency model: if row.NOISE: x += K2 * noise[slot];  xin = K3 * x
+ *
+ * Backward mode (gxin != NULL; sample(requires_grad=True) with the consistency model, csrc/grad.cuh): x <- x + K3 * gxin, IEEE
+ * fp32 multiply then add, with x holding d x (the direct part the update's backward wrote) and gxin = d xin (batch, row).  The
+ * re-noise is additive, so its gradient passes through unchanged.  K3 is read from coef + iter*coef_iter_stride (a signed
+ * stride: the backward program walks the forward iterations in reverse); xin and noise are unused.  Forward descriptors keep
+ * gxin NULL, and their row is coef + iter*CDS_ROW_FLOATS whatever coef_iter_stride holds. */
 typedef struct cds_prep_op {
   int32_t batch, row;
   float* x; float* xin; const float* noise; const float* coef;
+  const float* gxin; int64_t coef_iter_stride;      /* backward mode */
 } cds_prep_op;
 
 /* One reverse-process update on x (batch, row) in place; `coef` is the [n_iters][CDS_ROW_FLOATS] table.
@@ -264,13 +273,17 @@ typedef struct cds_stash_op {
   const float* grad;
 } cds_stash_op;
 
-/* Backward of CDS_OP_UPDATE for kinds DDPM, DDIM, EPS and X with a single prediction (no CFG combine, no history):
+/* Backward of CDS_OP_UPDATE for kinds DDPM, DDIM, EPS, X and CM with a single prediction (no CFG combine, no history):
  *   in:  gx = d x_{n+1} (batch, row); the forward's operands x_n and the raw prediction from their stashes
  *   out: gpred = d pred;  gx <- the direct part of d x_n (through the update and clip_prediction's x_t-dependent bounds;
  *        the part through the network is added by the operators that follow)
  * fix_mask: d out = gx * (1 - mask).  clip_prediction follows torch.clip's tensor-bound gradient: an element equal to a bound
  * is not clipped (its gradient goes to pred), a clipped element's gradient goes to the bound, and an eps-prediction bound
- * (x - alpha*x_lim)/sigma passes it to x_t divided by sigma. */
+ * (x - alpha*x_lim)/sigma passes it to x_t divided by sigma.
+ * Kind CM (the consistency model, forward final_clip = 1; x_n is the re-noised x_t that CDS_OP_PREP wrote): f = K0*x + K1*pred
+ * is recomputed with the forward's fp32 ops and clipped to [x_min, x_max] under the same rule (x_min > x_max: no element
+ * passes); g' = the masked gradient where f passes, else 0; gpred = K1*g', gx = K0*g'.  predict_noise is ignored.
+ * The kernel has no backward for kinds X2M, EDM and EDM_HEUN: a row of such a kind makes both outputs NaN. */
 typedef struct cds_update_bwd_op {
   int32_t batch, row;
   float* gx; float* gpred;
