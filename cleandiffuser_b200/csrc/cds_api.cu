@@ -176,6 +176,7 @@ int validate(const cds_op& op, Step* out) {
       if (u.aux && !u.xhat_prev) return fail(CDS_ERR_INVALID, "update: aux history without xhat_prev");
       if (u.x_cast && (u.cast_C_in <= 0 || u.cast_C_out < u.cast_C_in || u.row % u.cast_C_in != 0))
         return fail(CDS_ERR_INVALID, "update: bad x_cast geometry");
+      if (u.guide && !u.guide_s) return fail(CDS_ERR_INVALID, "update: guidance gradient without a scale");
       return CDS_OK;
     }
     case CDS_OP_LNMOD: {
@@ -449,6 +450,8 @@ static_assert(sizeof(cds_attn_op) <= sizeof(cds_conv_op) && sizeof(cds_lnmod_op)
               "backward modes must not grow the cds_op union");
 // ... nor does CDS_OP_PREP's
 static_assert(sizeof(cds_prep_op) <= sizeof(cds_conv_op), "cds_prep_op must not grow the cds_op union");
+// ... nor does CDS_OP_UPDATE's guidance operand (the ABI version was bumped for the update's new layout)
+static_assert(sizeof(cds_update_op) <= sizeof(cds_conv_op), "cds_update_op must not grow the cds_op union");
 
 struct cds_plan {
   int device = 0;

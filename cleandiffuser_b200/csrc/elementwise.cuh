@@ -19,6 +19,7 @@ __device__ __forceinline__ float div_(float a, float b) { return __fdiv_rn(a, b)
 // per-iteration scalars of the update (one row of the coefficient table)
 struct UpdRow {
   float alpha, sigma, k0, k1, k2, k3, k4, xw, dw;
+  float gs;                    // this iteration's guidance scale (0 without a guidance operand)
   int kind;
   const float* noise;          // this iteration's noise slot or NULL
 };
@@ -29,6 +30,7 @@ __device__ __forceinline__ UpdRow load_upd_row(const cds_update_op& p, int iter)
   r.k0 = row[CDS_ROW_K0]; r.k1 = row[CDS_ROW_K1]; r.k2 = row[CDS_ROW_K2]; r.k3 = row[CDS_ROW_K3]; r.k4 = row[CDS_ROW_K4];
   r.xw = row[CDS_ROW_XW]; r.dw = row[CDS_ROW_DW];
   r.kind = (int)row[CDS_ROW_KIND];
+  r.gs = p.guide ? p.guide_s[iter] : 0.f;
   const int slot = (int)row[CDS_ROW_NOISE] - 1;
   const int64_t slot_stride = p.noise_slot_stride > 0 ? p.noise_slot_stride : (int64_t)p.batch * p.row;
   r.noise = slot >= 0 ? p.noise + (int64_t)slot * slot_stride : nullptr;
@@ -37,15 +39,17 @@ __device__ __forceinline__ UpdRow load_upd_row(const cds_update_op& p, int iter)
 
 // One element of the reverse-process update as a pure function of its operands: e = index inside the trajectory, x = x_t,
 // pr = the network prediction (after the CFG combine), z = this iteration's noise draw (ignored without a slot), prior = the
-// conditioning value under the mask, hist = previous x0 estimate of the 2M solvers; *xhat_out receives the new estimate.
+// conditioning value under the mask, hist = previous x0 estimate of the 2M solvers; *xhat_out receives the new estimate;
+// g = the classifier's input gradient (EDM kinds with a guidance operand).
 __device__ __forceinline__ float solver_update_value(const cds_update_op& p, const UpdRow& r, int e, float x, float pr, float z,
                                                      float prior, float hist, float* xhat_out, float aux_in = 0.f,
-                                                     float* aux_out = nullptr) {
+                                                     float* aux_out = nullptr, float g = 0.f) {
   const float alpha = r.alpha, sigma = r.sigma;
   float out;
   if (r.kind == CDS_UPD_EDM || r.kind == CDS_UPD_EDM_HEUN) {
     // D = c_skip*x + c_out*net ; clip ; Euler / Heun step of the probability-flow ODE (newedm.py:142-148, :411-431)
     float d_theta = add_(mul_(r.k0, x), mul_(r.k1, pr));
+    if (p.guide) d_theta = add_(d_theta, mul_(r.gs, g));       // classifier guidance (newedm.py:231), before the clip
     if (p.final_clip) {
       if (p.x_min) d_theta = fmaxf(d_theta, p.x_min[e]);
       if (p.x_max) d_theta = fminf(d_theta, p.x_max[e]);
@@ -105,7 +109,7 @@ __device__ __forceinline__ void solver_update_element(const cds_update_op& p, co
   const bool heun2 = r.kind == CDS_UPD_EDM_HEUN;
   const float out = solver_update_value(p, r, e, p.x[i], pr, r.noise ? r.noise[i] : 0.f, p.mask ? p.prior[i] : 0.f,
                                         (p.xhat_prev && (r.kind == CDS_UPD_X2M || heun2)) ? p.xhat_prev[i] : 0.f, &xhat,
-                                        (p.aux && heun2) ? p.aux[i] : 0.f, &aux);
+                                        (p.aux && heun2) ? p.aux[i] : 0.f, &aux, p.guide ? p.guide[i] : 0.f);
   if (r.kind == CDS_UPD_EDM) {
     if (r.k4 != 0.f && p.xhat_prev && p.aux) { p.xhat_prev[i] = xhat; p.aux[i] = aux; }      // predictor of a Heun step
   } else if (p.xhat_prev && !heun2 && r.kind != CDS_UPD_CM && r.kind != CDS_UPD_DDPM && r.kind != CDS_UPD_DDIM) {
@@ -129,13 +133,14 @@ __device__ __forceinline__ void advance_iteration_when_last(int* advance, int it
 }
 
 // reads x, pred (+pred_uncond, noise, prior, xhat_prev), writes x (+xhat_prev): 12..28 B / element
-// One thread = 4 consecutive elements (float4 traffic on x / pred / noise / prior) when the row length allows it.
+// One thread = 4 consecutive elements (float4 traffic on x / pred / noise / prior) when the row length allows it and there is
+// no guidance operand (guided EDM programs take the scalar path).
 static __global__ void __launch_bounds__(256) solver_update_kernel(const cds_update_op p, const int* iter_ptr, int* advance) {
   const int iter = *iter_ptr;
   const UpdRow r = load_upd_row(p, iter);
   const int64_t total = (int64_t)p.batch * p.row;
   const bool small = total < (int64_t)0x7fffffff;            // 32-bit index arithmetic (64-bit divisions are ~20x dearer)
-  const bool vec4 = small && (p.row % 4 == 0) && !p.pred_uncond && !p.xhat_prev &&
+  const bool vec4 = small && (p.row % 4 == 0) && !p.pred_uncond && !p.xhat_prev && !p.guide &&
                     (((uintptr_t)p.x | (uintptr_t)p.pred | (uintptr_t)p.prior | (uintptr_t)r.noise) % 16 == 0);
   if (vec4) {
     const unsigned n4 = (unsigned)(total / 4);

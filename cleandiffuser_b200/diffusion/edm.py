@@ -8,6 +8,12 @@ whole loop runs on the engine -- every network evaluation is one engine iteratio
 ``CDS_OP_PREP`` (c_in * x) -> denoiser -> ``CDS_OP_UPDATE`` kind ``CDS_UPD_EDM`` / ``CDS_UPD_EDM_HEUN`` (c_skip / c_out
 combine, clip, Euler step or Heun corrector, fix_mask) -- otherwise the PyTorch loop below, the reference algorithm step for
 step.  The EDM teacher of ``ContinuousConsistencyModel.prepare_distillation`` is an instance of this class.
+
+Classifier guidance (newedm.py:217-235, ``D + w_cg * sigma**2 * grad`` at both Heun evaluations) enters the update operator:
+its guidance operand is the classifier's input gradient at the raw x_t, added to D between the combine and the clip.  A
+classifier ``lower.guidable`` accepts has that gradient lowered into the replayed program; any other one runs step by step, a
+host callback writing the gradient into the operand.  Guidance with two-branch CFG, ``requires_grad`` or ``preserve_history``
+keeps the PyTorch loop (``runtime.STATS["guidance_reason"]`` says why).
 """
 from typing import Optional, Union
 
@@ -18,6 +24,17 @@ import torch.nn as nn
 from .basic import DiffusionModel
 from . import solvers as S
 from ..utils import at_least_ndim
+
+
+def _guidance_decline(requires_grad, preserve_history, w_cfg):
+    """why a guided sample() of ContinuousEDM / the legacy DDPM keeps its PyTorch loop, or None"""
+    if requires_grad:
+        return "classifier guidance with requires_grad=True"
+    if preserve_history:
+        return "classifier guidance with preserve_history=True"
+    if w_cfg != 0.0 and w_cfg != 1.0:
+        return "classifier guidance together with two-branch classifier-free guidance"
+    return None
 
 
 def karras_grid(sample_steps: int, sigma_min: float, sigma_top, rho: float, device=None):
@@ -161,10 +178,20 @@ class ContinuousEDM(DiffusionModel):
         done = False
         if requires_grad:
             runtime.grad_fallback(self)
-        if not (requires_grad or preserve_history or guided) and runtime._device_ok(torch.device(self.device)):
+        declined = guided and _guidance_decline(requires_grad, preserve_history, w_cfg)
+        if declined:
+            runtime.guidance_declined(self, declined)
+        if not (requires_grad or preserve_history or declined) and runtime._device_ok(torch.device(self.device)):
+            # every network evaluation is one engine iteration: ``euler`` one per reverse step, ``heun`` a predictor and a
+            # corrector for every step but the last.  ev_sigma: the index into ``sigmas`` of every evaluation.
+            ev_sigma = []
+            for i in order:
+                ev_sigma.append(i)
+                if solver == "heun" and i > 1:
+                    # the corrector evaluates at t = t_i / sigma_i * sigma_{i-1} (newedm.py:421) = sigma_{i-1} exactly (x / x == 1)
+                    ev_sigma.append(i - 1)
+
             def table():
-                # every network evaluation is one engine iteration: ``euler`` one per reverse step, ``heun`` a predictor and a
-                # corrector for every step but the last
                 sig = sigmas.detach().float().cpu()
                 evals = []                      # (sigma of the evaluation, kind, dt, predictor flag)
                 for i in order:
@@ -172,14 +199,29 @@ class ContinuousEDM(DiffusionModel):
                     heun = solver == "heun" and i > 1
                     evals.append((sig[i], S.UPD_EDM, dt, 1.0 if heun else 0.0))
                     if heun:
-                        # the corrector evaluates at t = t_i / sigma_i * sigma_{i-1} (newedm.py:421) = sigma_{i-1} exactly (x / x == 1)
                         evals.append((sig[i - 1], S.UPD_EDM_HEUN, dt, 0.0))
                 return S.edm_table(evals, self.sigma_data)
-            out = runtime.try_sample(self, model=model, xt=xt, prior=prior, solver=solver, sample_steps=sample_steps, order=order,
+            cg = {}
+            if guided:
+                # the reference's expressions on the device (newedm.py:229-233): scale w * sigma ** 2 and classifier time
+                # t.log() / 4 of every evaluation
+                with torch.no_grad():
+                    sig_ev = sigmas[torch.as_tensor(ev_sigma, dtype=torch.long, device=sigmas.device)]
+                    cg = dict(cg_scale=w_cg * (sig_ev ** 2), cg_time=sig_ev.log() / 4.)
+
+                def guide(n, _, x_t, g):
+                    t = torch.full((n_samples,), sigmas[ev_sigma[n]], dtype=torch.float32, device=self.device)
+                    with torch.enable_grad():
+                        _, grad = self.classifier.gradients(x_t.clone(), t.log() / 4., condition_cg)
+                    with torch.no_grad():
+                        g.copy_(grad)
+                cg.update(guide=guide, classifier=self.classifier, w_cg=w_cg, cond_cg=condition_cg)
+            out = runtime.try_sample(self, model=model, xt=xt, prior=prior, solver=solver, sample_steps=sample_steps,
+                                     order=list(range(len(ev_sigma))) if guided else order,
                                      step_values=None, alphas=None, sigmas=None, hs=None, stds=None, cond_emb=cvec, w_cfg=w_cfg,
                                      n_samples=n_samples, predict_noise=False, consistency=True, aux_history=solver == "heun",
                                      table=table, sched_id=(int(sample_steps), float(self.sigma_min), float(top), float(self.rho),
-                                                            float(self.sigma_data)))
+                                                            float(self.sigma_data)), **cg)
             if out is not None:
                 xt, done = out, True
 

@@ -16,6 +16,11 @@ with a_t = alpha_t, ab_t = bar_alpha_t, b_t = beta_t,
 and the prediction is clipped with (alpha, sigma) = (sqrt(ab_t), sqrt(1 - ab_t)) exactly like BaseDiffusionSDE.clip_prediction.
 The reference additionally multiplies the prediction by (1 - fix_mask) (eps) / re-imposes x under the mask (x0) before the
 step; both only touch entries that the final ``x (1 - mask) + prior mask`` overwrites, so the engine skips them.
+
+Classifier guidance (ddpm.py:144-149) is added to the raw prediction before the clip, as in the SDE classes: CDS_OP_GUIDE with
+the per-iteration scale -(w_cg sqrt(1 - ab_t)) (eps) or w_cg (1 - ab_t) / sqrt(ab_t) (x0) when ``lower.guidable`` accepts the
+classifier, else a host callback between the denoiser and the update.  ``log["log_p"]`` is the reference's: the log p of the
+last guided evaluation, at the input of the final iteration.
 """
 import warnings
 from typing import Optional, Union
@@ -26,6 +31,7 @@ import torch.nn as nn
 
 from .basic import DiffusionModel
 from . import solvers as S
+from .edm import _guidance_decline
 from ..utils import at_least_ndim, cosine_beta_schedule, linear_beta_schedule
 
 
@@ -179,14 +185,37 @@ class DDPM(DiffusionModel):
         from ..engine import runtime
         if requires_grad:
             runtime.grad_fallback(self)
-        if not (requires_grad or preserve_history or guided) and runtime._device_ok(torch.device(self.device)):
+        declined = guided and _guidance_decline(requires_grad, preserve_history, w_cfg)
+        if declined:
+            runtime.guidance_declined(self, declined)
+        if not (requires_grad or preserve_history or declined) and runtime._device_ok(torch.device(self.device)):
             rows, slots, t_all = self._engine_table(extra_sample_steps)
+            cg, last = {}, {"log_p": None}
+            if guided:
+                t_dev = t_all.to(self.device)
+                with torch.no_grad():                    # the reference's expressions (ddpm.py:144-149) on the device
+                    ab = self.bar_alpha[t_dev]
+                    scale = -(w_cg * (1 - ab).sqrt()) if self.predict_noise else w_cg * (1 - ab) / ab.sqrt()
+
+                def guide(n, _, x_t, pred):
+                    t_batch = t_dev[n].repeat(n_samples)
+                    with torch.enable_grad():
+                        _, grad = self.classifier.gradients(x_t.clone(), t_batch, condition_cg)
+                    with torch.no_grad():
+                        pred.copy_(pred + scale[n] * grad)
+
+                def last_input(x):
+                    # the reference returns the log p of its last guided evaluation, taken at the final iteration's input
+                    with torch.no_grad():
+                        last["log_p"] = self.classifier.logp(x, t_dev[-1].repeat(n_samples), condition_cg)
+                cg = dict(guide=guide, classifier=self.classifier, w_cg=w_cg, cond_cg=condition_cg, cg_scale=scale,
+                          last_input=last_input)
             out = runtime.try_sample(self, model=model, xt=xt, prior=prior.to(self.device), solver="legacy_ddpm",
                                      sample_steps=sample_steps, order=list(range(rows.shape[0])), step_values=None, alphas=None,
                                      sigmas=None, hs=None, stds=None, cond_emb=cvec, w_cfg=w_cfg, n_samples=n_samples,
-                                     table=(rows, slots, t_all))
+                                     table=(rows, slots, t_all), **cg)
             if out is not None:
-                return out, {**log, "log_p": None}
+                return out, {**log, "log_p": last["log_p"]}
 
         extra = {"log_p": None}
         for t in range(self.diffusion_steps - 1, -1, -1):

@@ -10,7 +10,7 @@ import os
 
 _LIB_PATH = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "csrc", "libcds.so")
 
-ABI_VERSION = 11
+ABI_VERSION = 12
 OPF_BRANCH_SHIFT = 8   # cds_op.flags bits 8..15: branch index (independent chains run on parallel streams)
 OPF_ONCE = 1          # cds_op.flags: run once per plan run (before its first iteration), not in every iteration
 OP_CONV, OP_UPDATE, OP_LNMOD, OP_ATTN, OP_PREP, OP_CAST, OP_MHA = range(7)
@@ -96,6 +96,7 @@ class UpdateOp(C.Structure):
         ("x_max", _f32p),
         ("xhat_prev", _f32p), ("aux", _f32p), ("coef", _f32p), ("predict_noise", C.c_int32), ("final_clip", C.c_int32),
         ("x_cast", C.c_void_p), ("cast_C_in", C.c_int32), ("cast_C_out", C.c_int32), ("x_cast_dtype", C.c_int32),
+        ("guide", _f32p), ("guide_s", _f32p),      # EDM kinds: D += guide_s[iter] * guide (NULL: no guidance term)
     ]
 
 

@@ -134,15 +134,19 @@ class SamplerPlan:
     """Everything resident on the device for one (model, batch, x_shape, option set)."""
 
     def __init__(self, device, net, batch, x_shape, n_iters, n_slots, *, cfg_mode, predict_noise, has_mask,
-                 has_min, has_max, keep_history, math, consistency=False, aux_history=False, classifier=None):
+                 has_min, has_max, keep_history, math, consistency=False, aux_history=False, classifier=None,
+                 guide_operand=False):
         """classifier: a classifier ``lower.guidable`` accepts, whose input gradient at x_t enters the prediction between the
-        denoiser and the update of every iteration (``pred += cg_scale[iter] * grad``).
+        denoiser and the update of every iteration (``pred += cg_scale[iter] * grad``); in a consistency program (ContinuousEDM)
+        the gradient is instead the update's guidance operand, added to the denoised D inside the update.
         consistency: the EDM-preconditioned family (ContinuousConsistencyModel, ContinuousEDM): a CDS_OP_PREP in front of the
         denoiser (re-noise + c_in scaling) and the c_skip / c_out combine in the update; aux_history: second history buffer (the
-        EDM Heun corrector needs the predictor's x_t and slope)."""
+        EDM Heun corrector needs the predictor's x_t and slope).  guide_operand: the update of a consistency program takes a
+        guidance operand even without a lowered classifier -- ``cg_grad``, which a host callback fills every iteration."""
         self._resident(device, net, batch, x_shape, n_iters, n_slots, cfg_mode=cfg_mode, has_mask=has_mask, has_min=has_min,
                        has_max=has_max, keep_history=keep_history, aux_history=aux_history, math=math)
         self.classifier = classifier
+        self._cg_fillers = set()          # ids of the lowered classifier's table fillers (they read the classifier's time column)
         row, root = self.row, self.program
         K = _n_branches(batch, row, consistency)
         self.n_branches = K
@@ -166,13 +170,27 @@ class SamplerPlan:
             pred = lower_denoiser(p, net, xview, x_shape, cfg_mode != 0, sub if cfg_mode == 2 else 0)
             if K == 1:                 # the prediction buffer, for host callbacks between denoiser and update (guidance)
                 self.pred = pred.t if (pred.offset == 0 and pred.lstride == pred.C and pred.bstride == pred.L * pred.C) else None
+            grad = None
             if classifier is not None:
                 assert K == 1 and cfg_mode != 2
-                grad = lower_classifier_grad(p, classifier, _input_view(p, n_before, xview))
+                n_fill = len(p.per_call)
+                # the classifier reads the raw x_t: in a consistency program the denoiser's input is CDS_OP_PREP's c_in x
+                cx = View(self.x, L, Cn, offset=off * row) if consistency else _input_view(p, n_before, xview)
+                grad = lower_classifier_grad(p, classifier, cx)
+                self._cg_fillers = {id(fn) for fn in p.per_call[n_fill:]}
                 self.cg_scale = root.buf(n_iters)           # per-iteration guidance scale, filled by every guided call
-                emit_guide(p, pred, grad, self.cg_scale)
+                if not consistency:
+                    emit_guide(p, pred, grad, self.cg_scale)
+            elif guide_operand:
+                assert K == 1 and consistency
+                self.cg_scale = root.buf(n_iters)
+                self.cg_grad = root.buf(batch, *x_shape)    # written by the host callback of every iteration
+                grad = View(self.cg_grad, L, Cn)
 
             u = self._update_op(p, pred.ptr, sub, fo, predict_noise, consistency)
+            if consistency and grad is not None:            # ContinuousEDM: D += cg_scale[iter] * grad inside the update
+                assert grad.offset == 0 and grad.lstride == grad.C and grad.bstride == grad.L * grad.C and grad.C * grad.L == row
+                u.guide, u.guide_s = grad.ptr, self.cg_scale.data_ptr()
             # tensor-core UNets read x_t through a channel-padded bf16 copy (CDS_OP_CAST).  When that cast converts the very
             # buffer the update writes, the update emits the copy itself and the cast runs only once per sample() call.
             for cop in p.ops[n_before:]:
@@ -277,23 +295,27 @@ class SamplerPlan:
                 h.close()
         self.handle = self.back_handle = None
 
-    def fill_tables(self, t_all, cond_emb, t_key=None, cond_cg=None):
+    def fill_tables(self, t_all, cond_emb, t_key=None, cond_cg=None, cg_t=None):
         """Per-call tables (time-conditioning rows, per-trajectory condition terms of the denoiser and of a lowered
-        classifier), once per ``sample()``."""
+        classifier), once per ``sample()``.  ``cg_t``: the lowered classifier's time per iteration when it is not the
+        denoiser's (ContinuousEDM: log(sigma) / 4 evaluated on the device; those tables are then refilled every call)."""
         # table fillers that depend on (weights, timesteps) only are skipped when neither changed since the last call
         fresh = t_key is None or (t_key, self.version) != getattr(self, "_time_tables_key", None)
         with torch.no_grad():
             for fn, sl in self._fillers:             # every branch fills its own tables from its slice of the condition
-                if fresh or not getattr(fn, "time_only", False):
-                    fn(_Ctx(t_all, _cond_rows(self.cfg_mode, None if cond_emb is None else cond_emb[sl]),
+                own_t = cg_t is not None and id(fn) in self._cg_fillers
+                if fresh or own_t or not getattr(fn, "time_only", False):
+                    fn(_Ctx(cg_t if own_t else t_all, _cond_rows(self.cfg_mode, None if cond_emb is None else cond_emb[sl]),
                             None if cond_cg is None else cond_cg[sl]))
         self._time_tables_key = (t_key, self.version) if t_key is not None else None
 
-    def run_guided(self, t_all, cond_emb, xt, noise_slots, guide, t_key=None):
+    def run_guided(self, t_all, cond_emb, xt, noise_slots, guide, t_key=None, last_input=None):
         """The loop with a host callback between the denoiser and the update of every iteration (classifier guidance,
         diffusionsde.py:153-173): per iteration the denoiser operators are enqueued through the single-step entry
-        (cds_plan_run_range), ``guide(n, x_t, pred)`` edits the prediction in place with ordinary PyTorch ops on the same stream,
-        then the update operator runs.  ``noise_slots[n]`` = 1 + tape slot of iteration n's draw, 0 = none."""
+        (cds_plan_run_range), ``guide(n, x_t, out)`` works with ordinary PyTorch ops on the same stream, then the update operator
+        runs.  ``out`` is the prediction, which the callback edits in place, or, when the update has a guidance operand
+        (ContinuousEDM), that operand, into which the callback writes the classifier's gradient.  ``noise_slots[n]`` = 1 + tape
+        slot of iteration n's draw, 0 = none.  ``last_input(x_t)``: called with the last iteration's input before it runs."""
         assert self.n_branches == 1 and self.pred is not None
         ops = self.program.ops
         upd = max(i for i, op in enumerate(ops) if op.kind == cabi.OP_UPDATE)
@@ -301,24 +323,28 @@ class SamplerPlan:
         self.fill_tables(t_all, cond_emb, t_key)
         stream = torch.cuda.current_stream(self.device).cuda_stream if self.device.type == "cuda" else 0
         x_view = self.x.view(self.batch, *self.x_shape)
-        pred_view = self.pred.view(-1, *self.x_shape)[:self.batch]
+        out_view = self.cg_grad if hasattr(self, "cg_grad") else self.pred.view(-1, *self.x_shape)[:self.batch]
         self.handle.run(0, 0, stream, False)                       # the CDS_OPF_ONCE operators (x_t hand-over cast)
         for n in range(self.n_iters):
             slot = int(noise_slots[n]) - 1
             if slot >= 0:
                 with torch.no_grad():
                     _draw_noise(self.noise[slot], xt)
+            if last_input is not None and n == self.n_iters - 1:
+                last_input(x_view)
             self.handle.run_range(n, 0, upd, stream)
-            guide(n, x_view, pred_view)
+            guide(n, x_view, out_view)
             self.handle.run_range(n, upd, 1, stream)
         STATS["launches"] = (self.handle.launches_per_iter() + 2) * self.n_iters + 1
 
-    def run_chunked(self, t_all, cond_emb, xt, noise_rows, t_key=None, cond_cg=None):
+    def run_chunked(self, t_all, cond_emb, xt, noise_rows, t_key=None, cond_cg=None, cg_t=None, last_input=None):
         """The whole loop, with the noise tape refilled between chunks when it is shorter than the number of draws
         (``noise_rows[n]`` = does iteration n draw?).  The draws are taken in loop order, so a seeded run consumes the
-        generator like the reference loop; everything is enqueued on one stream, so a refill cannot overtake its readers."""
+        generator like the reference loop; everything is enqueued on one stream, so a refill cannot overtake its readers.
+        ``last_input(x_t)``: called with the last iteration's input (the loop is then split before that iteration)."""
         cap = self.noise.shape[0] if self.noise is not None else 0
-        self.fill_tables(t_all, cond_emb, t_key, cond_cg)
+        split = self.n_iters - 1 if last_input is not None else None
+        self.fill_tables(t_all, cond_emb, t_key, cond_cg, cg_t)
         stream = torch.cuda.current_stream(self.device).cuda_stream if self.device.type == "cuda" else 0
         use_graph = os.environ.get("CDS_GRAPH", "1") != "0"
         timed = STATS.get("time_loop") and self.device.type == "cuda"
@@ -329,10 +355,14 @@ class SamplerPlan:
         with torch.no_grad():
             for n in range(self.n_iters + 1):
                 draws = n < self.n_iters and bool(noise_rows[n])
-                if n == self.n_iters or (draws and used == cap):
+                if n == self.n_iters or (draws and used == cap) or n == split:
                     if n > first:
                         self.handle.run(first, n - first, stream, use_graph)
-                    first, used = n, 0
+                    first = n
+                    if n != split or (draws and used == cap):
+                        used = 0
+                    if n == split:
+                        last_input(self.x.view(self.batch, *self.x_shape))
                 if draws:
                     _draw_noise(self.noise[used], xt)
                     used += 1
@@ -503,7 +533,8 @@ def _load_resident(agent, plan, xt, prior, tab: _Table, tape_slots):
 
 def try_sample(agent, *, model, xt, prior, solver, sample_steps, order, step_values, alphas, sigmas, hs, stds,
                cond_emb, w_cfg, n_samples, guide=None, table=None, clip_in_loop=True, predict_noise=None, sched_id=None,
-               classifier=None, w_cg=0.0, cond_cg=None, consistency=False, aux_history=False):
+               classifier=None, w_cg=0.0, cond_cg=None, consistency=False, aux_history=False, cg_scale=None, cg_time=None,
+               last_input=None):
     """One ``sample()`` call of any sampler family on the engine -> x0, or None when the caller's PyTorch loop must run.
 
     ``table``: the coefficient rows for samplers that are "the same update kernel with another coefficient table" (the legacy
@@ -519,7 +550,12 @@ def try_sample(agent, *, model, xt, prior, solver, sample_steps, order, step_val
     accepts (a CumRewClassifier over HalfJannerUNet1d or an out_dim-1 MLPNNClassifier, an MSEClassifier over MLPNNClassifier
     or a QGPOClassifier over QGPONNClassifier with a condition) under
     CDS_MATH = fp32 | tf32 with one sub-batch chain: its input gradient and the guidance term are then operators of the replayed
-    program, and ``guide`` is not called."""
+    program, and ``guide`` is not called.
+    A guided table-driven family gives its own guidance terms: ``cg_scale``, the per-iteration scale on the device (the SDE
+    classes' is derived from ``sigmas`` / ``alphas``); ``cg_time``, the classifier's time per iteration when it is not the
+    table's time column.  In a consistency program (ContinuousEDM) the guidance term enters the update as its guidance
+    operand, and ``guide(n, i, x_t, g)`` writes the classifier's gradient into ``g`` instead of editing the prediction.
+    ``last_input(x_t)``: called with the input of the last iteration before it runs (the legacy DDPM's log p)."""
     def decline(cfg_mode):
         if guide is not None and cfg_mode == 2:
             # the update operator combines the two CFG branches itself; a guidance term would have to enter after that combine
@@ -553,14 +589,17 @@ def try_sample(agent, *, model, xt, prior, solver, sample_steps, order, step_val
         if cg_reason is None and _n_branches(batch, row_elems, False) != 1:
             cg_reason = "more than one sub-batch chain (CDS_BRANCHES)"
     lowered_cg = guide is not None and cg_reason is None
+    operand = guide is not None and consistency and not lowered_cg      # the EDM callback writes the update's guidance operand
     tape_slots = _tape_slots(tab.n_slots, batch, row_elems)
     key = (id(net), batch, x_shape, n_iters, tape_slots, cfg_mode, pn, has_mask, has_min, has_max, keep_history, aux_history,
-           consistency, math, float(w_cfg) if cfg_mode == 2 else 0.0, id(classifier.model_ema) if lowered_cg else None)
+           consistency, math, float(w_cfg) if cfg_mode == 2 else 0.0,
+           id(classifier.model_ema) if lowered_cg else ("operand" if operand else None))
 
     def factory():
         plan = SamplerPlan(device, net, batch, x_shape, n_iters, tape_slots, cfg_mode=cfg_mode, predict_noise=pn,
                            has_mask=has_mask, has_min=has_min, has_max=has_max, keep_history=keep_history, math=math,
-                           consistency=consistency, aux_history=aux_history, classifier=classifier if lowered_cg else None)
+                           consistency=consistency, aux_history=aux_history, classifier=classifier if lowered_cg else None,
+                           guide_operand=operand)
         plan.build(w_cfg)
         return plan
 
@@ -569,12 +608,15 @@ def try_sample(agent, *, model, xt, prior, solver, sample_steps, order, step_val
         return None
     _load_resident(agent, plan, xt, prior, tab, tape_slots)
     STATS["guidance_path"], STATS["guidance_reason"] = None, cg_reason
-    if lowered_cg:
+    if lowered_cg or operand:
         # the guidance scale of every iteration, the reference's own expression (classifier_guidance), evaluated on the device
         with torch.no_grad():
-            idx = torch.as_tensor(order, dtype=torch.long).to(device)
-            sig = sigmas.to(device)[idx]
-            plan.cg_scale.copy_(-(w_cg * sig) if pn else w_cg * ((sig ** 2) / alphas.to(device)[idx]))
+            if cg_scale is None:
+                idx = torch.as_tensor(order, dtype=torch.long).to(device)
+                sig = sigmas.to(device)[idx]
+                cg_scale = -(w_cg * sig) if pn else w_cg * ((sig ** 2) / alphas.to(device)[idx])
+            plan.cg_scale.copy_(cg_scale)
+    if lowered_cg:
         STATS["guidance_path"] = "graph"
         guide = None
     if guide is not None:
@@ -582,11 +624,13 @@ def try_sample(agent, *, model, xt, prior, solver, sample_steps, order, step_val
         if plan.n_branches != 1 or getattr(plan, "pred", None) is None:
             return _fallback("guided sampling needs a single-branch program with a dense prediction buffer")
         slots = plan.coef[:, S.R_NOISE].cpu().tolist()              # tape slot per iteration as the update kernel sees it
-        plan.run_guided(tab.t, cond_emb, xt, slots, lambda n, x, p: guide(n, order[n], x, p), t_key=tab.t_key)
+        plan.run_guided(tab.t, cond_emb, xt, slots, lambda n, x, p: guide(n, order[n], x, p), t_key=tab.t_key,
+                        last_input=last_input)
     else:
         # the loop's draws: same calls, same order, same shapes as the reference loop's (diffusionsde.py:548,571,...)
         plan.run_chunked(tab.t, cond_emb, xt, (tab.rows[:, S.R_NOISE] > 0).tolist(), t_key=tab.t_key,
-                         cond_cg=cond_cg if lowered_cg else None)
+                         cond_cg=cond_cg if lowered_cg else None, cg_t=cg_time if lowered_cg else None,
+                         last_input=last_input)
     STATS["engine_calls"] += 1
     return plan.x.clone()
 
@@ -669,6 +713,14 @@ class _GradSampleFn(torch.autograd.Function):
     @staticmethod
     def backward(ctx, grad_x0):
         return (None, None) + ctx.plan.backward(grad_x0, ctx.generation)
+
+
+def guidance_declined(agent, reason):
+    """A guided ``sample()`` that keeps its PyTorch loop (ContinuousEDM and the legacy DDPM under two-branch CFG,
+    ``requires_grad=True`` or ``preserve_history=True``): recorded in ``STATS["guidance_reason"]`` on a device the engine
+    serves, without counting a fallback."""
+    if _backend() != "torch" and _device_ok(_device_of(agent)):
+        STATS["guidance_path"], STATS["guidance_reason"] = None, reason
 
 
 def grad_fallback(agent):

@@ -33,6 +33,8 @@
  *                       nn_classifier/mlp.py): CDS_OP_CONV, CDS_OP_STASH and CDS_OP_DGRAD with CDS_ACT_RELU / SILU / MISH
  *   (kind + mode)       sample(requires_grad=True) with ContinuousConsistencyModel over DQLMlp (consistency_model.py:401-426
  *                       under autograd): CDS_OP_UPDATE_BWD's kind CM and CDS_OP_PREP's backward mode (gxin != NULL)
+ *   (operand)           classifier guidance with ContinuousEDM (newedm.py:217-235): CDS_OP_UPDATE's guide / guide_s add the
+ *                       term to the denoised D inside the EDM update
  *
  * Conventions
  *  - every function returns 0 on success, a negative cds_status otherwise; cds_last_error() gives the
@@ -59,7 +61,7 @@
 extern "C" {
 #endif
 
-#define CDS_ABI_VERSION 11
+#define CDS_ABI_VERSION 12
 
 typedef enum cds_status {
   CDS_OK = 0,
@@ -252,6 +254,12 @@ typedef struct cds_update_op {
    * written (a CDS_OPF_ONCE cast zeroes them and converts the initial x_t).  NULL = no copy. */
   void* x_cast; int32_t cast_C_in; int32_t cast_C_out;
   int32_t x_cast_dtype;          /* cds_dtype of x_cast */
+  /* optional classifier-guidance term of kinds CDS_UPD_EDM / CDS_UPD_EDM_HEUN (ContinuousEDM, newedm.py:217-235): between the
+   * c_skip / c_out combine and the clip, D <- D + guide_s[iter] * guide(b, e), IEEE fp32 multiply then add (no FMA contraction):
+   * with guide_s = w * sigma^2 of the evaluation this is bit for bit the reference's D + (w * sigma ** 2) * grad.  guide: dense
+   * (batch, row) fp32, the classifier's input gradient at the raw x_t; guide_s: one float per iteration.  NULL = no term (every
+   * unguided program); the other kinds ignore it. */
+  const float* guide; const float* guide_s;
 } cds_update_op;
 
 /* ---- backward operators of a differentiable reverse loop ------------------------------------------------------------
